@@ -2,17 +2,22 @@
 """bench.py -- headline benchmark of the hot path: forward 3-D C2C FFT, GFlops/s = 5 N^3 log2(N^3) / t
 (3dmpifft_opt/fftSpeed3d_c2c.cpp:126-128), per-stage t0..t3 ms, HBM-roofline fraction.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl dfft|reference] [--size 512] [--precision double]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl dfft|reference] [--size 512] [--precision double] [--dump-outputs DIR]
 
 A "step" is one forward transform of the synthetic N^3 cube (BASELINE.json configs[1]: 512^3 double on
 1 GPU; the same cube sharded over N GPUs = strong scaling).  N > 1 runs one process per GPU under
 torchrun; torch.distributed is plumbing only (bootstrap of IPC handles, barrier, max-over-ranks).
 
 `--impl reference` times the reference tree's own CPU FFT on the host cores: heFFTe 2.1.0 with its `stock` backend
-(oracle/_ref/libheffte_ref.so, built from /root/reference/heffte/heffteBenchmark by oracle/ref_heffte/Makefile; slab
+(oracle/_ref/libheffte_ref.so, built from the reference tree's heffte/heffteBenchmark by oracle/ref_heffte/Makefile; slab
 decomposition, p2p_plined reshape like heffteSpeed.sh), one rank per physical core, ranks pinned.  The reference's GPU hot
 path (3dmpifft_opt) needs HIP/hiprtc/rocFFT/MPI and cannot be built here (DESIGN.md).  If the prebuilt library is missing the
 arm falls back to the OpenMP oracle port (oracle/oracle_fft.c) and says so (`kind: "port"`).
+
+`--dump-outputs DIR` writes, after the timed steps, the forward spectrum the last timed step left in the plan's output
+buffer: DIR/spectrum_rank<r>.npy, float64 (float32 for --precision float) pairs of real and imaginary parts.  An output
+larger than 48 MB is sampled at fixed, seeded positions, also written (DIR/spectrum_rank<r>_index.npy, float64); the input
+is seeded too, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -37,8 +42,7 @@ except AttributeError:
 def pin_openmp_threads():
     """CPU legs only: OpenMP threads bound to cores, one per place.  Must run before the OpenMP runtime in question starts (the
     oracle's libgomp), and must NOT be set for the GPU arm's processes: under torchrun every rank's main thread would be bound to
-    the first place -- the same core -- and the ranks' kernel launches would time-share it (measured: 512^3 on 4 GPUs 1.88 ms per
-    step host-bound against 0.87 ms of device time, profiles/r2_final_bench_n4_hostbound.json)."""
+    the first place -- the same core -- and the ranks' kernel launches would time-share it."""
     os.environ.setdefault("OMP_PROC_BIND", "close")
     os.environ.setdefault("OMP_PLACES", "cores")
 
@@ -53,7 +57,7 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (of measured)"
     except Exception:
-        return 6650.0, "B200_PROFILING.md fallback 6.65 TB/s (of fallback)"
+        return 3350.0, "H100 SXM data sheet 3.35 TB/s HBM3 (of fallback)"
 
 
 class ClockSampler:
@@ -216,7 +220,7 @@ def run_reference_arm(args):
     pin_openmp_threads()
     n = args.size
     r = ref_forward_rate(n, args.steps, args.warmup, budget_s=150.0, precision=args.precision)
-    arm = "the reference tree's own CPU FFT: heFFTe 2.1.0 stock backend (oracle/_ref, built from /root/reference/heffte/heffteBenchmark)"
+    arm = "the reference tree's own CPU FFT: heFFTe 2.1.0 stock backend (oracle/_ref, built from the reference tree's heffte/heffteBenchmark)"
     if r is None:
         r = cpu_forward_rate(n, budget_s=20.0, steps=args.steps, warmup=args.warmup)
         r["kind"] = "port"
@@ -292,7 +296,7 @@ def run_dfft_arm(args):
             return out
         comm = dfft.BootstrapComm(rank, P, allgather)
 
-    # synthetic input: U(0,1) real/imag, seeded per rank; inputs (2 GiB at 512^3) are larger than L2 (126 MB)
+    # synthetic input: U(0,1) real/imag, seeded per rank; inputs (2 GiB at 512^3) are larger than L2 (50 MB)
     gen = torch.Generator(device=dev); gen.manual_seed(4242 + rank)
     tin = torch.empty(maxc, dtype=tdt, device=dev)
     torch.view_as_real(tin).uniform_(0.0, 1.0, generator=gen)
@@ -334,6 +338,8 @@ def run_dfft_arm(args):
     stage = [max_over_ranks(x) for x in plan.timings()]
     passes = [max_over_ranks(x) for x in plan.pass_timings()]
     launches = plan.launches * args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, tout[: plan.out_count], rank, P)
 
     # per-pass averages over a few more executes (events bracket each launch on the plan's stream)
     acc = [0.0, 0.0, 0.0]
@@ -417,14 +423,8 @@ def run_dfft_arm(args):
         kernels = [(kn(1, "Z pass (contiguous lines, fft_tma_pass_kernel TMA_Z: TMA ring)", "Z pass (contiguous, fft_tile_kernel MAP_T)"), passes_avg[0], slab_bytes, slab_bytes, kn(1, "z_tma", "z")),
                    (kn(2, "Y pass (strided columns, fft_tma_pass_kernel TMA_Y: 3-D tensor TMA ring, in place)", "Y pass (strided + fused pack, fft_tile_kernel MAP_C)"), passes_avg[1], slab_bytes, slab_bytes, kn(2, "y_tma", "y")),
                    (kn(4, "X pass (strided load + transposed store, fft_tma_pass_kernel TMA_XF)", "X pass (strided load + transposed store, fft_tile_kernel MAP_C->MAP_T)"), passes_avg[2], slab_bytes, slab_bytes, kn(4, "x_tma", "x"))]
-    kname, kms, alg_bytes, conv_bytes, kkey = max(kernels, key=lambda k: k[1])
+    kname, kms, alg_bytes, conv_bytes, _ = max(kernels, key=lambda k: k[1])
     achieved = alg_bytes / (kms * 1e-3) * 1e-9
-    traffic = None
-    try:   # ncu dram__bytes_read.sum + dram__bytes_write.sum per launch, captured under profiles/ (see profiles/traffic.json)
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            traffic = json.load(f).get(f"{n}^3:{args.precision}:P{P}:{kkey}")
-    except Exception:
-        pass
     transform_bytes = (6.0 + (2.0 if P > 1 else 0.0)) * esz * M   # SURVEY 8(d) / BASELINE.md: (6 + 2*[P>1]) * E * M per GPU
     line = {
         "metric": "3D C2C forward FFT GFlops/s (5*N^3*log2(N^3)/t)", "value": value, "unit": "GFlops/s",
@@ -433,7 +433,7 @@ def run_dfft_arm(args):
         "dtype": "f64" if prec == dfft.DOUBLE else "f32", "data": "synthetic",
         "config": {"workload": f"{n}x{n}x{n} C2C {args.precision} forward, slab decomposition over {P} GPU(s)",
                    "exchange": {1: "p2p-fused", 2: "nccl", 3: "staged"}[plan.exchange] if P > 1 else "none",
-                   "l2": "inputs (%.2f GiB per GPU) exceed the 126 MB L2; no flush needed" % (M * esz / 2 ** 30),
+                   "l2": "inputs (%.2f GiB per GPU) exceed the 50 MB L2; no flush needed" % (M * esz / 2 ** 30),
                    "parallelism": f"slab{P}", "pipeline_parts": plan.pipeline_parts,
                    "pipeline": ("kernel-chain" if plan.pipeline_chain else "two-stream") if plan.pipeline_parts else "none", "t0": "overlapped-single-kernel" if plan.overlapped else ("fused-L2" if plan.fused else "two-sweep")},
         "stage_ms": {"t0": stage[0], "t1": stage[1], "t2": stage[2], "t3": stage[3], "total": stage[4]},
@@ -441,7 +441,7 @@ def run_dfft_arm(args):
                     {"forward_single_kernel": passes_avg[0]} if plan.overlapped else {"t0_fused_zy": passes_avg[0], "x": passes_avg[2]} if plan.fused else
                     {"z": passes_avg[0], "y": passes_avg[1], "x": passes_avg[2]}),
         "roofline": {"bound": "hbm", "kernel": kname, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": achieved / peak, "traffic": traffic, "algorithmic_bytes_per_launch": alg_bytes,
+                     "frac": achieved / peak, "algorithmic_bytes_per_launch": alg_bytes,
                      "per_pass_convention_bytes_per_launch": conv_bytes, "kernel_ms": kms,
                      "peak_source": peak_src,
                      "transform": {"achieved": transform_bytes / (ms_per_step * 1e-3) * 1e-9,
@@ -488,10 +488,30 @@ def run_dfft_arm(args):
     return 0
 
 
+DUMP_LIMIT = 48 << 20     # bytes of all ranks' dumps together; larger outputs are sampled
+
+
+def dump_outputs(path, out, rank, P):
+    """out: the plan's output buffer (complex CUDA tensor).  Writes it whole when it fits DUMP_LIMIT / P, else a fixed,
+    seeded sample of its elements together with their indices (8 bytes each) within the same bound."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    vals = torch.view_as_real(out)
+    per = vals.element_size() * 2
+    name = os.path.join(path, f"spectrum_rank{rank}")
+    if out.numel() * per > DUMP_LIMIT // P:
+        gen = torch.Generator(device=out.device); gen.manual_seed(20240 + rank)
+        idx = torch.randint(0, out.numel(), (DUMP_LIMIT // P // (per + 8),), generator=gen, device=out.device).sort().values
+        vals = vals[idx]
+        np.save(name + "_index.npy", idx.double().cpu().numpy())
+    np.save(name + ".npy", vals.cpu().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=100)
+    ap.add_argument("--steps", type=int, default=100, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="dfft", choices=["dfft", "reference"])
     ap.add_argument("--size", type=int, default=512)
@@ -503,7 +523,10 @@ def main():
     ap.add_argument("--overlap", action="store_true", help="EXPERIMENTAL: whole forward transform as one kernel, t3 overlapped behind per-part arrivals (P2P, N > 1)")
     ap.add_argument("--no-pipeline", action="store_true", help="P > 1: disable the stream-pipelined z-part forward path (t2/t3 then run after t0)")
     ap.add_argument("--fuse", action="store_true", help="force the fused L2-resident t0 kernel (default: only with the P2P exchange)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/*.npy (float32/float64, <= 64 MB)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return run_reference_arm(args)
     return run_dfft_arm(args)

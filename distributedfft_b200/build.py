@@ -3,8 +3,8 @@
 
     python -m distributedfft_b200.build [--force] [--tools]
 
-Everything is compiled for sm_100a only:  nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo.
-The resulting .so/.exe are git-ignored but travel to the GPU box with the gpurun snapshot.
+Everything is compiled for sm_90a (H100) only:  nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo.
+The resulting .so and executables are git-ignored build products.
 """
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ BUILD = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libdfft.so")
 DRIVER = os.path.join(HERE, "distFFT")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++"]
 
 LIB_SOURCES = ["dfft_api.cu", "dfft_kernels_common.cu", "dfft_kernels_generic.cu", "dfft_kernels_f64.cu", "dfft_kernels_f32.cu", "dfft_kernels_tma.cu"]

@@ -1,7 +1,7 @@
 // dfft_api.cu -- C-ABI implementation: slab bookkeeping, communicator, plan, stage sequencing.
 //
 // Host-side counterpart of 3dmpifft_opt/include/fft_mpi_3d_api.cpp (plan :41-141, execute :181-214,
-// stages :466-699) re-designed for B200: three batched pass launches per transform instead of two
+// stages :466-699) re-designed for the GPU: three batched pass launches per transform instead of two
 // launches per plane, the pack folded into the Y-pass store, the all-to-all either fused into that
 // store over NVLink peer mappings or handed to NCCL, CUDA events instead of host timers, explicit
 // streams and no device-wide syncs on the production path.
@@ -388,7 +388,7 @@ __global__ void wait_flags_kernel(const unsigned long long* flags, int n, unsign
 // ------------------------------------------------------------------------------------------------
 struct dfft_plan_s {
     Geom g;
-    int P = 1, me = 0, direction = DFFT_FORWARD, prec = 0, device = 0, sms = 148;
+    int P = 1, me = 0, direction = DFFT_FORWARD, prec = 0, device = 0, sms = 132;
     unsigned flags = 0;
     int xmode = DFFT_EXCHANGE_P2P;
     size_t esz = 16;
@@ -658,7 +658,7 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
     {
         // policy: the fused kernel wins when the strided role's stores are NVLink-bound (P2P exchange: the
         // contiguous role then hides entirely under the link time); on one GPU / NCCL the two HBM-bound sweeps
-        // are currently faster (profiles/: SM-side time of both roles adds up), so it is opt-in there.
+        // were faster when measured (SM-side time of both roles adds up), so it is opt-in there.
         const char* env = getenv("DFFT_FUSE");
         const bool can = n1 == n2 && ez->fused[FK_ZY] != nullptr;
         bool want = P > 1 && xmode == DFFT_EXCHANGE_P2P;
@@ -707,14 +707,13 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
     {
         // stream-pipelined forward (z-parts): send side and receive side on two streams, see fwd_pipelined
         const char* env = getenv("DFFT_PIPELINE");
-        // Policy, from the sweeps under profiles/ (r2_sweep_pipeline_{2,4}gpu.log, r2_sweep_kernel_chain*_{2,4}gpu.log):
-        //  * 2 devices: the transform is HBM / L2-fabric bound and already at ~95 % of its (6+2) E M roofline without overlap
-        //    (512^3: 1.38 ms plain, 1.43-1.57 ms in parts): never pipelined by default.
+        // Policy (multi-GPU sweeps; not yet repeated on H100):
+        //  * 2 devices: the transform is HBM / L2-fabric bound and close to its (6+2) E M roofline without overlap, and cutting
+        //    it into parts was slower: never pipelined by default.
         //  * two streams (any exchange): a Y-part kernel and an X-part kernel each want both CTA slots of an SM, so they
-        //    serialise or halve each other; NCCL's kernels compete for the same slots (4 devices, 512^3: 0.86 ms plain, 0.97-1.10 ms
-        //    two-stream, NCCL 1.47 vs 1.50-1.62): opt-in only.
+        //    serialise or halve each other; NCCL's kernels compete for the same slots: opt-in only.
         //  * kernel chain (cubes, P2P): [Z + Y0] [Y1 + X0] ... [X last] with the two roles pinned to the two CTA slots of every SM.
-        //    4 devices: 1024^3 8.79 -> 7.47 ms (-15 %), 512^3 0.87 -> 0.86 ms (a tie), 768^3 fp32 and 256^3 slightly slower.
+        //    It paid off at 4 devices for 1024^3 and tied or lost for smaller cubes.
         //    Default from 4 devices on for axes >= 1024 points, where the X pass that it hides is long enough to pay for the
         //    extra launches and the second read of the intermediate.
         // DFFT_FORCE_PIPELINE / DFFT_PIPELINE=1 pipeline wherever it is possible, DFFT_NO_PIPELINE / DFFT_PIPELINE=0 never.
@@ -1957,7 +1956,7 @@ struct LinePass {
     int src = 0, dst = 0;        // 0 = the caller's data, 1 = the plan's temporary
 };
 struct dfft_lines_plan_s {
-    int prec = 0, device = 0, sms = 148, npass = 0;
+    int prec = 0, device = 0, sms = 132, npass = 0;
     bool ordered = false;        // passes run in the same order for both directions (four-step)
     void* temp = nullptr;
     LinePass pass[2];
@@ -2028,7 +2027,7 @@ extern "C" int dfft_lines_destroy(dfft_lines_plan p)
 //   A: view the line as [n1][n2]; FFT along n1 (stride n2), multiply by W_n^(n2*k1), store transposed -> temp [n2][k1]
 //   B: FFT along n2 (stride n1) of temp, stored to the caller's buffer at [k2][k1] = natural order X[k1 + n1*k2]
 // -- what the reference does with its multi-upload axes and reorderFourStep = 1 (templateFFT.cpp:4007-4106, 5951).
-// Validated against numpy on B200 (tests/test_gpu_parity.py::test_four_step_long_lines, profiles/r2_pytest_gpu_1xB200.log);
+// Validated against numpy (tests/test_gpu_parity.py::test_four_step_long_lines);
 // DFFT_NO_LONG_LINES=1 restores the "unsupported length" answer.
 static int make_four_step(dfft_lines_plan p, int n, long long nlines, int precision, bool dry = false)
 {

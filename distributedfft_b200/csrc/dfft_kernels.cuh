@@ -1,7 +1,7 @@
 // dfft_kernels.cuh -- table of pre-instantiated pass kernels, one entry per (length, precision).
 // The reference compiles one kernel per axis at plan time with hiprtc
 // (templateFFT/src/templateFFT.cpp:5614-5752); here the supported lengths are instantiated ahead
-// of time for sm_100a and looked up at plan time.
+// of time for sm_90a and looked up at plan time.
 #pragma once
 #include <cuda_runtime.h>
 #include <vector>
@@ -61,8 +61,8 @@ struct TmaEntry {
     int rows;              // rows per tensor copy (transform length split into N / rows boxes)
     int nstages, rad[24];  // radix schedule (its twiddle table: build_lut)
     TmaLaunchFn launch;
-    unsigned use;          // bit m set: mode m (TMA_Z, TMA_Y, TMA_XF, TMA_XB) beats the register-staged kernel on B200
-                           // (profiles/r2_sweep_tma_vs_register_1gpu.log); DFFT_TMA=2 uses every mode, DFFT_TMA=0 none
+    unsigned use;          // bit m set: mode m (TMA_Z, TMA_Y, TMA_XF, TMA_XB) beats the register-staged kernel
+                           // (per-pass sweeps, dfft_kernels_tma.cu); DFFT_TMA=2 uses every mode, DFFT_TMA=0 none
 };
 const TmaEntry* find_tma_entry(int N, int prec);   // nullptr: no instantiation, driver too old, or DFFT_TMA=0
 int tma_encode_3d(void* map, void* base, int prec, long long d0, long long d1, long long d2, long long s1, long long s2, int b0, int b1, int b2);

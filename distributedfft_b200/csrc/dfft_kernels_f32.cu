@@ -1,4 +1,4 @@
-// fp32 instantiations.  Per-length choices come from kbench sweeps on B200 (profiles/kbench*.log):
+// fp32 instantiations.  Per-length choices come from kbench sweeps (csrc/tools/kbench.cu):
 // small CTAs (finer barriers) win for the contiguous pass, 128-byte row segments (C = 8 complex
 // doubles) for the strided ones.
 #include "dfft_kernels_inst.cuh"
@@ -14,12 +14,11 @@ void register_f32(std::vector<SizeEntry>& v)
     v.push_back(make_entry<T, Cfg<Sched<128, 16, 16, 8>, 16, false, 4, true>, Cfg<Sched<128, 16, 16, 8>, 16, false, 4, true>>());
     v.push_back(make_entry<T, Cfg<Sched<256, 16, 16, 16>, 8, false, 4, true>, Cfg<Sched<256, 16, 16, 16>, 8, false, 4, true>>());
     v.push_back(make_entry<T, Cfg<Sched<512, 8, 8, 8, 8>, 2, true, 4, true>, Cfg<Sched<512, 16, 8, 8, 8>, 8, false, 2, false>>());
-    // fp32 strided passes want 16 columns (128-byte row segments) and 32 points per thread (sweep1: 12.4 vs 15.4 ms at 1024^3)
+    // fp32 strided passes want 16 columns (128-byte row segments) and 32 points per thread
     v.push_back(make_entry<T, Cfg<Sched<1024, 16, 16, 8, 8>, 2, false, 4, true>, Cfg<Sched<1024, 32, 16, 16, 4>, 16, false, 1, false>>());
     v.push_back(make_entry<T, Cfg<Sched<2048, 16, 16, 16, 8>, 1, false, 4, false>, Cfg<Sched<2048, 16, 16, 16, 8>, 4, false, 1, false>>());
     v.push_back(make_entry<T, Cfg<Sched<4096, 16, 16, 16, 16>, 1, false, 2, false>, Cfg<Sched<4096, 16, 16, 16, 16>, 2, false, 1, false>>());
     // mixed radix
-    // sweep1/2: 5.69 vs 7.69 ms at 768^3 on one GPU, 3.72 vs 4.70 ms on two
     v.push_back(make_entry<T, Cfg<Sched<768, 12, 4, 4, 4, 4, 3>, 2, false, 4, true>, Cfg<Sched<768, 24, 8, 8, 4, 3>, 16, false, 1, false>>());
     v.push_back(make_entry<T, Cfg<Sched<384, 12, 4, 4, 4, 3, 2>, 4, false, 4, true>, Cfg<Sched<384, 12, 4, 4, 4, 3, 2>, 8, false, 2, false>>());
     v.push_back(make_entry<T, Cfg<Sched<192, 12, 4, 4, 4, 3>, 8, false, 4, true>, Cfg<Sched<192, 12, 4, 4, 4, 3>, 8, false, 4, true>>());

@@ -1,4 +1,4 @@
-// fp64 instantiations.  Per-length choices come from kbench sweeps on B200 (profiles/kbench*.log):
+// fp64 instantiations.  Per-length choices come from kbench sweeps (csrc/tools/kbench.cu):
 // small CTAs (finer barriers) win for the contiguous pass, 128-byte row segments (C = 8 complex
 // doubles) for the strided ones.
 #include "dfft_kernels_inst.cuh"
@@ -14,7 +14,7 @@ void register_f64(std::vector<SizeEntry>& v)
     v.push_back(make_entry<T, Cfg<Sched<128, 16, 16, 8>, 16, false, 4, true>, Cfg<Sched<128, 16, 16, 8>, 16, false, 4, true>>());
     v.push_back(make_entry<T, Cfg<Sched<256, 16, 16, 16>, 8, false, 4, true>, Cfg<Sched<256, 16, 16, 16>, 8, false, 4, true>>());
     v.push_back(make_entry<T, Cfg<Sched<512, 8, 8, 8, 8>, 2, true, 4, true>, Cfg<Sched<512, 16, 8, 8, 8>, 8, false, 2, false>>());
-    // 1024 (kbench5): contiguous R=8 with register twiddles 6.66 ms vs 7.73; X pass C=8 8.34 vs 8.58; 128-byte rows for peer stores
+    // 1024: contiguous R=8 with register twiddles; X pass C=8; 128-byte rows for peer stores
     v.push_back(make_entry<T, Cfg<Sched<1024, 8, 8, 8, 8, 2>, 1, true, 4, true>, Cfg<Sched<1024, 16, 16, 8, 8>, 4, false, 2, false>,
                            Cfg<Sched<1024, 16, 16, 8, 8>, 8, false, 1, false>, Cfg<Sched<1024, 16, 16, 8, 8>, 8, false, 1, false>>());
     v.push_back(make_entry<T, Cfg<Sched<2048, 16, 16, 16, 8>, 1, false, 4, false>, Cfg<Sched<2048, 16, 16, 16, 8>, 4, false, 1, false>>());
@@ -23,7 +23,7 @@ void register_f64(std::vector<SizeEntry>& v)
                           // at run time with DFFT_VARIANT=n; the default library ships only configurations that passed parity on hardware
     // experiments for the fused t0 kernel (DFFT_VARIANT=1|2, not used by default): the strided role reads its tile from L2,
     // not HBM, so narrow tiles (64- / 32-byte rows) cost no DRAM efficiency there and allow 3-5 smaller CTAs per SM
-    // (finer-grained phases; the fused kernel's top stall is the CTA barrier, profiles/r1_ncu_full_fused_t0_512.txt)
+    // (finer-grained phases; the fused kernel's top stall is the CTA barrier)
     v.push_back(make_entry<T, Cfg<Sched<512, 8, 8, 8, 8>, 2, true, 4, true>, Cfg<Sched<512, 8, 8, 8, 8>, 4, false, 3, false>>(1));
     v.push_back(make_entry<T, Cfg<Sched<512, 8, 8, 8, 8>, 2, true, 4, true>, Cfg<Sched<512, 8, 8, 8, 8>, 2, false, 5, false>>(2));
     // DFFT_VARIANT=3|4: the default / the 3-CTA shapes with L2 eviction hints in the fused kernels (streamed data evict_first,
@@ -42,7 +42,7 @@ void register_f64(std::vector<SizeEntry>& v)
     // DFFT_VARIANT=5: 256-byte rows for the peer (NVLink) stores only; local passes keep the default shapes
     v.push_back(make_entry<T, Cfg<Sched<512, 8, 8, 8, 8>, 2, true, 4, true>, Y512d, Y512d, Cfg<Sched<512, 16, 8, 8, 8>, 16, false, 1, false>>(5));
     // mixed radix
-    // 768 (kbench5): 24 points/thread (8.8.4.3, three exchanges instead of four): Z 2.83 vs 3.45 ms, Y 3.87 vs 4.28, X 3.52 vs 4.19
+    // 768: 24 points/thread (8.8.4.3, three exchanges instead of four)
     v.push_back(make_entry<T, Cfg<Sched<768, 24, 8, 8, 4, 3>, 4, false, 2, false>, Cfg<Sched<768, 24, 8, 8, 4, 3>, 4, false, 2, false>>());
     v.push_back(make_entry<T, Cfg<Sched<384, 12, 4, 4, 4, 3, 2>, 4, false, 4, true>, Cfg<Sched<384, 12, 4, 4, 4, 3, 2>, 8, false, 2, false>>());
     v.push_back(make_entry<T, Cfg<Sched<192, 12, 4, 4, 4, 3>, 8, false, 4, true>, Cfg<Sched<192, 12, 4, 4, 4, 3>, 8, false, 4, true>>());

@@ -92,15 +92,16 @@ static std::vector<TmaEntry>& tma_table()
     static std::once_flag once;
     std::call_once(once, [] {
         // tile = C lines of N points = 64 KB (48 KB for 768), S::T * C threads, one CTA per SM
-        // which modes to use (measured per pass at N^3 on one B200, TMA vs register-staged ms):
-        constexpr unsigned Z = 1u << TMA_Z, Y = 1u << TMA_Y, X = (1u << TMA_XF) | (1u << TMA_XB);
-        t.push_back(make_tma_entry<Sched<512, 8, 8, 8, 8>, double, 8>(Y));               // Z .741/.697  Y .756/.781  X .781/.775
-        t.push_back(make_tma_entry<Sched<1024, 8, 8, 8, 8, 2>, double, 4>(Y | X));       // Z 7.21/6.73  Y 7.59/9.23  X 8.30/8.49
-        t.push_back(make_tma_entry<Sched<256, 8, 8, 8, 4>, double, 16>(Z | Y | X));      // Z .100/.120  Y .099/.113  X .103/.114
-        t.push_back(make_tma_entry<Sched<768, 12, 4, 4, 4, 4, 3>, double, 4>(Y));        // Z 3.57/2.83  Y 3.56/3.87  X 3.79/3.53
-        t.push_back(make_tma_entry<Sched<512, 16, 8, 8, 8>, float, 16>(Z | Y | X));      // Z .392/.454  Y .370/.523  X .380/.542
-        t.push_back(make_tma_entry<Sched<1024, 16, 16, 8, 8>, float, 8>(Y | X));         // Z 3.48/2.99  Y 3.23/5.10  X 3.95/4.39
-        t.push_back(make_tma_entry<Sched<768, 12, 4, 4, 4, 4, 3>, float, 8>(Y | X));     // Z 1.87/1.74  Y 1.78/1.92  X 1.90/2.01
+        // which modes to use: per pass, whichever of the TMA and the register-staged kernel was faster at N^3 on one GPU
+        // (chosen on an earlier GPU generation; 512 fp64 re-checked on H100, DESIGN.md section 7)
+        constexpr unsigned Z = 1u << TMA_Z, Y = 1u << TMA_Y, XF = 1u << TMA_XF, X = XF | (1u << TMA_XB);
+        t.push_back(make_tma_entry<Sched<512, 8, 8, 8, 8>, double, 8>(Y | XF));            // H100: forward X faster, Z a tie; X backward not measured
+        t.push_back(make_tma_entry<Sched<1024, 8, 8, 8, 8, 2>, double, 4>(Y | X));
+        t.push_back(make_tma_entry<Sched<256, 8, 8, 8, 4>, double, 16>(Z | Y | X));
+        t.push_back(make_tma_entry<Sched<768, 12, 4, 4, 4, 4, 3>, double, 4>(Y));
+        t.push_back(make_tma_entry<Sched<512, 16, 8, 8, 8>, float, 16>(Z | Y | X));
+        t.push_back(make_tma_entry<Sched<1024, 16, 16, 8, 8>, float, 8>(Y | X));
+        t.push_back(make_tma_entry<Sched<768, 12, 4, 4, 4, 4, 3>, float, 8>(Y | X));
     });
     return t;
 }

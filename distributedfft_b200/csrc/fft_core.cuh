@@ -1,6 +1,6 @@
 // fft_core.cuh -- in-register Stockham radix butterflies and the stage/exchange machinery shared
 // by the three pass kernels (Z contiguous, Y strided + fused pack, X strided + fused unpack and
-// transposed store).  Hand-written for sm_100a; no library FFT anywhere on this path.
+// transposed store).  Hand-written for sm_90a; no library FFT anywhere on this path.
 //
 // What this replaces in the reference: the hiprtc-generated `FFT_main` kernels of templateFFT
 // (templateFFT/src/templateFFT.cpp:4699-4996 shaderGenFFT; radix butterflies :315-1075

@@ -424,7 +424,7 @@ __global__ void __launch_bounds__(S::T* C, MINB) fft_tile_kernel(const TileArgs<
 // Two dependent passes over the same planes in ONE persistent kernel (t0 = Z then Y forward, Y then Z
 // backward): the reference runs them as two launches per plane (fft_mpi_3d_api.cpp:496-502), we ran
 // them as two full HBM sweeps; here a plane's intermediate is produced and consumed while it is still
-// resident in the 126 MB L2, so t0 costs one HBM read + one HBM write of the slab.
+// resident in L2 (50 MB on H100), so t0 costs one HBM read + one HBM write of the slab.
 //
 // Work is handed out by a global ticket counter in an order that interleaves "role A on plane
 // x + lag" with "role B on plane x".  A role-B tile waits on its plane's completion counter

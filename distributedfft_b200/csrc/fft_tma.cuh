@@ -1,4 +1,4 @@
-// fft_tma.cuh -- TMA-pipelined pass kernels (sm_100a): the same axis passes as fft_tile_kernel, with the data movement
+// fft_tma.cuh -- TMA-pipelined pass kernels (sm_90a): the same axis passes as fft_tile_kernel, with the data movement
 // handed to the Tensor Memory Accelerator.
 //
 // One CTA per SM owns a 3-slot shared-memory ring of tiles (C lines x N points, <= 72 KB).  A tile is fetched by TMA
@@ -6,8 +6,7 @@
 // slot by S::T * C threads (the Stockham exchanges go through the slot itself: XOR-swizzled inside a line for the
 // line-major thread map, row-interleaved for the column-major one), and written back by a TMA store.  While tile i is
 // being transformed, tile i+1 is landing and tile i-1 is draining, so global-memory latency never sits on the compute
-// threads and no registers are spent on staging.  Measured on B200 at 512^3 fp64 (profiles/r2_tma_prototype_512_1gpu.log):
-// Z 0.674 / Y 0.697 / X 0.741 ms against 0.696 / 0.784 / 0.775 ms for the register-staged kernels.
+// threads and no registers are spent on staging.  Which passes use it is chosen per length (dfft_kernels_tma.cu).
 //
 // What it replaces in the reference: the same generated FFT_main kernels as fft_tile_kernel (templateFFT.cpp:4699-4996);
 // X modes also fold the 201 / 120 transposes (fast_transpose/kernels_201.cpp:46-57, kernels_120.cpp:45-57) into the tile.

@@ -56,7 +56,7 @@ struct Result { std::string name; float ms; double gbs; double err; int regs; si
 static std::vector<Result> results;
 static double2 *d_a, *d_b; static double* d_err;
 static int NX = 512, NY = 512, NZ = 512;   // cube edge = transform length of the variant set being run
-static int g_sms = 148;
+static int g_sms = 132;
 static int g_only = -1, g_idx = 0;
 
 template <class S, int C, int MAPIN, int MAPOUT, bool TWREG, bool PREFETCH, int MINB, bool PP = true>

@@ -1,4 +1,4 @@
-// p2p_bw.cu -- developer micro-benchmark (not part of the product path): how fast can one B200 WRITE into a peer's
+// p2p_bw.cu -- developer micro-benchmark (not part of the product path): how fast can one GPU WRITE into a peer's
 // memory over NVLink, as a function of the store mechanism and of the contiguous run per row?  Answers which store
 // shape the exchange-fused Y role should use.   usage: p2p_bw [MiB]   (needs 2 GPUs with peer access)
 #include <cuda.h>

@@ -1,5 +1,5 @@
 /*
- * dfft.h -- C ABI of the B200-native slab-decomposed 3-D complex-to-complex FFT (libdfft.so).
+ * dfft.h -- C ABI of the H100-native slab-decomposed 3-D complex-to-complex FFT (libdfft.so).
  *
  * This is the drop-in boundary for the hot path of lueelu/DistributedFFT's `3dmpifft_opt`:
  * every entry point below names the reference interface it replaces (paths relative to the

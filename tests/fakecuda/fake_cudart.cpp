@@ -54,7 +54,7 @@ cudaError_t cudaLaunchKernel(const void*, dim3_ grid, dim3_ block, void**, size_
 cudaError_t cudaGetDeviceCount(int* n) { const char* e = getenv("FAKECUDA_DEVICES"); *n = e ? atoi(e) : 8; return 0; }
 cudaError_t cudaGetDevice(int* d) { *d = t_device; return 0; }
 cudaError_t cudaSetDevice(int d) { t_device = d; return 0; }
-cudaError_t cudaDeviceGetAttribute(int* v, int, int) { *v = 148; return 0; }
+cudaError_t cudaDeviceGetAttribute(int* v, int, int) { *v = 132; return 0; }
 cudaError_t cudaDeviceSynchronize(void) { return 0; }
 cudaError_t cudaDeviceCanAccessPeer(int* can, int, int) { *can = 1; return 0; }
 cudaError_t cudaDeviceEnablePeerAccess(int, unsigned) { return 0; }

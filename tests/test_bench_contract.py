@@ -18,8 +18,10 @@ def test_reference_arm_json_line():
               "data", "config", "cpu_baseline", "e2e"):
         assert k in d, k
     assert d["impl"] == "reference" and d["unit"] == "GFlops/s" and d["higher_is_better"] is True and d["value"] > 0
-    # "reference" = the reference tree's heFFTe from oracle/_ref (built here, shipped prebuilt); "port" only when that library is absent
-    have_ref = os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libheffte_ref.so")) or os.path.isdir("/root/reference")
+    # "reference" = the reference tree's heFFTe from oracle/_ref; "port" only when that library is absent
+    sys.path.insert(0, ROOT)
+    from oracle import build_ref
+    have_ref = build_ref() is not None
     assert d["cpu_baseline"]["kind"] == ("reference" if have_ref else "port")
     assert d["cpu_baseline"]["cores"] >= 1 and d["cpu_baseline"]["value"] == d["value"]
     assert d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["d2h_bytes_per_step"] == 0 and d["e2e"]["value"] == d["value"]

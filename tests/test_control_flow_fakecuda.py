@@ -30,7 +30,7 @@ def fake_lib():
     newest = max(os.path.getmtime(p) for p in objs + [stub_src])
     if not os.path.exists(FAKE_LIB) or os.path.getmtime(FAKE_LIB) < newest:
         subprocess.run(["g++", "-O1", "-fPIC", "-std=c++17", "-c", stub_src, "-o", stub_obj], check=True)
-        subprocess.run([NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-cudart", "none", "-o", FAKE_LIB] + objs +
+        subprocess.run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-cudart", "none", "-o", FAKE_LIB] + objs +
                        [stub_obj, "-ldl", "-lpthread", "-ccbin", "/usr/bin/g++"], check=True)
     return FAKE_LIB
 
@@ -210,16 +210,21 @@ def test_driver_stdout_surface_is_the_reference_drivers(fake_lib, tmp_path):
     import re
     sys.path.insert(0, ROOT)
     from oracle import build_ref3d
+    from ref_replay import reference
     ref_exe = os.path.join(ROOT, "oracle", "_ref", "distFFT_ref")
-    if build_ref3d() is None or not os.path.exists(ref_exe):
-        pytest.skip("oracle/_ref/distFFT_ref not built and /root/reference absent")
+
+    class RefDriver:
+        def run(self, args):
+            r = subprocess.run([ref_exe] + args, capture_output=True, text=True, timeout=120)
+            return r.returncode, r.stdout, r.stderr
+    ref = reference(RefDriver, lambda: ref_exe if build_ref3d() is not None and os.path.exists(ref_exe) else None)
     exe = tmp_path / "distFFT_fake"
     subprocess.run(["g++", "-O1", "-std=c++17", "-I", os.path.join(ROOT, "include"), "-I", "/usr/local/cuda/include", DRIVER_SRC, "-o", str(exe),
                     fake_lib, "-Wl,-rpath," + os.path.dirname(fake_lib), "-lpthread"], check=True)
     args = ["16", "16", "16", "1"]
     ours = subprocess.run([str(exe)] + args, capture_output=True, text=True, timeout=60, env=dict(os.environ, FAKECUDA_DEVICES="8"))
-    theirs = subprocess.run([ref_exe] + args, capture_output=True, text=True, timeout=120)
-    assert ours.returncode == 0 and theirs.returncode == 0, ours.stderr + theirs.stderr
+    rc, theirs_stdout, theirs_stderr = ref.run(args)
+    assert ours.returncode == 0 and rc == 0, ours.stderr + theirs_stderr
 
     def shape(text):
         out = []
@@ -230,13 +235,13 @@ def test_driver_stdout_surface_is_the_reference_drivers(fake_lib, tmp_path):
             if line:
                 out.append(line)
         return out
-    a, b = shape(theirs.stdout), shape(ours.stdout)
+    a, b = shape(theirs_stdout), shape(ours.stdout)
     assert "Size: #x#x#" in a and "Max error: #" in a and a.count("t#: #, t#: #, t#: #, t#: #, total: #") == 4
     it = iter(b)
     missing = [line for line in a if line not in it]          # `in` consumes the iterator: an ordered-subsequence check
     assert not missing, (missing, b)
     # the reference's argument check (fftSpeed3d_c2c.cpp:28-31)
-    bad = subprocess.run([ref_exe, "16", "16"], capture_output=True, text=True, timeout=60)
+    bad_rc, bad_stdout, _ = ref.run(["16", "16"])
     ours_bad = subprocess.run([str(exe), "16", "16"], capture_output=True, text=True, timeout=60)
-    assert bad.returncode != 0 and ours_bad.returncode != 0
-    assert [l for l in bad.stdout.splitlines() if "format of arguments" in l] == [l for l in ours_bad.stdout.splitlines() if "format of arguments" in l] != []
+    assert bad_rc != 0 and ours_bad.returncode != 0
+    assert [l for l in bad_stdout.splitlines() if "format of arguments" in l] == [l for l in ours_bad.stdout.splitlines() if "format of arguments" in l] != []

@@ -74,15 +74,18 @@ def test_slab_bookkeeping_random_geometries_match_oracle():
     assert checked > 150
 
 
-def test_fft_mpi_init_device_policy():
-    """getProperDeviceNum (api.cpp:232-272): without a GPU the wanted count is not clamped."""
+def test_fft_mpi_init_device_policy(n_gpus):
+    """getProperDeviceNum (api.cpp:232-272): the wanted count is clamped to the devices present (api.cpp:236-239); without a
+    GPU it is not clamped."""
     for n0, w in ((512, 8), (10, 4), (9, 4), (5, 4), (7, 3)):
         tot, loc, counts = dfft.fft_mpi_init([n0, 64, 4], w)
-        assert tot == loc == proper_device_num(n0, w)
+        assert tot == loc == proper_device_num(n0, min(w, n_gpus) if n_gpus else w)
         g = SlabGeometry(n0, 64, 4, tot)
         assert counts == [g.in_count(p) for p in range(tot)]
-    with pytest.raises(dfft.DfftError):
-        dfft.fft_mpi_init([8, 3, 4], 4)   # N1=3 over 4 devices leaves an empty y-slab
+    P = min(4, n_gpus) if n_gpus else 4
+    if P > 1:                             # (one device never leaves a y-slab empty)
+        with pytest.raises(dfft.DfftError):
+            dfft.fft_mpi_init([8, P - 1, 4], P)   # N1 = P-1 over P devices leaves an empty y-slab
 
 
 def test_plan_rejects_bad_arguments_without_touching_a_gpu():

@@ -2,10 +2,10 @@
 reference tree's own heFFTe 2.1.0 with its `stock` CPU backend (heffte/heffteBenchmark, the library the reference
 benchmarks against), built by oracle/ref_heffte/Makefile into oracle/_ref/libheffte_ref.so.
 
-* committed vectors (tests/golden/heffte_ref_vectors.json, made by tests/golden/make_heffte_ref_vectors.py in the
-  build container) are checked everywhere, also where /root/reference and the .so are absent;
-* when the .so is present (this container, or shipped prebuilt to the GPU box) the comparison is repeated live on
-  random and heFFTe-test inputs, even and uneven slab splits, forward and backward."""
+* committed vectors (tests/golden/heffte_ref_vectors.json, made by tests/golden/make_heffte_ref_vectors.py) are checked
+  everywhere, also where the reference tree and the .so are absent;
+* the comparison is repeated on random and heFFTe-test inputs, even and uneven slab splits, forward and backward: live
+  when the .so is present, else against the library's recorded answers (tests/ref_replay.py)."""
 import json
 import os
 
@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 
 from oracle import BACKWARD, FORWARD, COracle, NumpySlab, SlabGeometry, build_ref, minstd_uniform
+from ref_replay import reference
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -59,10 +60,8 @@ def test_restated_oracles_reproduce_the_reference_librarys_spectra(co, gold):
 
 @pytest.fixture(scope="module")
 def ref():
-    if build_ref() is None:
-        pytest.skip("oracle/_ref/libheffte_ref.so not present and /root/reference not available to build it")
     from oracle import HeffteRef
-    return HeffteRef()
+    return reference(HeffteRef, build_ref)
 
 
 @pytest.mark.parametrize("n0,n1,n2,P,alg", [(8, 16, 4, 1, "alltoallv"), (16, 16, 16, 2, "p2p_plined"), (10, 9, 4, 3, "p2p"), (9, 10, 4, 3, "alltoall"),
@@ -74,13 +73,14 @@ def test_live_reference_library_agrees_with_the_oracle(co, ref, n0, n1, n2, P, a
     S = ref.fft3d(A, P, FORWARD, alg)
     got = _oracle_spectrum(co, A, P)
     assert np.abs(got - S).max() <= 1e-13 * np.log2(A.size) * np.abs(S).max()
-    # backward: the oracle's unnormalised inverse (3dmpifft_opt leaves normalize=0) equals heFFTe's scale::none backward
+    # backward: the oracle's unnormalised inverse (3dmpifft_opt leaves normalize=0) of the spectrum equals heFFTe's scale::none
+    # backward (the oracle's own spectrum is its input: a recorded S holds only a sample of the elements)
     g = SlabGeometry(n0, n1, n2, P)
     ns = NumpySlab(n0, n1, n2, P)
     b1 = []
     for q in range(P):
         b = np.zeros(g.max_count(q), dtype=np.complex128)
-        blk = S[:, q * g.yd: q * g.yd + g.n1l(q), :].transpose(1, 2, 0).reshape(-1)
+        blk = got[:, q * g.yd: q * g.yd + g.n1l(q), :].transpose(1, 2, 0).reshape(-1)
         b[: blk.size] = blk
         b1.append(b)
     b2 = [np.zeros_like(b) for b in b1]

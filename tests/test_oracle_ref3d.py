@@ -3,17 +3,17 @@
 oracle/ref_3dmpifft compiles 3dmpifft_opt/include/fft_mpi_3d_api.cpp (plan creation, TransInfo tables, fftZY,
 localTransposeUneven, slabAlltoall, fftX, fft_mpi_execute_dft_3d_c2c), kernel_func.cpp (the pack / unpack kernels),
 fast_transpose/kernels_{201,120}.cpp (the cuTranspose tile kernels) and the FFT engine templateFFT/src/templateFFT.cpp (the
-kernel generator) from /root/reference, in place, against a HIP-on-CPU shim and runs them on host memory: GPU threads are
+kernel generator) from the reference tree, in place, against a HIP-on-CPU shim and runs them on host memory: GPU threads are
 fibers, and the kernels the engine generates at run time are compiled with g++ in place of hiprtc -- so the butterflies and
 twiddles that run are the reference's too.
 
-* committed vectors (tests/golden/ref3d_vectors.json, made by tests/golden/make_ref3d_vectors.py in the build container):
+* committed vectors (tests/golden/ref3d_vectors.json, made by tests/golden/make_ref3d_vectors.py):
   BOTH plan buffers of every device after EVERY stage, the outputs and the exchange tables -- compared with both
   restatements (oracle_fft.c and the numpy twin) and, for the tables / counts / device policy, with the product library's
   host logic (libdfft.so; no GPU needed for those entry points);
-* live, whenever oracle/_ref/libref3dmpifft.so is present (this container; shipped prebuilt to the GPU box): random inputs
-  over even and uneven splits up to 8 devices, both directions, against numpy's fftn, against the oracle stage by stage, and
-  against the product's recorded multi-device schedule interpreted on the CPU (tests/test_dry_run.py)."""
+* random inputs over even and uneven splits up to 8 devices, both directions, against numpy's fftn, against the oracle stage
+  by stage, and against the product's recorded multi-device schedule interpreted on the CPU (tests/test_dry_run.py): live
+  whenever oracle/_ref/libref3dmpifft.so is present, else against its recorded answers (tests/ref_replay.py)."""
 import json
 import os
 
@@ -22,6 +22,7 @@ import pytest
 
 import distributedfft_b200 as dfft
 from oracle import BACKWARD, FORWARD, COracle, NumpySlab, SlabGeometry, build_ref3d, proper_device_num
+from ref_replay import reference
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 TOL = 2e-13          # absolute, on O(1) inputs of <= 10^4 points: DFT vs Stockham vs pocketfft rounding
@@ -99,7 +100,7 @@ def test_binary_fixture_of_the_gpu_test_matches_the_oracle(co):
     assert np.abs(z["backward"] / z["input"].size - z["input"]).max() <= 1e-13
 
 
-def test_exchange_tables_counts_and_device_policy_match_the_executed_reference(co, gold):
+def test_exchange_tables_counts_and_device_policy_match_the_executed_reference(co, gold, n_gpus):
     """Integers, so exact: the oracle's AND the product library's TransInfo tables (dfft_exchange_table), getMaxDataCount
     (dfft_max_data_count) and the device-count policy (dfft_init) against what the reference's own functions returned."""
     for case in gold["cases"] + gold["table_cases"]:
@@ -116,15 +117,15 @@ def test_exchange_tables_counts_and_device_policy_match_the_executed_reference(c
                 assert dfft.getMaxDataCount(n0, n1, n2, P, last) == case["max_data_count"][int(last)] == co.lib.oracle_max_data_count(n0, n1, n2, P, int(last))
     for row in gold["device_policy"]:
         assert proper_device_num(row["n0"], row["wanted"]) == row["proper"]
-        assert dfft.fft_mpi_init([row["n0"], 64, 4], row["wanted"])[0] == row["proper"]
+        # the library, like the reference (api.cpp:236-239), first clamps the wanted count to the devices present
+        wanted = min(row["wanted"], n_gpus) if n_gpus else row["wanted"]
+        assert dfft.fft_mpi_init([row["n0"], 64, 4], row["wanted"])[0] == (row["proper"] if wanted == row["wanted"] else proper_device_num(row["n0"], wanted))
 
 
 @pytest.fixture(scope="module")
 def ref():
-    if build_ref3d() is None:
-        pytest.skip("oracle/_ref/libref3dmpifft.so not built and /root/reference absent")
     from oracle import Ref3dmpifft
-    return Ref3dmpifft()
+    return reference(Ref3dmpifft, build_ref3d)
 
 
 def _inputs(g, A, direction):
