@@ -104,6 +104,8 @@ def lib():
     L.dfft_length_schedule.argtypes = [i, i, P(ctypes.c_int), i]
     L.dfft_debug_fused3_order.argtypes = [ll, ll, i, i, i, i, i, ll, P(ll)]
     L.dfft_debug_fused3_order.restype = ll
+    L.dfft_debug_fused2_order.argtypes = [ll, i, i, i, ll, P(ll)]
+    L.dfft_debug_fused2_order.restype = ll
     L.dfft_memcpy.argtypes = [vp, vp, ctypes.c_size_t, i]
     L.dfft_debug_timeline.argtypes = [vp, P(ctypes.c_double)]
     _lib = L

@@ -85,6 +85,22 @@ extern "C" long long dfft_debug_fused3_order(long long planes, long long rows, i
     return total;
 }
 
+/* test hook (host only): ticket order of the two-role t0 kernels (fft_fused2_kernel, fft_tma_fused_zy_kernel); out = role
+ * (0 first role, 1 second role), plane, tile; returns the number of tickets (ticket < 0: only that) */
+extern "C" long long dfft_debug_fused2_order(long long planes, int GA, int GB, int lag, long long ticket, long long out[3])
+{
+    FusedCtl F{};
+    F.planes = planes; F.GA = GA; F.GB = GB; F.lag = lag;
+    const Fused2Order o = fused2_prepare(F);
+    const long long total = (long long)o.total;
+    if (ticket < 0 || ticket >= total || !out) return total;
+    bool roleA;
+    unsigned plane, idx;
+    fused2_decode(o, (unsigned)ticket, roleA, plane, idx);
+    out[0] = roleA ? 0 : 1; out[1] = plane; out[2] = idx;
+    return total;
+}
+
 extern "C" int dfft_supported_lengths(int precision, int* lengths, int max_lengths)
 {
     std::vector<int> v;
@@ -420,6 +436,7 @@ struct dfft_plan_s {
     bool timed = false;
     // fused two-pass t0 (L2-resident intermediate): per-plane completion counters + ticket words
     bool fuse = false;
+    bool fuse_tma = false;   // forward, one device: t0 runs on the TMA fused kernel of tz (fft_tma_fused_zy_kernel)
     int lag = 0;
     unsigned long long* plane_done = nullptr;
     unsigned int* ticket = nullptr;
@@ -657,15 +674,19 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
     // the fused kernels pair the contiguous and the strided role of one table entry: square planes only
     {
         // policy: the fused kernel wins when the strided role's stores are NVLink-bound (P2P exchange: the
-        // contiguous role then hides entirely under the link time); on one GPU / NCCL the two HBM-bound sweeps
-        // were faster when measured (SM-side time of both roles adds up), so it is opt-in there.
+        // contiguous role then hides entirely under the link time).  On one device the register-staged fused kernel
+        // loses to the TMA-pipelined sweeps, but the TMA fused kernel (fft_tma_fused_zy_kernel) beats them where it is
+        // instantiated and measured (TmaEntry::use bit TMA_USE_ZY, DESIGN.md 3.4): it is the default forward t0 there.
+        // Forced fusion takes the TMA kernel whenever one exists, the register-staged kernel otherwise.
         const char* env = getenv("DFFT_FUSE");
-        const bool can = n1 == n2 && ez->fused[FK_ZY] != nullptr;
-        bool want = P > 1 && xmode == DFFT_EXCHANGE_P2P;
+        const bool tma_zy = P == 1 && direction == DFFT_FORWARD && n1 == n2 && !dry && p->tz && p->tz->fused_zy != nullptr && n2 % p->tz->C == 0;
+        const bool can = n1 == n2 && (ez->fused[FK_ZY] != nullptr || tma_zy);
+        bool want = (P > 1 && xmode == DFFT_EXCHANGE_P2P) || (tma_zy && (p->tz->use & (1u << TMA_USE_ZY)));
         if (env) want = strcmp(env, "0") != 0;
         if (flags & DFFT_FORCE_FUSE) want = true;
         if (flags & DFFT_NO_FUSE) want = false;
         p->fuse = can && want;
+        p->fuse_tma = p->fuse && tma_zy;
         if (getenv("DFFT_LAG")) p->lag = atoi(getenv("DFFT_LAG"));
         if (p->fuse && !dry) {
             CUP(cudaMalloc((void**)&p->plane_done, (size_t)p->n0l * sizeof(unsigned long long)));
@@ -1023,6 +1044,30 @@ template <typename T> struct Pass {
         ev_record(p, p->pev[1][0]);
         ev_record(p, p->pev[1][1]);
         if (err != cudaSuccess) return fail(DFFT_ECUDA, "fused t0 launch (kind %d, N=%d) failed: %s", kind, e->N, cudaGetErrorString(err));
+        p->launches++;
+        return 0;
+    }
+    // forward t0 of one device in one TMA-pipelined kernel (square planes): Z: src -> mid, Y: mid -> mid in place
+    static int zy_fused_tma(dfft_plan p, const void* src, void* mid)
+    {
+        const Geom& g = p->g;
+        const TmaEntry* e = p->tz;
+        alignas(64) unsigned char mm[128];
+        const int rc = tma_encode_3d(mm, mid, p->prec, g.n2, g.n1, p->n0l, g.n2, g.n1 * g.n2, e->C, e->rows, 1);   // y_pass's map
+        if (rc != 0) return fail(DFFT_ECUDA, "cuTensorMapEncodeTiled failed (%d) for a %lldx%lldx%lld tensor", rc, g.n2, g.n1, p->n0l);
+        TmaFusedArgs<T> a{};
+        a.src = (const cx<T>*)src; a.mid = (cx<T>*)mid; a.lut = (const cx<T>*)p->lut_tz;
+        FusedCtl c{};
+        c.plane_done = p->plane_done; c.ticket = p->ticket; c.planes = p->n0l;
+        c.GA = (int)(g.n1 / e->C); c.GB = (int)(g.n2 / e->C);
+        c.target = ++p->fuse_epoch * (unsigned long long)c.GA;
+        c.lag = p->lag;
+        ev_record(p, p->pev[0][0]);
+        cudaError_t err = e->fused_zy(&a, &c, mm, p->sms, p->stream);
+        ev_record(p, p->pev[0][1]);
+        ev_record(p, p->pev[1][0]);
+        ev_record(p, p->pev[1][1]);
+        if (err != cudaSuccess) return fail(DFFT_ECUDA, "TMA fused t0 launch (N=%d) failed: %s", e->N, cudaGetErrorString(err));
         p->launches++;
         return 0;
     }
@@ -1626,7 +1671,9 @@ template <typename T> static int execute_fused(dfft_plan p)
         // t0 (+t1): Z pass out of place (bufferDev1 survives), Y pass with the pack (and, P2P, the
         // all-to-all) folded into its store
         if (P == 1) {
-            if (p->fuse) {
+            if (p->fuse_tma) {
+                if ((rc = Pass<T>::zy_fused_tma(p, p->buf1, p->work))) return rc;
+            } else if (p->fuse) {
                 if ((rc = Pass<T>::zy_fused(p, p->buf1, p->work, p->work, 0, nullptr, false))) return rc;
             } else {
                 if ((rc = Pass<T>::z_pass(p, p->buf1, p->work, false))) return rc;

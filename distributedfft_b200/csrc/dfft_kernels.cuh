@@ -55,14 +55,19 @@ struct SizeEntry {
 
 // TMA-pipelined pass kernels (fft_tma.cuh), instantiated for the lengths whose C-line tile fills a 64 KB ring slot
 typedef cudaError_t (*TmaLaunchFn)(int mode, const void* tma_args, const void* map_in, const void* map_out, int sm_count, cudaStream_t stream);
+// forward t0 of square planes in one kernel (fft_tma_fused_zy_kernel): args = TmaFusedArgs<T>, map_mid = 3-D map of the intermediate
+typedef cudaError_t (*TmaFusedLaunchFn)(const void* fused_args, const FusedCtl* ctl, const void* map_mid, int sm_count, cudaStream_t stream);
+constexpr int TMA_USE_ZY = 4;   // TmaEntry::use bit of the fused forward t0
 struct TmaEntry {
     int N, prec;
     int C;                 // lines / columns per tile
     int rows;              // rows per tensor copy (transform length split into N / rows boxes)
     int nstages, rad[24];  // radix schedule (its twiddle table: build_lut)
     TmaLaunchFn launch;
+    TmaFusedLaunchFn fused_zy;   // nullptr: no fused forward t0 for this length
     unsigned use;          // bit m set: mode m (TMA_Z, TMA_Y, TMA_XF, TMA_XB) beats the register-staged kernel
-                           // (per-pass sweeps, dfft_kernels_tma.cu); DFFT_TMA=2 uses every mode, DFFT_TMA=0 none
+                           // (per-pass sweeps, dfft_kernels_tma.cu); DFFT_TMA=2 uses every mode, DFFT_TMA=0 none;
+                           // bit TMA_USE_ZY: fused_zy is the default forward t0 of one-device plans
 };
 const TmaEntry* find_tma_entry(int N, int prec);   // nullptr: no instantiation, driver too old, or DFFT_TMA=0
 int tma_encode_3d(void* map, void* base, int prec, long long d0, long long d1, long long d2, long long s1, long long s2, int b0, int b1, int b2);

@@ -72,7 +72,32 @@ static cudaError_t launch_tma(int mode, const void* vargs, const void* map_in, c
     return cudaGetLastError();
 }
 
-template <class S, typename T, int C> static TmaEntry make_tma_entry(unsigned use)
+template <class S, typename T, int C>
+static cudaError_t launch_tma_fused_zy(const void* vargs, const FusedCtl* ctl, const void* map_mid, int sm_count, cudaStream_t st)
+{
+    const TmaFusedArgs<T>& a = *reinterpret_cast<const TmaFusedArgs<T>*>(vargs);
+    using G_ = TmaGeom<S, T, C>;
+    auto kern = fft_tma_fused_zy_kernel<S, T, C>;
+    static bool attr = false;
+    if (!attr) {
+        const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_::SMEM);
+        if (e != cudaSuccess) return e;
+        attr = true;
+    }
+    if (ctl->planes <= 0) return cudaSuccess;
+    const long long total = ctl->planes * ((long long)ctl->GA + ctl->GB);
+    if (total >= (1ll << 31)) return cudaErrorInvalidConfiguration;   // the kernel decodes tickets in 32 bits
+    long long grid = sm_count;
+    if (grid > total) grid = total;
+    FusedCtl c = *ctl;
+    // the Z role runs ahead of the Y role by the tiles the rings hold (TMA_NSLOT per CTA): 4 planes at 512 points on 132 SMs.
+    // One plane more, as fft_fused2_kernel's default adds, measured 0.1 ms slower on H100 (more of the L2 holds intermediate)
+    if (c.lag <= 0) c.lag = (int)((grid * TMA_NSLOT + c.GA + c.GB - 1) / ((long long)c.GA + c.GB));
+    kern<<<(unsigned)grid, G_::NT + 32, G_::SMEM, st>>>(a, c, *reinterpret_cast<const CUtensorMap*>(map_mid));
+    return cudaGetLastError();
+}
+
+template <class S, typename T, int C, bool FUSED_ZY = false> static TmaEntry make_tma_entry(unsigned use)
 {
     TmaEntry e{};
     e.use = use;
@@ -83,6 +108,7 @@ template <class S, typename T, int C> static TmaEntry make_tma_entry(unsigned us
     e.nstages = S::NSTAGES;
     for (int i = 0; i < S::NSTAGES; i++) e.rad[i] = S::rad(i);
     e.launch = launch_tma<S, T, C>;
+    if constexpr (FUSED_ZY) e.fused_zy = launch_tma_fused_zy<S, T, C>;
     return e;
 }
 
@@ -94,8 +120,9 @@ static std::vector<TmaEntry>& tma_table()
         // tile = C lines of N points = 64 KB (48 KB for 768), S::T * C threads, one CTA per SM
         // which modes to use: per pass, whichever of the TMA and the register-staged kernel was faster at N^3 on one GPU
         // (chosen on an earlier GPU generation; 512 fp64 re-checked on H100, DESIGN.md section 7)
-        constexpr unsigned Z = 1u << TMA_Z, Y = 1u << TMA_Y, XF = 1u << TMA_XF, X = XF | (1u << TMA_XB);
-        t.push_back(make_tma_entry<Sched<512, 8, 8, 8, 8>, double, 8>(Y | XF));            // H100: forward X faster, Z a tie; X backward not measured
+        constexpr unsigned Z = 1u << TMA_Z, Y = 1u << TMA_Y, XF = 1u << TMA_XF, X = XF | (1u << TMA_XB), ZY = 1u << TMA_USE_ZY;
+        // H100: forward X faster, Z a tie; X backward not measured; the fused forward t0 beats the Z + Y sweeps (DESIGN.md 3.4)
+        t.push_back(make_tma_entry<Sched<512, 8, 8, 8, 8>, double, 8, true>(Y | XF | ZY));
         t.push_back(make_tma_entry<Sched<1024, 8, 8, 8, 8, 2>, double, 4>(Y | X));
         t.push_back(make_tma_entry<Sched<256, 8, 8, 8, 4>, double, 16>(Z | Y | X));
         t.push_back(make_tma_entry<Sched<768, 12, 4, 4, 4, 4, 3>, double, 4>(Y));

@@ -441,6 +441,39 @@ struct FusedCtl {
     int lag;                          // role A runs this many planes ahead of role B
 };
 
+// Ticket order of the two-role t0 kernels (fft_fused2_kernel, fft_tma_fused_zy_kernel), host-callable so that the CPU tests
+// can check that it is a bijection onto the tiles and that every role-B tile comes after all role-A tiles of its plane:
+//   head : role A on planes [0, lag)
+//   pairs: role A on plane lag + i, then role B on plane i
+//   tail : role B on the last `lag` planes
+// 32-bit arithmetic: a ticket is decoded for every tile, and 64-bit divisions cost several hundred cycles each.
+struct Fused2Order {
+    unsigned GA, GB, per, lag, planes, headT, midT, total;
+};
+__host__ __device__ inline Fused2Order fused2_prepare(const FusedCtl& F)
+{
+    Fused2Order o;
+    o.GA = (unsigned)F.GA; o.GB = (unsigned)F.GB; o.per = o.GA + o.GB;
+    o.planes = (unsigned)F.planes;
+    o.lag = (unsigned)(F.lag < F.planes ? F.lag : F.planes);
+    o.headT = o.lag * o.GA;
+    o.midT = (o.planes - o.lag) * o.per;
+    o.total = o.headT + o.midT + o.lag * o.GB;
+    return o;
+}
+__host__ __device__ inline void fused2_decode(const Fused2Order& o, unsigned t, bool& roleA, unsigned& plane, unsigned& idx)
+{
+    if (t < o.headT) { roleA = true; plane = t / o.GA; idx = t - plane * o.GA; }
+    else if (t < o.headT + o.midT) {
+        const unsigned u = t - o.headT, i = u / o.per, r = u - i * o.per;
+        if (r < o.GA) { roleA = true; plane = o.lag + i; idx = r; }
+        else { roleA = false; plane = i; idx = r - o.GA; }
+    } else {
+        const unsigned u = t - o.headT - o.midT, i = u / o.GB;
+        roleA = false; plane = o.planes - o.lag + i; idx = u - i * o.GB;
+    }
+}
+
 template <class OpA, class OpB, typename T, int MINB>
 __global__ void __launch_bounds__(OpA::NT, MINB) fft_fused2_kernel(const TileArgs<T> A, const TileArgs<T> B, const FusedCtl F)
 {
@@ -457,29 +490,16 @@ __global__ void __launch_bounds__(OpA::NT, MINB) fft_fused2_kernel(const TileArg
     OpB::load_twiddles(kb, twb);
     wait_flags_at_start<T>(B);   // the second role's stores may target buffers a peer is still reading (previous execute)
 
-    // ticket arithmetic in 32 bits (a ticket is decoded for every tile; 64-bit divisions cost several hundred cycles each)
-    const unsigned GA = (unsigned)F.GA, GB = (unsigned)F.GB, per = GA + GB;
-    const unsigned lag = (unsigned)(F.lag < F.planes ? F.lag : F.planes);
-    const unsigned headT = lag * GA;                                   // role A on planes [0, lag)
-    const unsigned midT = ((unsigned)F.planes - lag) * per;           // pairs: A on plane lag+i, then B on plane i
-    const unsigned total = headT + midT + lag * GB;                    // tail: B on the last `lag` planes
+    const Fused2Order o = fused2_prepare(F);
     for (;;) {
         __syncthreads();   // previous tile's smem traffic and s_ticket readers are done
         if (threadIdx.x == 0) s_ticket = (long long)atomicAdd(F.ticket, 1u);
         __syncthreads();
         const unsigned t = (unsigned)s_ticket;
-        if (t >= total) break;
+        if (t >= o.total) break;
         bool roleA;
         unsigned plane, idx;
-        if (t < headT) { roleA = true; plane = t / GA; idx = t - plane * GA; }
-        else if (t < headT + midT) {
-            const unsigned u = t - headT, i = u / per, r = u - i * per;
-            if (r < GA) { roleA = true; plane = lag + i; idx = r; }
-            else { roleA = false; plane = i; idx = r - GA; }
-        } else {
-            const unsigned u = t - headT - midT, i = u / GB;
-            roleA = false; plane = (unsigned)F.planes - lag + i; idx = u - i * GB;
-        }
+        fused2_decode(o, t, roleA, plane, idx);
         if (roleA) {
             OpA::run(A, ka, (long long)plane * F.GA + idx, twa);
             __syncthreads();                       // every thread's stores are issued ...

@@ -20,6 +20,7 @@
 #include <cuda.h>
 
 #include "fft_core.cuh"
+#include "fft_passes.cuh"
 
 namespace dfft {
 
@@ -71,7 +72,15 @@ template <int LAY, int N, int C> __device__ __forceinline__ int tma_idx(int c, i
     else return pos * C + (c ^ (pos & (C - 1)));
 }
 
-template <class S, int s, typename T, int LAY, int C, int NT>
+// CTA-wide barrier of the threads that transform a tile: the whole CTA in the pass kernels; in the fused kernel, whose
+// producer warp has left the loop, the NT consumer threads on named barrier 1
+template <bool CONS, int NT> __device__ __forceinline__ void tma_sync()
+{
+    if constexpr (CONS) asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory");
+    else __syncthreads();
+}
+
+template <class S, int s, typename T, int LAY, int C, int NT, bool CONS = false>
 __device__ __forceinline__ void tma_exchange(cx<T>* v, cx<T>* buf, int t_w, int c_w, int t_r, int c_r)
 {
     constexpr int RAD = S::rad(s), NS = S::ns(s), NB = S::R / RAD;
@@ -83,23 +92,23 @@ __device__ __forceinline__ void tma_exchange(cx<T>* v, cx<T>* buf, int t_w, int 
 #pragma unroll
         for (int m = 0; m < RAD; m++) buf[tma_idx<LAY, S::N, C>(c_w, j0 + m * NS)] = v[i + m * NB];
     }
-    __syncthreads();
+    tma_sync<CONS, NT>();
 #pragma unroll
     for (int u = 0; u < S::R; u++) v[u] = buf[tma_idx<LAY, S::N, C>(c_r, t_r + u * S::T)];
 }
 
-template <class S, int s, typename T, int MODE, int C, int NT> struct TmaStages {
+template <class S, int s, typename T, int MODE, int C, int NT, bool CONS = false> struct TmaStages {
     static constexpr int LAST = S::NSTAGES - 1;
     static __device__ __forceinline__ void run(cx<T>* v, cx<T>* buf, const cx<T>* lut, int t_in, int c_in, int t_out, int c_out)
     {
         stage_compute<S, s, T, false>(v, s == LAST ? t_out : t_in, lut, nullptr);
-        __syncthreads();   // s == 0: every thread has read its inputs; s > 0: all gathers of the previous exchange are done
+        tma_sync<CONS, NT>();   // s == 0: every thread has read its inputs; s > 0: all gathers of the previous exchange are done
         if constexpr (s < LAST) {
             constexpr bool SWITCH = (MODE == TMA_XF || MODE == TMA_XB) && s + 1 == LAST;   // the thread map changes here
             constexpr int LAY = SWITCH ? LAY_COLX : ((MODE == TMA_Z || MODE == TMA_XB) ? LAY_LINES : LAY_COL);
-            if constexpr (SWITCH) tma_exchange<S, s, T, LAY, C, NT>(v, buf, t_in, c_in, t_out, c_out);
-            else tma_exchange<S, s, T, LAY, C, NT>(v, buf, t_in, c_in, t_in, c_in);
-            TmaStages<S, s + 1, T, MODE, C, NT>::run(v, buf, lut, t_in, c_in, t_out, c_out);
+            if constexpr (SWITCH) tma_exchange<S, s, T, LAY, C, NT, CONS>(v, buf, t_in, c_in, t_out, c_out);
+            else tma_exchange<S, s, T, LAY, C, NT, CONS>(v, buf, t_in, c_in, t_in, c_in);
+            TmaStages<S, s + 1, T, MODE, C, NT, CONS>::run(v, buf, lut, t_in, c_in, t_out, c_out);
         }
     }
 };
@@ -199,6 +208,189 @@ __global__ void __launch_bounds__(S::T* C, 1) fft_tma_pass_kernel(const TmaArgs<
         }
     }
     if (tid == 0) tma_wait_all<0>();
+}
+
+// ---- forward t0 in one kernel: the Z pass and the natural Y pass of square planes, intermediate resident in L2 -------------
+// The two-sweep t0 reads and writes the slab twice through DRAM; here a plane's Z output is consumed by its Y tiles while it
+// is still in L2, so t0 costs one DRAM read and one DRAM write of the slab.  Work comes from the ticket order of
+// fft_fused2_kernel (fused2_decode: Z runs `lag` planes ahead of Y) and the same monotonic per-plane counters.
+//   Z role: src -> mid, C contiguous lines per tile, 1-D bulk copies (TMA_Z's tile and thread map)
+//   Y role: mid -> mid in place, C columns per tile, 3-D tensor copies through map_mid (TMA_Y's tile, map and thread map)
+// The CTA is NT consumer threads and one producer warp.  The producer (one lane) draws a ticket only when it owns an empty
+// ring slot, and issues that tile's load at once -- for a Y tile after its plane's counter has reached the target (it may
+// block there).  Consumers transform the slots in order; thread 0 issues the stores and retires a tile (frees its slot,
+// and for a Z tile publishes it on the plane counter) once its store is complete.
+// Deadlock freedom, whatever the residency: a Y ticket waits only for Z tickets of its plane, and all of them are lower.
+// Each of those was drawn by a running producer with an empty slot, so its load is in flight; the tiles ahead of it in
+// that CTA's ring have still lower tickets (tickets rise per CTA), so by induction they complete; and the Z tile itself is
+// retired as soon as its store completes, because thread 0 never blocks on the next slot while a tile is unretired: it
+// polls the next slot and retires the previous tile in the meantime (the next slot may hold exactly the Y tile that waits
+// for it).  Moving the producer into the consumer loop, as in fft_tma_pass_kernel, breaks this: a blocked Y load would
+// then hold back the retirement of the Z tiles in front of it.
+// Proxy order of the hand-over: producer of the Z tile: store's wait_group, fence.proxy.async, __threadfence, counter add;
+// producer of the Y tile: ld.acquire.gpu of the counter, fence.proxy.async, tensor load.
+// L2 policy per instruction (createpolicy): the slab is read once and the finished Y columns are not read again by this
+// kernel, so the Z loads and the Y stores are evict_first; the Z stores of the intermediate are evict_last, so that they
+// survive until their Y tiles read them.  At 512^3 fp64 on H100 the three hints together take t0 from 2.90 to 2.30 ms at
+// lag 4 (DESIGN.md 3.4).  No persisting-L2 carve-out is used: that is a device-wide setting.
+template <typename T> struct TmaFusedArgs {
+    const cx<T>* src;    // Z role input (dense planes of N x N)
+    cx<T>* mid;          // Z role output, Y role input and output (described by map_mid)
+    const cx<T>* lut;
+};
+
+__device__ __forceinline__ uint64_t l2_policy_evict_first()
+{
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_last()
+{
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ void tma_bulk_g2s_hint(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t pol)
+{
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void tma_bulk_s2g_hint(void* dst, const void* src, uint32_t bytes, uint64_t pol)
+{
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(dst), "r"(smem_u32(src)), "r"(bytes), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void tma_tensor_s2g_3d_hint(const CUtensorMap* map, int c0, int c1, int c2, const void* src, uint64_t pol)
+{
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%1, %2, %3}], [%4], %5;"
+                 ::"l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(src)), "l"(pol) : "memory");
+}
+
+__device__ __forceinline__ void tma_mbar_arrive(uint64_t* bar)
+{
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+
+template <class S, typename T, int C>
+__global__ void __launch_bounds__(S::T* C + 32, 1) fft_tma_fused_zy_kernel(const TmaFusedArgs<T> A, const FusedCtl F,
+                                                                            const __grid_constant__ CUtensorMap map_mid)
+{
+    using G_ = TmaGeom<S, T, C>;
+    constexpr int N = S::N, NT = G_::NT, TT = S::T, ROWS = G_::ROWS, NBOX = G_::NBOX;
+    extern __shared__ __align__(128) unsigned char tma_raw[];
+    cx<T>* const lut_s = reinterpret_cast<cx<T>*>(tma_raw + (size_t)TMA_NSLOT * G_::TILE_BYTES);
+    uint64_t* const full = reinterpret_cast<uint64_t*>(tma_raw + (size_t)TMA_NSLOT * G_::TILE_BYTES + G_::LUT_BYTES);
+    uint64_t* const empty = full + TMA_NSLOT;
+    int* const desc = reinterpret_cast<int*>(empty + TMA_NSLOT);   // per slot: role (-1 end, 0 Z, 1 Y), plane, tile
+    static_assert(2 * TMA_NSLOT * sizeof(uint64_t) + 3 * TMA_NSLOT * sizeof(int) <= 128, "ring control words exceed the reserve");
+    auto slot = [&](int i) { return reinterpret_cast<cx<T>*>(tma_raw + (size_t)i * G_::TILE_BYTES); };
+    const int tid = threadIdx.x;
+    if (tid == 0) {
+        for (int i = 0; i < TMA_NSLOT; i++) { mbar_init(full + i, 1); mbar_init(empty + i, 1); }
+        fence_barrier_init();
+    }
+    for (int i = tid; i < S::lut_size(); i += NT + 32) lut_s[i] = A.lut[i];
+    __syncthreads();
+    const Fused2Order o = fused2_prepare(F);
+
+    if (tid >= NT) {
+        // ---- producer: one lane, up to TMA_NSLOT tiles ahead of the consumers ----
+        if (tid == NT) {
+            const uint64_t read_once = l2_policy_evict_first();
+            for (unsigned n = 0;; n++) {
+                const int s = (int)(n % TMA_NSLOT);
+                if (n >= TMA_NSLOT) mbar_wait(empty + s, ((n / TMA_NSLOT) - 1) & 1);   // the slot's previous tile is retired
+                const unsigned t = atomicAdd(F.ticket, 1u);
+                if (t >= o.total) { desc[s * 3] = -1; tma_mbar_arrive(full + s); break; }   // end marker, no bytes
+                bool z;
+                unsigned plane, idx;
+                fused2_decode(o, t, z, plane, idx);
+                desc[s * 3 + 0] = z ? 0 : 1; desc[s * 3 + 1] = (int)plane; desc[s * 3 + 2] = (int)idx;
+                if (!z) {   // every Z tile of the plane is stored
+                    unsigned long long v;
+                    SpinGuard guard;
+                    for (;;) {
+                        asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(F.plane_done + plane) : "memory");
+                        if (v >= F.target) break;
+                        __nanosleep(64);
+                        guard.tick();
+                    }
+                    asm volatile("fence.proxy.async;" ::: "memory");   // the acquired data is read through the async proxy
+                }
+                mbar_expect_tx(full + s, G_::TILE_BYTES);
+                if (z) tma_bulk_g2s_hint(slot(s), A.src + ((long long)plane * o.GA + idx) * (C * N), G_::TILE_BYTES, full + s, read_once);
+                else {
+#pragma unroll
+                    for (int r = 0; r < NBOX; r++) tma_tensor_g2s_3d(slot(s) + r * ROWS * C, &map_mid, (int)idx * C * 2, r * ROWS, (int)plane, full + s);
+                }
+            }
+        }
+        return;
+    }
+
+    // ---- consumers ----
+    int prev_role = -1, prev_slot = 0;
+    unsigned prev_plane = 0;
+    auto retire_prev = [&]() {   // thread 0, the previous tile's store is complete
+        tma_mbar_arrive(empty + prev_slot);
+        if (prev_role == 0) {
+            asm volatile("fence.proxy.async;" ::: "memory");
+            __threadfence();
+            atomicAdd(F.plane_done + prev_plane, 1ull);
+        }
+        prev_role = -1;
+    };
+    for (unsigned n = 0;; n++) {
+        const int s = (int)(n % TMA_NSLOT);
+        const uint32_t ph = (n / TMA_NSLOT) & 1;
+        if (tid == 0) {
+            SpinGuard guard;
+            while (!mbar_try_wait(full + s, ph)) {
+                if (prev_role >= 0) { tma_wait_all<0>(); retire_prev(); }
+                guard.tick();
+            }
+        }
+        mbar_wait(full + s, ph);
+        const int role = desc[s * 3 + 0], plane = desc[s * 3 + 1], idx = desc[s * 3 + 2];
+        if (role < 0) break;
+        cx<T>* buf = slot(s);
+        cx<T> v[S::R];
+        if (role == 0) {
+            const int t = tid % TT, c = tid / TT;
+#pragma unroll
+            for (int u = 0; u < S::R; u++) v[u] = buf[tma_idx<LAY_LINE, N, C>(c, t + u * TT)];
+            TmaStages<S, 0, T, TMA_Z, C, NT, true>::run(v, buf, lut_s, t, c, t, c);
+#pragma unroll
+            for (int u = 0; u < S::R; u++) buf[tma_idx<LAY_LINE, N, C>(c, t + u * TT)] = v[u];
+        } else {
+            const int t = tid / C, c = tid % C;
+#pragma unroll
+            for (int u = 0; u < S::R; u++) v[u] = buf[tma_idx<LAY_COL, N, C>(c, t + u * TT)];
+            TmaStages<S, 0, T, TMA_Y, C, NT, true>::run(v, buf, lut_s, t, c, t, c);
+#pragma unroll
+            for (int u = 0; u < S::R; u++) buf[tma_idx<LAY_COL, N, C>(c, t + u * TT)] = v[u];
+        }
+        tma_fence_smem_writes();
+        tma_sync<true, NT>();
+        if (tid == 0) {
+            // policies made at the point of use: held across the loop they cost thread 0 spill slots
+            if (role == 0) tma_bulk_s2g_hint(A.mid + ((long long)plane * o.GA + idx) * (C * N), buf, G_::TILE_BYTES, l2_policy_evict_last());
+            else {
+                const uint64_t read_once = l2_policy_evict_first();
+#pragma unroll
+                for (int r = 0; r < NBOX; r++) tma_tensor_s2g_3d_hint(&map_mid, idx * C * 2, r * ROWS, plane, buf + r * ROWS * C, read_once);
+            }
+            tma_commit();
+            if (prev_role >= 0) { tma_wait_all<1>(); retire_prev(); }
+            prev_role = role; prev_plane = (unsigned)plane; prev_slot = s;
+        }
+    }
+    if (tid == 0) {
+        tma_wait_all<0>();
+        if (prev_role >= 0) retire_prev();
+        const unsigned left = atomicAdd(F.ticket + 1, 1u);   // the last CTA to leave re-arms the ticket counter
+        if (left == gridDim.x - 1) { F.ticket[0] = 0; F.ticket[1] = 0; __threadfence(); }
+    }
 }
 
 }  // namespace dfft

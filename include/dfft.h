@@ -50,7 +50,9 @@ extern "C" {
 #define DFFT_NO_FUSE 8u          /* t0 as two HBM sweeps (Z pass, Y pass) */
 #define DFFT_FORCE_FUSE 16u      /* t0 as ONE persistent kernel whose Z->Y intermediate stays in L2 (square planes only).
                                     Default: fused when the exchange is P2P (the Y stores are NVLink-bound and hide the
-                                    Z role), two sweeps otherwise */
+                                    Z role), and for one-device forward plans whose axis length has the TMA-pipelined fused
+                                    kernel (512-point fp64); two sweeps otherwise.  Forced fusion of a one-device forward
+                                    plan uses the TMA-pipelined kernel where it exists */
 
 #define DFFT_NATURAL_SPECTRUM 64u /* single device: the spectrum (forward output / backward input) is kept in natural
                                     [x][y][z] order instead of the reference's transposed [y][z][x] (SURVEY 8f rank 1) */
@@ -102,6 +104,9 @@ int dfft_length_schedule(int n, int precision, int* radices, int max_radices);
  * part, plane, tile; returns the number of tickets (ticket < 0: only that) */
 long long dfft_debug_fused3_order(long long planes, long long rows, int GA, int GBk, int GXk, int K, int lag, long long ticket,
                                   long long out[4]);
+/* test hook (host only): ticket order of the two-role t0 kernels (fft_fused2_kernel, fft_tma_fused_zy_kernel); out = role
+ * (0 first role, 1 second role), plane, tile; returns the number of tickets (ticket < 0: only that) */
+long long dfft_debug_fused2_order(long long planes, int GA, int GB, int lag, long long ticket, long long out[3]);
 /* test hook: JSON description of the passes recorded by the last dfft_execute of a DFFT_DRY_RUN plan (affine maps, chunk
  * tables, symbolic buffer addresses: device d, buffer b at ((d+1) << 44) | (b << 40), b = 1 bufferDev1, 2 out, 3 receive/work,
  * 4 intermediate, 5 in).  Returns the number of bytes needed (including the terminator). */
