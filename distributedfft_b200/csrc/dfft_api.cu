@@ -13,6 +13,7 @@
 #include <cmath>
 #include <condition_variable>
 #include <cstdarg>
+#include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -568,6 +569,11 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
     const SizeEntry* ex = find_size_entry((int)n0, precision);
     if (n0 > 1 << 20 || n1 > 1 << 20 || n2 > 1 << 20 || !ez || !ey || !ex)
         return fail(DFFT_EUNSUPPORTED, "unsupported transform length in %lldx%lldx%lld (see dfft_supported_lengths)", n0, n1, n2);
+    // bufferDev2 (`out`, or `in` in place) is written by the pass kernels; an out-of-place `in` is only copied (cudaMemcpy).
+    // TMA needs 16-byte-aligned global addresses, and so do the fp64 kernels' double2 accesses: such a buffer is rejected in
+    // fp64, and in fp32 (float2 accesses, 8 bytes) it keeps the plan on the register-staged kernels
+    const bool buf2_aligned = ((uintptr_t)((!out || out == in) ? in : out) & 15) == 0;
+    if (precision == DFFT_DOUBLE && !buf2_aligned) return fail(DFFT_EINVAL, "a double-precision output buffer must be 16-byte aligned");
 
     dfft_plan p = new dfft_plan_s;
     p->g = g; p->P = P; p->me = dev_idx; p->direction = direction; p->prec = precision; p->flags = flags;
@@ -614,7 +620,7 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
         CUP(upload_lut<float>(&p->lut_x, ex->x_nstages, ex->x_rad));
     }
     if (!dry) CUP(cudaGetLastError());
-    if (!dry && !(flags & DFFT_NO_TMA)) {
+    if (!dry && !(flags & DFFT_NO_TMA) && buf2_aligned) {
         p->tz = find_tma_entry((int)n2, precision);
         p->ty = find_tma_entry((int)n1, precision);
         p->tx = find_tma_entry((int)n0, precision);

@@ -112,11 +112,15 @@ template <class S, typename T, int C, bool FUSED_ZY = false> static TmaEntry mak
     return e;
 }
 
-static std::vector<TmaEntry>& tma_table()
+// per length: the default entry, and its copy with every pass mode switched on (DFFT_TMA=2).  A plan keeps pointers to the
+// entries of its three axes, so both tables are built once and never change
+struct TmaTables { std::vector<TmaEntry> dflt, forced; };
+static const TmaTables& tma_tables()
 {
-    static std::vector<TmaEntry> t;
+    static TmaTables tt;
     static std::once_flag once;
     std::call_once(once, [] {
+        std::vector<TmaEntry>& t = tt.dflt;
         // tile = C lines of N points = 64 KB (48 KB for 768), S::T * C threads, one CTA per SM
         // which modes to use: per pass, whichever of the TMA and the register-staged kernel was faster at N^3 on one GPU
         // (chosen on an earlier GPU generation; 512 fp64 re-checked on H100, DESIGN.md section 7)
@@ -129,8 +133,11 @@ static std::vector<TmaEntry>& tma_table()
         t.push_back(make_tma_entry<Sched<512, 16, 8, 8, 8>, float, 16>(Z | Y | X));
         t.push_back(make_tma_entry<Sched<1024, 16, 16, 8, 8>, float, 8>(Y | X));
         t.push_back(make_tma_entry<Sched<768, 12, 4, 4, 4, 4, 3>, float, 8>(Y | X));
+        // the forced copies keep bit TMA_USE_ZY: the fused forward t0 stays the default where it is one
+        tt.forced = t;
+        for (TmaEntry& e : tt.forced) e.use |= Z | Y | X;
     });
-    return t;
+    return tt;
 }
 
 const TmaEntry* find_tma_entry(int N, int prec)
@@ -139,12 +146,10 @@ const TmaEntry* find_tma_entry(int N, int prec)
     if (env && atoi(env) == 0) return nullptr;
     if (getenv("DFFT_GENERIC") && atoi(getenv("DFFT_GENERIC")) != 0) return nullptr;
     if (!tma_available()) return nullptr;
-    static thread_local TmaEntry forced;
-    for (const TmaEntry& e : tma_table())
-        if (e.N == N && e.prec == prec) {
-            if (env && atoi(env) == 2) { forced = e; forced.use = 0xf; return &forced; }
-            return &e;
-        }
+    const TmaTables& tt = tma_tables();
+    const std::vector<TmaEntry>& t = env && atoi(env) == 2 ? tt.forced : tt.dflt;
+    for (const TmaEntry& e : t)
+        if (e.N == N && e.prec == prec) return &e;
     return nullptr;
 }
 

@@ -74,7 +74,9 @@ extern "C" {
 #define DFFT_NO_TMA 512u          /* use the register-staged pass kernels everywhere.  Default: passes whose load and store are both
                                     local and un-chunked (Z, natural Y, X) run on the TMA-pipelined kernels (fft_tma.cuh: 3-slot
                                     shared-memory ring fed and drained by cp.async.bulk / cp.async.bulk.tensor) for the lengths
-                                    that have an instantiation; env DFFT_TMA=0 has the same effect */
+                                    that have an instantiation; env DFFT_TMA=0 has the same effect.  TMA needs 16-byte-aligned
+                                    addresses: a float plan whose bufferDev2 (`out`, or `in` in place) is only 8-byte aligned
+                                    gets no TMA kernel either (a double plan with such a buffer is rejected, DFFT_EINVAL) */
 
 #define DFFT_EINVAL (-1)
 #define DFFT_ECUDA (-2)

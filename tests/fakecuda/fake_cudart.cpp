@@ -9,6 +9,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
+#include <vector>
 
 extern "C" {
 
@@ -87,6 +89,59 @@ cudaError_t cudaEventDestroy(cudaEvent_t e) { free(e); return 0; }
 cudaError_t cudaEventRecord(cudaEvent_t, cudaStream_t) { g_events++; return 0; }
 cudaError_t cudaEventSynchronize(cudaEvent_t) { return 0; }
 cudaError_t cudaEventElapsedTime(float* ms, cudaEvent_t, cudaEvent_t) { *ms = 0.25f; return 0; }
-cudaError_t cudaGetDriverEntryPoint(const char*, void** fn, unsigned long long, void*) { *fn = nullptr; return 0; }
+// --- tensor maps (FAKECUDA_TMA=1): a stand-in for cuTensorMapEncodeTiled that enforces the driver's documented constraints on
+// the maps the library encodes (rank 3 here, 16-byte-aligned base, strides multiples of 16 bytes, box dims 1..256 and within
+// their dims, inner box row a multiple of 16 bytes) and logs each one.  Without FAKECUDA_TMA there is no driver entry point,
+// as before, and the library runs no TMA kernel.
+struct TmaMapLog { long long ok, dtype, base_mod16, dims[3], strides[2], box[3]; };
+static std::mutex g_tma_mu;
+static std::vector<TmaMapLog> g_tma_log;
+
+static int fake_encode_tiled(void* map, int dtype, unsigned rank, void* base, const unsigned long long* dims, const unsigned long long* strides,
+                             const unsigned* box, const unsigned* estr, int, int, int, int)
+{
+    TmaMapLog l{};
+    l.dtype = dtype;
+    l.base_mod16 = (long long)((uintptr_t)base & 15);
+    const long long esize = dtype == 8 ? 8 : dtype == 7 ? 4 : 0;   // CU_TENSOR_MAP_DATA_TYPE_FLOAT64 / FLOAT32
+    bool ok = rank == 3 && esize != 0 && l.base_mod16 == 0 && map != nullptr;
+    for (unsigned i = 0; i < 3 && i < rank; i++) {
+        l.dims[i] = (long long)dims[i];
+        l.box[i] = box[i];
+        ok = ok && box[i] >= 1 && box[i] <= 256 && box[i] <= dims[i] && estr[i] == 1;
+        if (i < 2) { l.strides[i] = (long long)strides[i]; ok = ok && strides[i] % 16 == 0; }
+    }
+    ok = ok && (box[0] * esize) % 16 == 0;
+    l.ok = ok;
+    if (map) memset(map, 0, 128);
+    std::lock_guard<std::mutex> g(g_tma_mu);
+    g_tma_log.push_back(l);
+    return ok ? 0 : 1;   // CUDA_ERROR_INVALID_VALUE
+}
+// maps encoded since the last reset, 11 values each (ok, dtype, base mod 16, dims[3], strides[2], box[3])
+long long fakecuda_tma_maps(long long* out, long long cap)
+{
+    std::lock_guard<std::mutex> g(g_tma_mu);
+    const long long n = (long long)g_tma_log.size();
+    for (long long i = 0; i < n && (i + 1) * 11 <= cap; i++) {
+        const TmaMapLog& l = g_tma_log[i];
+        const long long v[11] = {l.ok, l.dtype, l.base_mod16, l.dims[0], l.dims[1], l.dims[2], l.strides[0], l.strides[1], l.box[0], l.box[1], l.box[2]};
+        memcpy(out + i * 11, v, sizeof(v));
+    }
+    return n;
+}
+void fakecuda_tma_reset(void) { std::lock_guard<std::mutex> g(g_tma_mu); g_tma_log.clear(); }
+
+cudaError_t cudaGetDriverEntryPoint(const char* name, void** fn, unsigned long long, int* query)
+{
+    const char* e = getenv("FAKECUDA_TMA");
+    if (e && atoi(e) != 0 && name && !strcmp(name, "cuTensorMapEncodeTiled")) {
+        *fn = (void*)fake_encode_tiled;
+        if (query) *query = 0;   // cudaDriverEntryPointSuccess
+        return 0;
+    }
+    *fn = nullptr;
+    return 0;
+}
 cudaError_t cudaGetDriverEntryPointByVersion(const char*, void** fn, unsigned, unsigned long long, void*) { *fn = nullptr; return 0; }
 }
