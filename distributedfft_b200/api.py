@@ -37,6 +37,7 @@ __all__ = [
     "EXCHANGE_NCCL", "EXCHANGE_STAGED", "SCALE_BACKWARD", "NO_FUSE", "FORCE_FUSE", "OVERLAP_X", "NATURAL_SPECTRUM", "DRY_RUN", "NO_PIPELINE", "NO_TMA", "FORCE_PIPELINE", "DfftError", "lib", "LIB_PATH", "Plan", "LocalComm",
     "BootstrapComm", "fft_mpi_init", "fft_mpi_plan_dft_c2c_3d", "fft_mpi_execute_dft_3d_c2c", "fft_mpi_destroy_plan",
     "fft_mpi_alloc_local_memory", "fft_mpi_local_size_3d", "fft_mpi_cleanup", "getMaxDataCount", "supported_lengths",
+    "fft_mpi_plan_dft_r2c_3d", "local_size_r2c_3d",
     "fft_lines", "lines_ops", "LinesPlan", "length_kind", "length_schedule", "memcpy_htod", "memcpy_dtoh", "exchange_table", "comm_allgather",
 ]
 
@@ -77,6 +78,8 @@ def lib():
     L.dfft_comm_allgather.argtypes = [vp, i, vp, vp, ctypes.c_size_t]
     L.dfft_exchange_table.argtypes = [ll, ll, ll, i, i, i, P(ll), P(ll), P(ll), P(ll)]
     L.dfft_plan_c2c_3d.argtypes = [ll, ll, ll, vp, vp, vp, i, i, i, i, u, P(vp)]
+    L.dfft_plan_r2c_3d.argtypes = [ll, ll, ll, vp, vp, vp, i, i, i, i, u, P(vp)]
+    L.dfft_local_size_r2c_3d.argtypes = [ll, ll, ll, i, i, P(ll), P(ll)]
     for name in ("dfft_execute", "dfft_synchronize", "dfft_destroy", "dfft_plan_launches", "dfft_plan_exchange", "dfft_plan_fused", "dfft_plan_pipeline_parts", "dfft_plan_tma_mask", "dfft_plan_pipeline_chain"):
         getattr(L, name).argtypes = [vp]
     L.dfft_execute_stage.argtypes = [vp, i]
@@ -329,6 +332,25 @@ def fft_mpi_plan_dft_c2c_3d(n0, n1, n2, in_ptr, out_ptr, comm, devIdx, totalDevC
     _check(lib().dfft_plan_c2c_3d(n0, n1, n2, in_ptr, out_ptr, ch, devIdx, totalDevCount, direction, precision, flags, ctypes.byref(h)),
            "fft_mpi_plan_dft_c2c_3d")
     return Plan(h)
+
+
+def fft_mpi_plan_dft_r2c_3d(n0, n1, n2, in_ptr, out_ptr, comm, devIdx, totalDevCount, direction, precision=DOUBLE, flags=0):
+    """Real-to-complex (FORWARD) / complex-to-real (BACKWARD) slab transform (dfft_plan_r2c_3d).  FORWARD: `in_ptr` holds the
+    real x-slab [x_l][y][z], `out_ptr` receives the half spectrum [y_l][n2//2+1][x]; BACKWARD is the exact inverse layout,
+    unnormalised unless SCALE_BACKWARD.  Buffer sizes: local_size_r2c_3d; `out_ptr` must be a separate buffer.  Plan.in_count /
+    out_count are in elements of their own type (reals or complex)."""
+    h = ctypes.c_void_p()
+    ch = comm.handle if comm is not None else None
+    _check(lib().dfft_plan_r2c_3d(n0, n1, n2, in_ptr, out_ptr, ch, devIdx, totalDevCount, direction, precision, flags, ctypes.byref(h)),
+           "fft_mpi_plan_dft_r2c_3d")
+    return Plan(h)
+
+
+def local_size_r2c_3d(n0, n1, n2, totalDevCount, devIdx):
+    """(real_count, complex_count) of one device: reals of its x-slab, complex elements of its half-spectrum y-slab"""
+    r, c = ctypes.c_longlong(0), ctypes.c_longlong(0)
+    _check(lib().dfft_local_size_r2c_3d(n0, n1, n2, totalDevCount, devIdx, ctypes.byref(r), ctypes.byref(c)), "dfft_local_size_r2c_3d")
+    return r.value, c.value
 
 
 def fft_mpi_execute_dft_3d_c2c(plan: Plan):

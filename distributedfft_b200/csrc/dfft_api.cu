@@ -465,6 +465,12 @@ struct dfft_plan_s {
     void* sendbuf = nullptr;         // NCCL: part-major packed send buffer
     unsigned long long* dbg = nullptr;   // DFFT_DEBUG_TIMELINE: device-side timeline of the single-kernel forward path
     unsigned int* done_ctr = nullptr; // [DFFT_MAX_PARTS] finished-CTA counters of the part kernels (arrival signal folded into the kernel)
+    // real-data plans (dfft_plan_r2c_3d): g.n2 is the half-spectrum extent nzh = n2r / 2 + 1, which is all the Y, X and exchange
+    // code sees; only the Z pass (fft_real.cuh) and the scale factor use the real length n2r.  in_count / out_count are in
+    // elements of each side's own type (in_esz / out_esz bytes)
+    bool r2c = false;
+    long long n2r = 0;
+    size_t in_esz = 16, out_esz = 16;
 };
 
 // symbolic device address of a describe-only plan: device d (0-based), buffer id b: 1 bufferDev1, 2 bufferDev2 / user out,
@@ -537,7 +543,7 @@ static int share_pointer(dfft_plan p, void* mine, std::vector<void*>& peers)
 }
 
 static int plan_create(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
-                       int P, int direction, int precision, unsigned flags, dfft_plan* plan_out);
+                       int P, int direction, int precision, unsigned flags, dfft_plan* plan_out, bool real = false);
 
 extern "C" int dfft_plan_c2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
                                 int P, int direction, int precision, unsigned flags, dfft_plan* plan_out)
@@ -549,19 +555,42 @@ extern "C" int dfft_plan_c2c_3d(long long n0, long long n1, long long n2, void* 
     return rc;
 }
 
+extern "C" int dfft_plan_r2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
+                                int P, int direction, int precision, unsigned flags, dfft_plan* plan_out)
+{
+    const int rc = plan_create(n0, n1, n2, in, out, comm, dev_idx, P, direction, precision, flags, plan_out, true);
+    if (rc != 0 && P > 1 && comm && comm->local && !(flags & DFFT_DRY_RUN)) comm->poison();
+    return rc;
+}
+
+extern "C" int dfft_local_size_r2c_3d(long long n0, long long n1, long long n2, int P, int dev, long long* real_count, long long* complex_count)
+{
+    if (P < 1 || dev < 0 || dev >= P || n0 < 1 || n1 < 1 || n2 < 1) return fail(DFFT_EINVAL, "dfft_local_size_r2c_3d: bad arguments");
+    Geom g{n0, n1, n2 / 2 + 1, P};
+    if (g.last_n0() < 1 || g.last_n1() < 1) return fail(DFFT_EUNSUPPORTED, "%lldx%lldx%lld cannot be split over %d devices (empty last slab)", n0, n1, n2, P);
+    if (real_count) *real_count = g.n0l(dev) * n1 * n2;
+    if (complex_count) *complex_count = g.out_count(dev);
+    return 0;
+}
+
 static int plan_create(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
-                       int P, int direction, int precision, unsigned flags, dfft_plan* plan_out)
+                       int P, int direction, int precision, unsigned flags, dfft_plan* plan_out, bool real)
 {
     if (!plan_out) return fail(DFFT_EINVAL, "null plan pointer");
     *plan_out = nullptr;
     if (n0 < 1 || n1 < 1 || n2 < 1 || P < 1 || dev_idx < 0 || dev_idx >= P || !in)
-        return fail(DFFT_EINVAL, "dfft_plan_c2c_3d: bad arguments");
+        return fail(DFFT_EINVAL, real ? "dfft_plan_r2c_3d: bad arguments" : "dfft_plan_c2c_3d: bad arguments");
     if (direction != DFFT_FORWARD && direction != DFFT_BACKWARD) return fail(DFFT_EINVAL, "direction must be +1 or -1");
     if (precision != DFFT_DOUBLE && precision != DFFT_FLOAT) return fail(DFFT_EINVAL, "bad precision");
     if (P > DFFT_MAX_CHUNKS) return fail(DFFT_EUNSUPPORTED, "at most %d devices", DFFT_MAX_CHUNKS);
     const bool dry = (flags & DFFT_DRY_RUN) != 0;
+    if (real) {
+        // the real and the complex slab differ in size and layout: no in-place (padded) layout, no stage-by-stage mode
+        if (!out || out == in) return fail(DFFT_EINVAL, "dfft_plan_r2c_3d: `out` must be a separate buffer (in-place R2C is not supported)");
+        if ((flags & DFFT_EXCHANGE_MASK) == DFFT_EXCHANGE_STAGED) return fail(DFFT_EUNSUPPORTED, "R2C / C2R plans do not support DFFT_EXCHANGE_STAGED");
+    }
     if (!dry && P > 1 && (!comm || comm->nranks != P)) return fail(DFFT_EINVAL, "a communicator of %d ranks is required", P);
-    Geom g{n0, n1, n2, P};
+    Geom g{n0, n1, real ? n2 / 2 + 1 : n2, P};   // R2C: everything but the Z pass works on the nzh = n2/2 + 1 half-spectrum columns
     if (g.last_n0() < 1 || g.last_n1() < 1)
         return fail(DFFT_EUNSUPPORTED, "%lldx%lldx%lld cannot be split over %d devices (empty last slab); use dfft_init", n0, n1, n2, P);
     const SizeEntry* ez = find_size_entry((int)n2, precision);
@@ -569,11 +598,17 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
     const SizeEntry* ex = find_size_entry((int)n0, precision);
     if (n0 > 1 << 20 || n1 > 1 << 20 || n2 > 1 << 20 || !ez || !ey || !ex)
         return fail(DFFT_EUNSUPPORTED, "unsupported transform length in %lldx%lldx%lld (see dfft_supported_lengths)", n0, n1, n2);
+    if (real && (ez->gen || !ez->launch[PK_Z_R2C] || !ez->launch[PK_Z_C2R]))
+        return fail(DFFT_EUNSUPPORTED, "R2C / C2R needs a z length with a tuned kernel (dfft_length_kind == 2); %lld has none", n2);
     // bufferDev2 (`out`, or `in` in place) is written by the pass kernels; an out-of-place `in` is only copied (cudaMemcpy).
     // TMA needs 16-byte-aligned global addresses, and so do the fp64 kernels' double2 accesses: such a buffer is rejected in
-    // fp64, and in fp32 (float2 accesses, 8 bytes) it keeps the plan on the register-staged kernels
-    const bool buf2_aligned = ((uintptr_t)((!out || out == in) ? in : out) & 15) == 0;
+    // fp64, and in fp32 (float2 accesses, 8 bytes) it keeps the plan on the register-staged kernels.  R2C plans apply the rule
+    // to their complex-side buffer (forward `out`, backward `in`); the real side only needs the alignment of its element type
+    const void* cbuf = real ? (direction == DFFT_FORWARD ? out : in) : ((!out || out == in) ? in : out);
+    const bool buf2_aligned = ((uintptr_t)cbuf & 15) == 0;
     if (precision == DFFT_DOUBLE && !buf2_aligned) return fail(DFFT_EINVAL, "a double-precision output buffer must be 16-byte aligned");
+    const size_t rsz = precision == DFFT_FLOAT ? 4 : 8;
+    if (real && ((uintptr_t)(direction == DFFT_FORWARD ? in : out) % rsz) != 0) return fail(DFFT_EINVAL, "the real buffer is not aligned to its element size");
 
     dfft_plan p = new dfft_plan_s;
     p->g = g; p->P = P; p->me = dev_idx; p->direction = direction; p->prec = precision; p->flags = flags;
@@ -582,6 +617,14 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
     p->in_count = direction == DFFT_FORWARD ? g.in_count(dev_idx) : g.out_count(dev_idx);
     p->out_count = direction == DFFT_FORWARD ? g.out_count(dev_idx) : g.in_count(dev_idx);
     p->max_count = g.max_count(dev_idx);
+    p->in_esz = p->out_esz = p->esz;
+    if (real) {
+        p->r2c = true;
+        p->n2r = n2;
+        const long long rcount = p->n0l * n1 * n2;
+        if (direction == DFFT_FORWARD) { p->in_count = rcount; p->in_esz = rsz; }
+        else { p->out_count = rcount; p->out_esz = rsz; }
+    }
     p->ez = ez; p->ey = ey; p->ex = ex; p->comm = comm;
     p->in = in; p->out = out;
     p->dry = dry;
@@ -602,8 +645,10 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
     else p->buf2 = out;
     if (dry) p->buf1 = fake_addr(dev_idx, 1);
     else {
-        CUP(cudaMalloc(&p->buf1, (size_t)p->max_count * p->esz));
-        CUP(cudaMemcpy(p->buf1, in, (size_t)p->max_count * p->esz, cudaMemcpyDeviceToDevice));
+        // R2C: bufferDev1 holds exactly the input slab (the user's buffer has only that many elements of its type)
+        const size_t b1 = p->r2c ? (size_t)p->in_count * p->in_esz : (size_t)p->max_count * p->esz;
+        CUP(cudaMalloc(&p->buf1, b1));
+        CUP(cudaMemcpy(p->buf1, in, b1, cudaMemcpyDeviceToDevice));
         CUP(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
         for (auto& e : p->ev) CUP(cudaEventCreate(&e));
         for (auto& pe : p->pev) for (auto& e : pe) CUP(cudaEventCreate(&e));
@@ -621,7 +666,7 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
     }
     if (!dry) CUP(cudaGetLastError());
     if (!dry && !(flags & DFFT_NO_TMA) && buf2_aligned) {
-        p->tz = find_tma_entry((int)n2, precision);
+        p->tz = real ? nullptr : find_tma_entry((int)n2, precision);   // R2C: the Z pass is always the real-data kernel
         p->ty = find_tma_entry((int)n1, precision);
         p->tx = find_tma_entry((int)n0, precision);
         const TmaEntry* te[3] = {p->tz, p->ty, p->tx};
@@ -677,6 +722,7 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
         }
     }
     p->xmode = xmode;
+    if (real && xmode == DFFT_EXCHANGE_STAGED) return bail(fail(DFFT_EUNSUPPORTED, "R2C / C2R plans do not support the staged exchange (DFFT_EXCHANGE=staged)"));
     // the fused kernels pair the contiguous and the strided role of one table entry: square planes only
     {
         // policy: the fused kernel wins when the strided role's stores are NVLink-bound (P2P exchange: the
@@ -691,7 +737,7 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
         if (env) want = strcmp(env, "0") != 0;
         if (flags & DFFT_FORCE_FUSE) want = true;
         if (flags & DFFT_NO_FUSE) want = false;
-        p->fuse = can && want;
+        p->fuse = can && want && !real;   // R2C: the real Z pass has no fused form; the fusion flags are accepted and do nothing
         p->fuse_tma = p->fuse && tma_zy;
         if (getenv("DFFT_LAG")) p->lag = atoi(getenv("DFFT_LAG"));
         if (p->fuse && !dry) {
@@ -744,7 +790,7 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
         //    Default from 4 devices on for axes >= 1024 points, where the X pass that it hides is long enough to pay for the
         //    extra launches and the second read of the intermediate.
         // DFFT_FORCE_PIPELINE / DFFT_PIPELINE=1 pipeline wherever it is possible, DFFT_NO_PIPELINE / DFFT_PIPELINE=0 never.
-        const bool possible = P > 1 && !p->overlap && (xmode == DFFT_EXCHANGE_P2P || xmode == DFFT_EXCHANGE_NCCL);
+        const bool possible = P > 1 && !p->overlap && !real && (xmode == DFFT_EXCHANGE_P2P || xmode == DFFT_EXCHANGE_NCCL);
         const bool chain_ok = direction == DFFT_FORWARD && xmode == DFFT_EXCHANGE_P2P && p->fuse && ey == ex && ey->fused_yx != nullptr;
         bool want = possible && chain_ok && P >= 4 && n2 >= 1024;
         if (env) want = possible && strcmp(env, "0") != 0;
@@ -793,6 +839,11 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
                 }
             }
         }
+    }
+    if (real && P > 1) {
+        // R2C scratch where the C2C schedules borrow `out`: the forward Z output / NCCL send buffer, the backward Y output
+        if (dry) p->mid = fake_addr(dev_idx, 4);
+        else CUP(cudaMalloc(&p->mid, (size_t)p->max_count * p->esz));
     }
     if (P > 1 && dry) {
         p->peer_work.resize(P);
@@ -919,7 +970,7 @@ template <typename T> struct Pass {
         a.gen = e->gen;
         const int axis = axis_override >= 0 ? axis_override : (kind == PK_Z ? 0 : (kind == PK_Y || kind == PK_Y_CO || kind == PK_Y_CI ? 1 : 2));
         if (p->dry) {
-            static const char* names[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW"};
+            static const char* names[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW", "Z_R2C", "Z_C2R"};
             const int C = kind == PK_Z ? e->z_C : (kind == PK_Y || kind == PK_Y_CI ? e->s_C : (kind == PK_Y_CO ? e->p_C : e->x_C));
             // phase 1 = runs after the exchange has delivered this device's receive buffer
             const bool fwd = p->direction == DFFT_FORWARD;
@@ -980,6 +1031,43 @@ template <typename T> struct Pass {
         a.ia = Affine{0, (long long)C * g.n2, g.n2, 1}; a.oa = a.ia;
         a.do_scale = scale ? 1 : 0; a.scale = (T)(1.0 / ((double)g.n0 * (double)g.n1 * (double)g.n2));
         return launch(p, p->ez, PK_Z, a);
+    }
+    // real-data Z pass of an R2C plan (fft_real.cuh): the n0l*N1 real lines of N2r points, two per complex transform, <-> as many
+    // half-spectrum lines of nzh = g.n2 points.  Forward: src real -> dst complex; backward: src complex -> dst real (+ scale)
+    static int z_real(dfft_plan p, const void* src, void* dst, bool scale)
+    {
+        const Geom& g = p->g;
+        const bool fwd = p->direction == DFFT_FORWARD;
+        const int C = p->ez->z_C;
+        const long long nlines = p->n0l * g.n1, N = p->n2r, H = g.n2;
+        RealZArgs<T> r{};
+        TileArgs<T>& a = r.t;
+        a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)p->lut_z;
+        a.G = (int)cdiv(cdiv(nlines, 2), C); a.ntiles = a.G; a.W = (int)std::min<long long>(nlines, 0x7fffffff);
+        const Affine rmap{0, 2LL * C * N, 2 * N, 1}, cmap{0, 2LL * C * H, 2 * H, 1};   // tile, pair and point strides of each side
+        a.ia = fwd ? rmap : cmap; a.oa = fwd ? cmap : rmap;
+        r.ld_in = fwd ? N : H; r.ld_out = fwd ? H : N;   // the kernel derives nzh = N/2 + 1 from its schedule
+        if (fwd) r.rin = (const T*)src;
+        else r.rout = (T*)dst;
+        a.inv = fwd ? 0 : 1;
+        a.do_scale = scale ? 1 : 0; a.scale = (T)(1.0 / ((double)g.n0 * (double)g.n1 * (double)N));
+        const int kind = fwd ? PK_Z_R2C : PK_Z_C2R;
+        if (p->dry) {
+            // real-side maps are in real elements; "pair" = distance between the two lines of a pair (input side, output side)
+            record_op<T>(p, fwd ? "Z_R2C" : "Z_C2R", fwd ? 0 : 1, (int)N, C, false, false, false, a);
+            char buf[128];
+            snprintf(buf, sizeof(buf), ", \"nzh\": %lld, \"pair\": [%lld, %lld]}", H, r.ld_in, r.ld_out);
+            p->ops.back().pop_back();
+            p->ops.back() += buf;
+            p->launches++;
+            return 0;
+        }
+        ev_record(p, p->pev[0][0]);
+        cudaError_t err = p->ez->launch[kind](&r, p->sms, p->stream);
+        ev_record(p, p->pev[0][1]);
+        if (err != cudaSuccess) return fail(DFFT_ECUDA, "real Z pass launch (N=%lld) failed: %s", N, cudaGetErrorString(err));
+        p->launches++;
+        return 0;
     }
     // columns of length N1 (stride N2) of every local plane.  mode 0: src -> dst natural (in place when equal)
     // mode 1: chunked (packed / peer) store, mode 2: chunked (unpack) load
@@ -1785,6 +1873,92 @@ template <typename T> static int execute_fused(dfft_plan p)
     return 0;
 }
 
+// R2C / C2R plans: the C2C Y and X passes and exchanges over the nzh half-spectrum columns around the real-data Z pass; never fused
+// or pipelined.  The user's real buffer never holds complex data: where the C2C schedules borrow `out` (the forward Z output of the
+// P2P exchange, the NCCL send buffer, the backward Y output) an R2C plan uses its own `mid`.
+template <typename T> static int execute_real(dfft_plan p)
+{
+    const Geom& g = p->g;
+    const int P = p->P, me = p->me;
+    int rc;
+    p->launches = 0;
+    CU(ev_record(p, p->ev[0]));
+    if (p->direction == DFFT_FORWARD) {
+        if (P == 1) {
+            if ((rc = Pass<T>::z_real(p, p->buf1, p->work, false))) return rc;
+            if ((rc = Pass<T>::y_pass(p, p->work, p->work, 0, nullptr))) return rc;
+            CU(ev_record(p, p->ev[1]));
+            CU(ev_record(p, p->ev[2]));
+            if (p->natural) { if ((rc = Pass<T>::x_natural(p, p->work, p->buf2))) return rc; }
+            else if ((rc = Pass<T>::x_fwd(p, p->work, p->buf2))) return rc;
+        } else if (p->xmode == DFFT_EXCHANGE_P2P) {
+            void* base[DFFT_MAX_CHUNKS];
+            for (int q = 0; q < P; q++) base[q] = eoff(p->peer_work[q], recv_off(g, me, q, DFFT_FORWARD), p->esz);
+            p->epoch++;
+            const bool fold = p->done_ctr != nullptr && !p->dry;   // completion signals inside the pass kernels, as in execute_fused
+            Fold fy; fy.sig_which = 1; fy.sig_val = p->epoch; fy.ctr = 0;
+            Fold fx; fx.sig_which = 0; fx.sig_val = p->epoch; fx.ctr = 1;
+            const bool foldx = fold && Pass<T>::x_fwd_folds(p);
+            if ((rc = Pass<T>::z_real(p, p->buf1, p->mid, false))) return rc;
+            if ((rc = flags_wait(p, 0, p->epoch - 1))) return rc;   // every receiver has consumed the previous epoch
+            if ((rc = Pass<T>::y_pass(p, p->mid, nullptr, 1, base, fold ? &fy : nullptr))) return rc;
+            if (!fold && (rc = flags_signal(p, 1, p->epoch))) return rc;
+            CU(ev_record(p, p->ev[1]));
+            if ((rc = flags_wait(p, 1, p->epoch))) return rc;
+            CU(ev_record(p, p->ev[2]));
+            if ((rc = Pass<T>::x_fwd(p, p->work, p->buf2, foldx ? &fx : nullptr))) return rc;
+            if (!foldx && (rc = flags_signal(p, 0, p->epoch))) return rc;
+        } else {
+            void* base[DFFT_MAX_CHUNKS];
+            for (int q = 0; q < P; q++) base[q] = eoff(p->mid, send_off(g, me, q, DFFT_FORWARD), p->esz);
+            if ((rc = Pass<T>::z_real(p, p->buf1, p->work, false))) return rc;
+            if ((rc = Pass<T>::y_pass(p, p->work, nullptr, 1, base))) return rc;
+            CU(ev_record(p, p->ev[1]));
+            if ((rc = nccl_exchange(p, p->mid, p->work))) return rc;
+            CU(ev_record(p, p->ev[2]));
+            if ((rc = Pass<T>::x_fwd(p, p->work, p->buf2))) return rc;
+        }
+    } else {
+        const bool scale = (p->flags & DFFT_SCALE_BACKWARD) != 0;
+        if (P == 1) {
+            if (p->natural) { if ((rc = Pass<T>::x_natural(p, p->buf1, p->work))) return rc; }
+            else if ((rc = Pass<T>::x_bwd(p, p->buf1, p->work, nullptr))) return rc;
+            CU(ev_record(p, p->ev[1]));
+            CU(ev_record(p, p->ev[2]));
+            if ((rc = Pass<T>::y_pass(p, p->work, p->work, 0, nullptr))) return rc;
+            if ((rc = Pass<T>::z_real(p, p->work, p->buf2, scale))) return rc;
+        } else {
+            void* cb[DFFT_MAX_CHUNKS];
+            for (int q = 0; q < P; q++) cb[q] = eoff(p->work, (long long)q * p->n0l * g.yd() * g.n2, p->esz);
+            if (p->xmode == DFFT_EXCHANGE_P2P) {
+                p->epoch++;
+                const bool fold = p->done_ctr != nullptr && !p->dry;
+                Fold fxb; fxb.sig_which = 1; fxb.sig_val = p->epoch; fxb.ctr = 0;
+                if ((rc = flags_wait(p, 0, p->epoch - 1))) return rc;
+                void* base[DFFT_MAX_CHUNKS];
+                for (int q = 0; q < P; q++) base[q] = eoff(p->peer_work[q], recv_off(g, me, q, DFFT_BACKWARD), p->esz);
+                if ((rc = Pass<T>::x_bwd(p, p->buf1, nullptr, base, fold ? &fxb : nullptr))) return rc;
+                if (!fold && (rc = flags_signal(p, 1, p->epoch))) return rc;
+                CU(ev_record(p, p->ev[1]));
+                if ((rc = flags_wait(p, 1, p->epoch))) return rc;
+                CU(ev_record(p, p->ev[2]));
+                if ((rc = Pass<T>::y_pass(p, nullptr, p->mid, 2, cb))) return rc;
+                if ((rc = flags_signal(p, 0, p->epoch))) return rc;   // the receive buffer is consumed
+            } else {
+                if ((rc = Pass<T>::x_bwd(p, p->buf1, p->mid, nullptr))) return rc;
+                CU(ev_record(p, p->ev[1]));
+                if ((rc = nccl_exchange(p, p->mid, p->work))) return rc;
+                CU(ev_record(p, p->ev[2]));
+                if ((rc = Pass<T>::y_pass(p, nullptr, p->mid, 2, cb))) return rc;
+            }
+            if ((rc = Pass<T>::z_real(p, p->mid, p->buf2, scale))) return rc;
+        }
+    }
+    CU(ev_record(p, p->ev[3]));
+    p->timed = true;
+    return 0;
+}
+
 // reference-like stage-by-stage execution (api.cpp:181-214 with its device-wide syncs)
 template <typename T> static int execute_stage(dfft_plan p, int stage)
 {
@@ -1832,6 +2006,7 @@ template <typename T> static int execute_stage(dfft_plan p, int stage)
 
 extern "C" int dfft_execute_stage(dfft_plan p, int stage)
 {
+    if (p && p->r2c) return fail(DFFT_EUNSUPPORTED, "dfft_execute_stage: R2C / C2R plans have no stage-by-stage mode");
     if (!p || stage < 0 || stage > 3 || p->dry) return fail(DFFT_EINVAL, "dfft_execute_stage: bad arguments");
     if (p->xmode != DFFT_EXCHANGE_STAGED) return fail(DFFT_EINVAL, "dfft_execute_stage needs a plan created with DFFT_EXCHANGE_STAGED");
     CU(cudaSetDevice(p->device));
@@ -1854,6 +2029,7 @@ extern "C" int dfft_execute(dfft_plan p)
         p->timed = true;
         return 0;
     }
+    if (p->r2c) return p->prec == DFFT_DOUBLE ? execute_real<double>(p) : execute_real<float>(p);
     return p->prec == DFFT_DOUBLE ? execute_fused<double>(p) : execute_fused<float>(p);
 }
 
@@ -1917,10 +2093,10 @@ extern "C" int dfft_execute_host_async(dfft_plan p, const void* host_in, void* h
 {
     if (!p || !host_in || !host_out || p->dry) return fail(DFFT_EINVAL, "bad arguments");
     CU(cudaSetDevice(p->device));
-    CU(cudaMemcpyAsync(p->buf1, host_in, (size_t)p->in_count * p->esz, cudaMemcpyHostToDevice, p->stream));
+    CU(cudaMemcpyAsync(p->buf1, host_in, (size_t)p->in_count * p->in_esz, cudaMemcpyHostToDevice, p->stream));
     int rc = dfft_execute(p);
     if (rc) return rc;
-    CU(cudaMemcpyAsync(host_out, p->buf2, (size_t)p->out_count * p->esz, cudaMemcpyDeviceToHost, p->stream));
+    CU(cudaMemcpyAsync(host_out, p->buf2, (size_t)p->out_count * p->out_esz, cudaMemcpyDeviceToHost, p->stream));
     return 0;
 }
 
@@ -2227,7 +2403,7 @@ extern "C" long long dfft_debug_lines_ops(int n, long long stride, long long nli
         lp.npass = 1;
     }
     if (rc) return rc;
-    static const char* names[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW"};
+    static const char* names[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW", "Z_R2C", "Z_C2R"};
     for (int k = 0; k < lp.npass; k++) {
         const LinePass& ps = lp.pass[(direction == DFFT_BACKWARD && !lp.ordered) ? lp.npass - 1 - k : k];
         TileArgs<double> a{};

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <vector>
 #include "fft_passes.cuh"
+#include "fft_real.cuh"
 
 namespace dfft {
 
@@ -18,6 +19,8 @@ enum PassKind {
     PK_XB,         // contiguous load, strided store (MAP_T -> MAP_C)
     PK_XB_CO,      // + chunked (peer) store
     PK_XF_TW,      // PK_XF + four-step twiddle epilogue (first pass of a long 1-D transform)
+    PK_Z_R2C,      // real lines -> half spectra, two lines per complex transform (fft_real.cuh; args = RealZArgs)
+    PK_Z_C2R,      // half spectra -> real lines (fft_real.cuh; args = RealZArgs)
     PK_COUNT
 };
 

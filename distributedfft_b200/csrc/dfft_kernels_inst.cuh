@@ -34,6 +34,36 @@ cudaError_t launch_pass(const void* vargs, int sm_count, cudaStream_t st)
     return cudaGetLastError();
 }
 
+// real-data Z passes (fft_real.cuh): vargs is a RealZArgs<T>
+template <class S, typename T, int C, bool TW, int MINB, bool PP, bool C2R>
+cudaError_t launch_real(const void* vargs, int sm_count, cudaStream_t st)
+{
+    const RealZArgs<T>& a = *reinterpret_cast<const RealZArgs<T>*>(vargs);
+    auto kern = [] {   // only the kernel of this direction is instantiated
+        if constexpr (C2R) return fft_z_c2r_kernel<S, T, C, TW, MINB, PP>;
+        else return fft_z_r2c_kernel<S, T, C, TW, MINB, PP>;
+    }();
+    constexpr size_t smem = TileSmem<S, T, C, PP>::bytes(false);
+    static std::atomic<int> occ_cache[64];
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    int occ = occ_cache[dev & 63].load();
+    if (occ == 0) {
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, S::T * C, smem);
+        if (e != cudaSuccess) return e;
+        if (occ < 1) return cudaErrorLaunchOutOfResources;
+        occ_cache[dev & 63].store(occ);
+    }
+    if (a.t.ntiles <= 0) return cudaSuccess;
+    long long grid = (long long)sm_count * occ;
+    if (grid > a.t.ntiles) grid = a.t.ntiles;
+    kern<<<(unsigned)grid, S::T * C, smem, st>>>(a);
+    return cudaGetLastError();
+}
+
 template <class OpA, class OpB, typename T, int MINB>
 cudaError_t launch_fused(const void* va, const void* vb, const FusedCtl* ctl, int sm_count, cudaStream_t st)
 {
@@ -174,6 +204,15 @@ SizeEntry make_entry(int variant = 0)
     e.launch[PK_XB] = launch_pass<XS, T, X::C, MAP_T, MAP_C, X::TW, false, false, X::MB, X::PP>;
     e.launch[PK_XB_CO] = launch_pass<XS, T, X::C, MAP_T, MAP_C, X::TW, false, true, X::MB, X::PP>;
     e.launch[PK_XF_TW] = launch_pass<XS, T, X::C, MAP_C, MAP_T, X::TW, false, false, X::MB, X::PP, true>;
+    // real-data Z passes with the contiguous configuration (C line pairs per tile); default entries only -- the alternate
+    // tunings are experiments on the C2C path.  Twiddles come from shared memory (TWREG off): the pair loads and the split
+    // epilogue need the registers the twiddles would hold, and register twiddles spilled at 512 / 1024.  The inverse loads two
+    // lines per point and runs with one resident CTA less than the forward (no spills at 1024 fp32 otherwise)
+    if (variant == 0) {
+        constexpr int MBI = Z::MB > 3 ? 3 : Z::MB;
+        e.launch[PK_Z_R2C] = launch_real<ZS, T, Z::C, false, Z::MB, Z::PP, false>;
+        e.launch[PK_Z_C2R] = launch_real<ZS, T, Z::C, false, MBI, Z::PP, true>;
+    }
     // fused two-pass kernels: the contiguous role is re-tiled so that both roles fill the same CTA
     constexpr int NT = SS::T * Y::C, NTP = SS::T * PEER::C;
     static_assert(NT % ZS::T == 0 && NTP % ZS::T == 0, "strided CTA size must be a multiple of the contiguous line's thread count");

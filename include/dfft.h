@@ -1,5 +1,6 @@
 /*
- * dfft.h -- C ABI of the H100-native slab-decomposed 3-D complex-to-complex FFT (libdfft.so).
+ * dfft.h -- C ABI of the H100-native slab-decomposed 3-D complex-to-complex FFT (libdfft.so), with real-to-complex /
+ * complex-to-real plans over the same slabs (dfft_plan_r2c_3d).
  *
  * This is the drop-in boundary for the hot path of lueelu/DistributedFFT's `3dmpifft_opt`:
  * every entry point below names the reference interface it replaces (paths relative to the
@@ -161,6 +162,23 @@ int dfft_exchange_table(long long n0, long long n1, long long n2, int total_devi
  * The CUDA device current at the call is the plan's device. */
 int dfft_plan_c2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
                      int total_devices, int direction, int precision, unsigned flags, dfft_plan* plan);
+/* Real-to-complex (direction DFFT_FORWARD) and complex-to-real (DFFT_BACKWARD) transforms over the same slabs.
+ * R2C: in = real x-slab [x_l][y][z] (n0_l*n1*n2 reals) -> out = half spectrum, the C2C forward layout with z cut to
+ *      nzh = n2/2 + 1: [y_l][nzh][x] (x fastest), or [x][y][nzh] with DFFT_NATURAL_SPECTRUM (one device).
+ * C2R: the exact inverse layout, unnormalised (DFFT_SCALE_BACKWARD: 1/(n0*n1*n2)).  Any complex input is accepted and the
+ *      result is numpy.fft.irfftn(., s=(n0,n1,n2)) * n0*n1*n2: the imaginary parts at z = 0 and z = n2/2 (even n2) of every
+ *      z-line are ignored, as FFTW and numpy do.
+ * The buffers hold exactly dfft_local_size_r2c_3d()'s counts (reals on the real side, complex elements on the other); the
+ * plan never touches anything past them and copies `in` into its bufferDev1 at creation like the C2C plan.  `out` must be a
+ * separate buffer (NULL or out == in: DFFT_EINVAL).  The z length needs a tuned kernel (dfft_length_kind(n2, precision) == 2);
+ * y and x may be any length the C2C plan accepts.  Every device count and the P2P / NCCL exchanges work; DFFT_EXCHANGE_STAGED
+ * (and dfft_execute_stage) is DFFT_EUNSUPPORTED.  The fusion / overlap / pipeline flags are accepted and have no effect.
+ * dfft_plan_counts gives in_count / out_count in elements of their own type. */
+int dfft_plan_r2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
+                     int total_devices, int direction, int precision, unsigned flags, dfft_plan* plan);
+/* element counts of one device: reals of its x-slab, complex elements of its half-spectrum slab */
+int dfft_local_size_r2c_3d(long long n0, long long n1, long long n2, int total_devices, int dev_idx,
+                           long long* real_count, long long* complex_count);
 /* fft_mpi_execute_dft_3d_c2c, fft_mpi_3d_api.cpp:181-214.  Asynchronous on the plan's stream;
  * dfft_synchronize() or dfft_get_timings() waits.  Result in bufferDev2 (= out). */
 int dfft_execute(dfft_plan plan);

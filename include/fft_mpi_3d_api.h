@@ -139,6 +139,31 @@ inline fft_mpi_3d_plan_p fft_mpi_plan_dft_c2c_3d(longInt64 n0, longInt64 n1, lon
     return plan;
 }
 
+/* Real-to-complex (direction FORWARD: `in` = real x-slab [x_l][y][z], `out` = half spectrum [y_l][n2/2+1][x]) and
+ * complex-to-real (BACKWARD: the reverse) over the same slabs.  The reference has no R2C; this follows the C2C wrapper above.
+ * `in` and `out` are separate buffers of the sizes dfft_local_size_r2c_3d gives, so bufferDev1 / bufferDev2 hold real or
+ * complex data according to the direction (bufferDev1 = the input side).  Executed and destroyed like a C2C plan. */
+inline fft_mpi_3d_plan_p fft_mpi_plan_dft_r2c_3d(longInt64 n0, longInt64 n1, longInt64 n2, void* in, void* out, MPI_Comm, int devIdx,
+                                                 int devCountInNode, int totalDevCount, int direction)
+{
+    fft_mpi_3d_plan_p plan = new fft_mpi_3d_plan();
+    plan->N[0] = (int)n0; plan->N[1] = (int)n1; plan->N[2] = (int)n2;
+    plan->direction = direction;
+    plan->locGPUIdx = devIdx; plan->devCountInNode = devCountInNode; plan->totalDevCount = totalDevCount;
+    plan->globalDevIdx = devIdx;
+    plan->isLastDevice = devIdx == totalDevCount - 1;
+    plan->inDev = (Complex*)in; plan->outDev = (Complex*)out;
+    plan->isInplace = false;
+    dfft_comm comm = totalDevCount > 1 ? dfft_shim::local_comm(totalDevCount) : nullptr;
+    DFFT_CHECK(dfft_plan_r2c_3d(n0, n1, n2, in, out, comm, devIdx, totalDevCount, direction, DFFT_DOUBLE, DFFT_EXCHANGE_AUTO, &plan->impl));
+    DFFT_CHECK(dfft_plan_counts(plan->impl, nullptr, nullptr, &plan->maxDataCountInDevice));
+    void *b1 = nullptr, *b2 = nullptr;
+    DFFT_CHECK(dfft_plan_buffers(plan->impl, &b1, &b2));
+    plan->bufferDev1 = (Complex*)b1; plan->bufferDev2 = (Complex*)b2;
+    plan->nodeDataDev = nullptr;
+    return plan;
+}
+
 /* fft_mpi_3d_api.cpp:181-214: synchronous, prints the stage line on forward */
 inline void fft_mpi_execute_dft_3d_c2c(fft_mpi_3d_plan_p p)
 {
