@@ -732,7 +732,10 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
         // Forced fusion takes the TMA kernel whenever one exists, the register-staged kernel otherwise.
         const char* env = getenv("DFFT_FUSE");
         const bool tma_zy = P == 1 && direction == DFFT_FORWARD && n1 == n2 && !dry && p->tz && p->tz->fused_zy != nullptr && n2 % p->tz->C == 0;
-        const bool can = n1 == n2 && (ez->fused[FK_ZY] != nullptr || tma_zy);
+        // the register-staged kind this plan would launch (zy_fused, and the part kernels of the pipelined schedules) must exist:
+        // an entry leaves a kind null when its roles do not fit in shared memory together
+        const int kind = direction == DFFT_FORWARD ? (P == 1 ? FK_ZY : FK_ZY_CO) : (P == 1 ? FK_YZ : FK_YZ_CI);
+        const bool can = n1 == n2 && (ez->fused[kind] != nullptr || tma_zy);
         bool want = (P > 1 && xmode == DFFT_EXCHANGE_P2P) || (tma_zy && (p->tz->use & (1u << TMA_USE_ZY)));
         if (env) want = strcmp(env, "0") != 0;
         if (flags & DFFT_FORCE_FUSE) want = true;

@@ -159,6 +159,23 @@ cudaError_t launch_fused3(const void* va, const void* vb, const void* vc, const 
     return cudaGetLastError();
 }
 
+// Dynamic shared memory of the multi-role kernels: one exchange buffer (the largest role's) + every role's own twiddles, barrier
+// and chunk tables.  sm_90 grants at most 227 KB per block; a combination above that cannot be launched, so its entry is left
+// null and plans run the separate passes instead (4096 fp64: two 64 KB twiddle tables + a 136 KB exchange buffer; 2048 fp64 with
+// the chunk tables of the peer-store / unpack roles)
+constexpr size_t SMEM_OPTIN_MAX = 227 * 1024;
+template <class... Ops> constexpr size_t roles_smem()
+{
+    size_t exch = 0;
+    ((exch = Ops::SM::exch_bytes > exch ? Ops::SM::exch_bytes : exch), ...);
+    return exch + (Ops::aux_bytes + ...);
+}
+template <class OpA, class OpB, typename T, int MINB> constexpr FusedLaunchFn fused_if_fits()
+{
+    if constexpr (roles_smem<OpA, OpB>() <= SMEM_OPTIN_MAX) return launch_fused<OpA, OpB, T, MINB>;
+    else return nullptr;
+}
+
 template <class S> void fill_rad(int& n, int* rad)
 {
     n = S::NSTAGES;
@@ -229,16 +246,17 @@ SizeEntry make_entry(int variant = 0)
     using OY2 = TileOp<SS, T, Y::C, MAP_C, MAP_C, false, false, false, false, false, H1, H1>;
     using OYco = TileOp<SS, T, PEER::C, MAP_C, MAP_C, false, false, true, false, false, H1, 0>;
     using OYci = TileOp<SS, T, Y::C, MAP_C, MAP_C, false, true, false, false, false, H1, H2>;
-    e.fused[FK_ZY] = launch_fused<OZ, OY2, T, Y::MB>;
-    e.fused[FK_ZY_CO] = launch_fused<OZp, OYco, T, PEER::MB>;
-    e.fused[FK_YZ] = launch_fused<OY, OZ2, T, Y::MB>;
-    e.fused[FK_YZ_CI] = launch_fused<OYci, OZ2, T, Y::MB>;
+    e.fused[FK_ZY] = fused_if_fits<OZ, OY2, T, Y::MB>();
+    e.fused[FK_ZY_CO] = fused_if_fits<OZp, OYco, T, PEER::MB>();
+    e.fused[FK_YZ] = fused_if_fits<OY, OZ2, T, Y::MB>();
+    e.fused[FK_YZ_CI] = fused_if_fits<OYci, OZ2, T, Y::MB>();
     // whole forward transform of a device in one kernel: needs the X role to fill the peer-store CTA shape
+    e.fused3 = nullptr; e.fused_yx = nullptr;
     if constexpr (XS::T * X::C == NTP) {
         using OX = TileOp<XS, T, X::C, MAP_C, MAP_T, false, false, false, false>;
-        e.fused3 = launch_fused3<OZp, OYco, OX, T, (PEER::MB < X::MB ? PEER::MB : X::MB)>;
-        e.fused_yx = launch_fused_yx<OYco, OX, T, (PEER::MB < X::MB ? PEER::MB : X::MB)>;
-    } else { e.fused3 = nullptr; e.fused_yx = nullptr; }
+        if constexpr (roles_smem<OZp, OYco, OX>() <= SMEM_OPTIN_MAX) e.fused3 = launch_fused3<OZp, OYco, OX, T, (PEER::MB < X::MB ? PEER::MB : X::MB)>;
+        if constexpr (roles_smem<OYco, OX>() <= SMEM_OPTIN_MAX) e.fused_yx = launch_fused_yx<OYco, OX, T, (PEER::MB < X::MB ? PEER::MB : X::MB)>;
+    }
     return e;
 }
 

@@ -22,6 +22,7 @@ pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
 import distributedfft_b200 as dfft  # noqa: E402
 import ldfft  # noqa: E402
+from ld_harness import ratios64  # noqa: E402
 
 FWD, BWD = dfft.FORWARD, dfft.BACKWARD
 RDT = {dfft.DOUBLE: (np.float64, torch.float64), dfft.FLOAT: (np.float32, torch.float32)}
@@ -111,16 +112,6 @@ def ld_c2r(S, n2):
     full[:, :, :H] = y
     full[:, :, H:] = np.conj(y[:, :, 1: n2 - H + 1][:, :, ::-1])
     return ldfft.fft(full, 2, +1).real
-
-
-def ratios64(got, ref, eps, ntot):
-    """ldfft.ratios evaluated in fp64 (full cubes: the long-double copies would need tens of GB); the difference of two fp64
-    values this close is exact, so only the reference's own error (scipy, about 0.14 / 0.6 in these units) is added"""
-    ref = np.asarray(ref).ravel()
-    d = np.abs(np.asarray(got).ravel().astype(ref.dtype) - ref)
-    n2 = np.sum(np.abs(ref) ** 2)
-    u = eps * np.log2(ntot)
-    return float(np.sqrt(np.sum(d ** 2) / n2)) / u, float(d.max() / np.sqrt(n2 / ref.size)) / u
 
 
 def check(got, ref, prec, ntot, what):

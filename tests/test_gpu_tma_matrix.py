@@ -14,7 +14,6 @@ and the plan executes three times without a refill.  No NaN may survive, the can
 outputs bit-identical and an out-of-place input unchanged.  The shapes are thin slabs (only the axis under test is long);
 tile counts are derived from the device's SM count, since a pass kernel launches min(SMs, tiles) persistent CTAs, each
 running a 3-slot ring."""
-import collections
 import faulthandler
 import math
 import sys
@@ -26,13 +25,12 @@ pytestmark = pytest.mark.gpu
 
 torch = pytest.importorskip("torch")
 import distributedfft_b200 as dfft  # noqa: E402
+import ld_harness  # noqa: E402
 import ldfft  # noqa: E402
+from ld_harness import bits as _bits, layouts as _layouts, run_fenced  # noqa: E402
 from tma_entries import DOUBLE, ENTRIES, FLOAT, MASK_BIT, TMA_LENGTHS, entry_id, modes, thin_shape  # noqa: E402
 
 FWD, BWD = dfft.FORWARD, dfft.BACKWARD
-CDT = {DOUBLE: (np.complex128, torch.complex128), FLOAT: (np.complex64, torch.complex64)}
-EPS = {DOUBLE: ldfft.EPS["double"], FLOAT: ldfft.EPS["float"]}
-CANARY = 48
 BY = {(e[0], e[1]): e for e in ENTRIES}
 REF_FLAGS = dfft.NO_FUSE | dfft.NO_TMA
 
@@ -56,54 +54,7 @@ def sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-# ---- inputs and long-double references, cached per (shape, seed, precision, sign, kind) ------------------------------------
-_refs = collections.OrderedDict()
-
-
-def _logical_input(shape, seed, prec, sign, kind):
-    npdt = CDT[prec][0]
-    if kind == "rand":
-        rng = np.random.default_rng(seed)
-        return (rng.standard_normal(shape) + 1j * rng.standard_normal(shape)).astype(npdt)
-    x = np.zeros(shape, dtype=npdt)
-    if kind == "delta":                   # the last element of the device buffer in either layout (and of the last tile)
-        x[-1, -1, -1] = 1
-        return x
-    axis = int(np.argmax(shape))          # kind == "expo": one exponential at bin N-1 of the long axis
-    n = shape[axis]
-    e = ldfft._expi((n - 1) * np.arange(n), n, -sign).astype(npdt)
-    sl = [None, None, None]
-    sl[axis] = slice(None)
-    return np.broadcast_to(e[tuple(sl)], shape).astype(npdt)
-
-
-def _reference(shape, seed, prec, sign, kind="rand"):
-    key = (tuple(shape), seed, prec, sign, kind)
-    if key not in _refs:
-        x = _logical_input(shape, seed, prec, sign, kind)
-        _refs[key] = (x, ldfft.fftn(x, sign=sign))
-        while len(_refs) > 6:
-            _refs.popitem(last=False)
-    _refs.move_to_end(key)
-    return _refs[key]
-
-
-def _layouts(shape, seed, prec, direction, kind="rand", natural=False, scale=False):
-    """(device input, expected output), both flat, for a P = 1 plan: forward [x][y][z] -> [y][z][x], backward the reverse
-    (natural spectrum: [x][y][z] both ways)"""
-    x, y = _reference(shape, seed, prec, -1 if direction == FWD else 1, kind)
-    if natural:
-        dev_in, want = x.reshape(-1), y.reshape(-1)
-    elif direction == FWD:
-        dev_in, want = x.reshape(-1), y.transpose(1, 2, 0).reshape(-1)
-    else:
-        dev_in, want = x.transpose(1, 2, 0).reshape(-1), y.reshape(-1)
-    if scale:
-        want = want / np.longdouble(x.size)
-    return np.ascontiguousarray(dev_in), want
-
-
-# ---- one plan on its own fenced buffers ----------------------------------------------------------------------------------
+# ---- inputs, references and fenced runs: tests/ld_harness.py ------------------------------------------------------------
 def _set_tma(monkeypatch, forced):
     if forced:
         monkeypatch.setenv("DFFT_TMA", "2")
@@ -111,58 +62,8 @@ def _set_tma(monkeypatch, forced):
         monkeypatch.delenv("DFFT_TMA", raising=False)
 
 
-def _bits(a):
-    return np.ascontiguousarray(a).view(np.uint8)
-
-
-def run_fenced(shape, prec, direction, dev_in, flags=0, inplace=False, offset=0, repeat=3):
-    """create a P = 1 plan on fresh buffers and execute it `repeat` times; returns (output, tma_mask, fused).  The output
-    view starts `offset` elements after a canary block and is followed by another (the arena itself is 256-byte aligned)."""
-    npdt, tdt = CDT[prec]
-    n = int(np.prod(shape))
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(0)
-    total = CANARY + offset + n + CANARY
-    rng = np.random.default_rng(12345)
-    pattern = (rng.standard_normal(total) + 1j * rng.standard_normal(total)).astype(npdt)
-    arena = torch.from_numpy(pattern).to(dev)
-    view = arena[CANARY + offset: CANARY + offset + n]
-    if inplace:
-        view.copy_(torch.from_numpy(dev_in).to(dev))
-        tin = None
-    else:
-        view.fill_(complex(float("nan"), float("nan")))
-        tin = torch.from_numpy(dev_in).to(dev)
-    torch.cuda.synchronize(dev)
-    plan = dfft.fft_mpi_plan_dft_c2c_3d(*shape, (view if inplace else tin).data_ptr(), None if inplace else view.data_ptr(), None, 0, 1,
-                                        direction, prec, flags)
-    try:
-        outs = []
-        for _ in range(repeat):
-            plan.execute()
-            plan.synchronize()
-            outs.append(view.cpu().numpy().copy())
-        mask, fused = plan.tma_mask, plan.fused
-    finally:
-        plan.destroy()
-    host = arena.cpu().numpy()
-    got = outs[0]
-    assert not np.isnan(got.view(npdt().real.dtype)).any(), "NaN left in the output region: an element was never written"
-    lo, hi = CANARY + offset, CANARY + offset + n
-    assert np.array_equal(_bits(host[:lo]), _bits(pattern[:lo])), "canary before the output overwritten"
-    assert np.array_equal(_bits(host[hi:]), _bits(pattern[hi:])), "canary after the output overwritten"
-    for k in range(1, repeat):
-        assert np.array_equal(_bits(outs[k]), _bits(got)), "execute %d differs from the first" % k
-    if tin is not None:
-        assert np.array_equal(_bits(tin.cpu().numpy()), _bits(dev_in)), "out-of-place input modified"
-    return got, mask, fused
-
-
 def check(got, want, prec, ntot, label, linf_scale="rms"):
-    r = ldfft.ratios(got, want, EPS[prec], ntot, linf_scale)
-    print("TMA-RATIO %-52s rel_l2 %6.3f  linf %6.3f" % (label, r[0], r[1]))
-    assert r[0] <= ldfft.REL_L2_K and r[1] <= ldfft.LINF_K, (label, r)
-    return r
+    return ld_harness.check("TMA-RATIO", got, want, prec, ntot, label, linf_scale)
 
 
 def _label(entry, mode, forced, what):
