@@ -38,7 +38,7 @@ __all__ = [
     "BootstrapComm", "fft_mpi_init", "fft_mpi_plan_dft_c2c_3d", "fft_mpi_execute_dft_3d_c2c", "fft_mpi_destroy_plan",
     "fft_mpi_alloc_local_memory", "fft_mpi_local_size_3d", "fft_mpi_cleanup", "getMaxDataCount", "supported_lengths",
     "fft_mpi_plan_dft_r2c_3d", "local_size_r2c_3d",
-    "fft_lines", "lines_ops", "LinesPlan", "length_kind", "length_schedule", "memcpy_htod", "memcpy_dtoh", "exchange_table", "comm_allgather",
+    "fft_lines", "lines_ops", "LinesPlan", "RealLinesPlan", "real_lines_ops", "length_kind", "length_schedule", "memcpy_htod", "memcpy_dtoh", "exchange_table", "comm_allgather",
 ]
 
 
@@ -99,6 +99,11 @@ def lib():
     L.dfft_lines_destroy.argtypes = [vp]
     L.dfft_lines_stream.argtypes = [vp]
     L.dfft_lines_stream.restype = vp
+    L.dfft_lines_plan_create_r2c.argtypes = [i, ll, i, P(vp)]
+    L.dfft_lines_plan_create_r2c_2d.argtypes = [i, i, ll, i, P(vp)]
+    L.dfft_lines_execute_real.argtypes = [vp, vp, vp, i]
+    L.dfft_debug_real_lines_ops.argtypes = [i, i, ll, i, i, i, ctypes.c_char_p, ll]
+    L.dfft_debug_real_lines_ops.restype = ll
     L.dfft_length_kind.argtypes = [i, i]
     L.dfft_debug_plan_ops.argtypes = [vp, ctypes.c_char_p, ll]
     L.dfft_debug_plan_ops.restype = ll
@@ -395,6 +400,48 @@ class LinesPlan:
         if self.handle:
             lib().dfft_lines_destroy(self.handle)
             self.handle = None
+
+
+class RealLinesPlan:
+    """Real-data lines: R2C (FORWARD) / C2R (BACKWARD, unnormalised), out of place.  `nlines` densely packed real lines of `n`
+    points <-> as many half spectra of n//2+1 complex points, or, with `two_d=(nx, ny, batch)`, `batch` row-major ny x nx real
+    matrices <-> ny x (nx//2+1) complex matrices (numpy.fft.rfft2 layout)."""
+
+    def __init__(self, n=None, nlines=0, precision=DOUBLE, two_d=None):
+        h = ctypes.c_void_p()
+        if two_d is not None:
+            _check(lib().dfft_lines_plan_create_r2c_2d(two_d[0], two_d[1], two_d[2], precision, ctypes.byref(h)), "dfft_lines_plan_create_r2c_2d")
+        else:
+            _check(lib().dfft_lines_plan_create_r2c(n, nlines, precision, ctypes.byref(h)), "dfft_lines_plan_create_r2c")
+        self.handle = h
+
+    def execute(self, in_ptr, out_ptr, direction):
+        _check(lib().dfft_lines_execute_real(self.handle, in_ptr, out_ptr, direction), "dfft_lines_execute_real")
+
+    def synchronize(self):
+        _check(lib().dfft_lines_synchronize(self.handle), "dfft_lines_synchronize")
+
+    @property
+    def stream(self):
+        return lib().dfft_lines_stream(self.handle)
+
+    def destroy(self):
+        if self.handle:
+            lib().dfft_lines_destroy(self.handle)
+            self.handle = None
+
+
+def real_lines_ops(n, nlines, direction, precision=DOUBLE, two_d=None):
+    """passes a RealLinesPlan(n, nlines, precision, two_d) would launch for `direction` (host-only test hook, see
+    dfft_debug_real_lines_ops)"""
+    import json
+    args = (two_d[0], two_d[1], two_d[2], precision, direction, 1) if two_d is not None else (n, 1, nlines, precision, direction, 0)
+    need = lib().dfft_debug_real_lines_ops(*args, None, 0)
+    if need < 0:
+        raise DfftError(f"dfft_debug_real_lines_ops failed ({need}): " + lib().dfft_last_error().decode())
+    buf = ctypes.create_string_buffer(int(need))
+    lib().dfft_debug_real_lines_ops(*args, buf, need)
+    return json.loads(buf.value.decode())
 
 
 def lines_ops(n, stride, nlines, inner, inner_dist, outer_dist, direction, precision=DOUBLE, two_d=False):

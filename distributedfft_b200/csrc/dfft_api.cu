@@ -2185,13 +2185,21 @@ struct LinePass {
     int G = 0, W = 0;
     long long ntiles = 0;
     long long tw_n = 0;          // four-step twiddle modulus (PK_XF_TW)
-    int src = 0, dst = 0;        // 0 = the caller's data, 1 = the plan's temporary
+    int src = 0, dst = 0;        // LB_IN (the caller's data / a real plan's `in`), LB_TEMP (the plan's temporary), LB_OUT
+    long long ld_in = 0, ld_out = 0;   // PK_Z_R2C / PK_Z_C2R: distance between the two lines of a pair (RealZArgs), each side's elements
 };
+enum { LB_IN = 0, LB_TEMP = 1, LB_OUT = 2 };
 struct dfft_lines_plan_s {
     int prec = 0, device = 0, sms = 132, npass = 0;
     bool ordered = false;        // passes run in the same order for both directions (four-step)
     void* temp = nullptr;
     LinePass pass[2];
+    // real plans (dfft_lines_plan_create_r2c[_2d]): the passes of each direction in execution order, [0] forward, [1] backward;
+    // `pass` stays empty.  Read by dfft_lines_execute_real and dfft_debug_real_lines_ops alike
+    bool real = false;
+    int nreal = 0;
+    LinePass rpass[2][2];
+    long long rcount = 0, ccount = 0;   // reals and complex elements of the caller's real / complex buffer
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[2] = {nullptr, nullptr};
     bool timed = false;
@@ -2247,6 +2255,8 @@ extern "C" int dfft_lines_destroy(dfft_lines_plan p)
     cudaSetDevice(p->device);
     if (p->stream) cudaStreamSynchronize(p->stream);
     for (int i = 0; i < 2; i++) if (p->pass[i].lut) cudaFree(p->pass[i].lut);
+    for (auto& dir : p->rpass)
+        for (auto& lp : dir) if (lp.lut) cudaFree(lp.lut);
     if (p->temp) cudaFree(p->temp);
     for (auto& e : p->ev) if (e) cudaEventDestroy(e);
     if (p->stream) cudaStreamDestroy(p->stream);
@@ -2368,6 +2378,7 @@ template <typename T> static int lines_execute_impl(dfft_lines_plan p, void* dat
 extern "C" int dfft_lines_execute(dfft_lines_plan p, void* data, int direction)
 {
     if (!p || !data || (direction != DFFT_FORWARD && direction != DFFT_BACKWARD)) return fail(DFFT_EINVAL, "bad arguments");
+    if (p->real) return fail(DFFT_EINVAL, "a real lines plan runs with dfft_lines_execute_real");
     CU(cudaSetDevice(p->device));
     return p->prec == DFFT_DOUBLE ? lines_execute_impl<double>(p, data, direction) : lines_execute_impl<float>(p, data, direction);
 }
@@ -2415,6 +2426,174 @@ extern "C" long long dfft_debug_lines_ops(int n, long long stride, long long nli
         a.inv = direction == DFFT_BACKWARD; a.tw_n = ps.tw_n;
         const int C = ps.kind == PK_Z ? ps.e->z_C : (ps.kind == PK_Y ? ps.e->s_C : ps.e->x_C);
         record_op<double>(&rec, names[ps.kind], k, ps.e->N, C, false, false, ps.kind == PK_XF_TW, a);
+    }
+    lp.temp = nullptr;
+    std::string o = "[";
+    for (size_t i = 0; i < rec.ops.size(); i++) { if (i) o += ", "; o += rec.ops[i]; }
+    o += "]";
+    if (buf && cap > (long long)o.size()) memcpy(buf, o.c_str(), o.size() + 1);
+    return (long long)o.size() + 1;
+}
+
+// ---- real lines: R2C / C2R over densely packed lines (1-D) and the rows of row-major matrices (2-D) --------------------------
+// The real pass is the kernel pair of the 3-D plan's Z pass (Pass<T>::z_real): two real lines per complex transform, lines
+// paired in order, on the tuned kernels (fft_real.cuh) or, for a run-time-scheduled length, fft_generic_r2c / c2r_kernel.
+static void make_real_pass(LinePass& lp, const SizeEntry* e, long long nlines, bool fwd, int src, int dst)
+{
+    const int C = e->z_C;
+    const long long N = e->N, H = N / 2 + 1;
+    lp.e = e;
+    lp.kind = fwd ? PK_Z_R2C : PK_Z_C2R;
+    lp.G = (int)cdiv(cdiv(nlines, 2), C); lp.ntiles = lp.G; lp.W = (int)nlines;
+    const Affine rmap{0, 2LL * C * N, 2 * N, 1}, cmap{0, 2LL * C * H, 2 * H, 1};   // tile, pair and point strides of each side
+    lp.ia = fwd ? rmap : cmap; lp.oa = fwd ? cmap : rmap;
+    lp.ld_in = fwd ? N : H; lp.ld_out = fwd ? H : N;
+    lp.src = src; lp.dst = dst;
+}
+
+// 1-D: `batch` lines of n points (ny unused).  2-D: `batch` ny x n matrices, rows real <-> rows of n/2+1 complex points
+static int make_real_lines(dfft_lines_plan p, int n, int ny, long long batch, int precision, bool two_d, bool dry)
+{
+    if (batch < 0 || (two_d && ny < 1) || (precision != DFFT_DOUBLE && precision != DFFT_FLOAT)) return fail(DFFT_EINVAL, "bad arguments");
+    const SizeEntry* e = n < 2 ? nullptr : find_size_entry(n, precision);
+    if (!e) return fail(DFFT_EUNSUPPORTED, "real lines of %d points: the length must be 2..13-smooth and fit one shared-memory line", n);
+    if (!e->launch[PK_Z_R2C] || !e->launch[PK_Z_C2R]) return fail(DFFT_EUNSUPPORTED, "the kernel entry of length %d has no real-data kernels", n);
+    const long long rows = two_d ? (long long)ny * batch : batch;
+    if (rows > 0x7fffffffLL) return fail(DFFT_EUNSUPPORTED, "%lld real lines: at most 2^31 - 1 per plan", rows);
+    const long long H = n / 2 + 1;
+    p->real = true;
+    p->prec = precision;
+    p->rcount = rows * n;
+    p->ccount = rows * H;
+    LinePass* f = p->rpass[0];
+    LinePass* b = p->rpass[1];
+    make_real_pass(f[0], e, rows, true, LB_IN, LB_OUT);
+    if (!two_d) {
+        make_real_pass(b[0], e, rows, false, LB_IN, LB_OUT);
+        p->nreal = 1;
+    } else {
+        // along ny: the H columns of every half-spectrum matrix, matrices ny*H apart.  Forward in place in `out`; backward from
+        // `in` into the temporary, so that `in` is never written
+        int rc = make_line_pass(f[1], ny, H, H * batch, H, 1, H * ny, precision, dry);
+        if (!rc) rc = make_line_pass(b[0], ny, H, H * batch, H, 1, H * ny, precision, dry);
+        if (rc) return rc;
+        f[1].src = f[1].dst = LB_OUT;
+        b[0].src = LB_IN; b[0].dst = LB_TEMP;
+        make_real_pass(b[1], e, rows, false, LB_TEMP, LB_OUT);
+        p->nreal = 2;
+        const size_t esz = precision == DFFT_FLOAT ? 8 : 16;
+        if (dry) p->temp = fake_addr(0, 4);
+        else if (p->ccount > 0) CU(cudaMalloc(&p->temp, (size_t)p->ccount * esz));
+    }
+    if (dry) return 0;
+    for (auto& dir : p->rpass)
+        for (int k = 0; k < p->nreal; k++) {
+            LinePass& lp = dir[k];
+            if (lp.kind != PK_Z_R2C && lp.kind != PK_Z_C2R) continue;
+            if (precision == DFFT_DOUBLE) upload_lut_e<double>(&lp.lut, e, true);
+            else upload_lut_e<float>(&lp.lut, e, true);
+            if (!lp.lut) break;
+        }
+    if (cudaGetLastError() != cudaSuccess || !f[0].lut || !b[p->nreal - 1].lut) return fail(DFFT_ECUDA, "twiddle table upload failed");
+    return 0;
+}
+
+static inline void* line_buf(int which, const void* in, void* out, void* temp)
+{
+    return which == LB_TEMP ? temp : (which == LB_OUT ? out : const_cast<void*>(in));
+}
+
+// the kernel arguments of one pass of a real plan (a C2C pass uses r.t alone)
+template <typename T> static void real_line_args(const LinePass& lp, const void* src, void* dst, int direction, RealZArgs<T>& r)
+{
+    TileArgs<T>& a = r.t;
+    a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)lp.lut;
+    a.ia = lp.ia; a.oa = lp.oa; a.G = lp.G; a.W = lp.W; a.ntiles = lp.ntiles;
+    a.inv = direction == DFFT_BACKWARD; a.gen = lp.e->gen; a.tw_n = lp.tw_n;
+    r.rin = (const T*)src; r.rout = (T*)dst;
+    r.ld_in = lp.ld_in; r.ld_out = lp.ld_out;
+}
+
+static int real_plan_create(int n, int ny, long long batch, int precision, bool two_d, dfft_lines_plan* out)
+{
+    if (!out) return fail(DFFT_EINVAL, "null plan pointer");
+    *out = nullptr;
+    dfft_lines_plan p = new dfft_lines_plan_s;
+    int rc = lines_plan_common(p, precision);
+    if (!rc) rc = make_real_lines(p, n, ny, batch, precision, two_d, false);
+    if (rc) { dfft_lines_destroy(p); return rc; }
+    *out = p;
+    return 0;
+}
+
+extern "C" int dfft_lines_plan_create_r2c(int n, long long nlines, int precision, dfft_lines_plan* plan)
+{
+    return real_plan_create(n, 1, nlines, precision, false, plan);
+}
+
+extern "C" int dfft_lines_plan_create_r2c_2d(int nx, int ny, long long batch, int precision, dfft_lines_plan* plan)
+{
+    return real_plan_create(nx, ny, batch, precision, true, plan);
+}
+
+template <typename T> static int lines_execute_real_impl(dfft_lines_plan p, const void* in, void* out, int direction)
+{
+    const int d = direction == DFFT_FORWARD ? 0 : 1;
+    CU(cudaEventRecord(p->ev[0], p->stream));
+    for (int k = 0; k < p->nreal; k++) {
+        const LinePass& lp = p->rpass[d][k];
+        if (lp.ntiles <= 0) continue;
+        RealZArgs<T> r{};
+        real_line_args<T>(lp, line_buf(lp.src, in, out, p->temp), line_buf(lp.dst, in, out, p->temp), direction, r);
+        const bool realk = lp.kind == PK_Z_R2C || lp.kind == PK_Z_C2R;
+        cudaError_t err = lp.e->launch[lp.kind](realk ? (const void*)&r : (const void*)&r.t, p->sms, p->stream);
+        if (err != cudaSuccess) return fail(DFFT_ECUDA, "real line pass launch failed: %s", cudaGetErrorString(err));
+    }
+    CU(cudaEventRecord(p->ev[1], p->stream));
+    p->timed = true;
+    return 0;
+}
+
+extern "C" int dfft_lines_execute_real(dfft_lines_plan p, const void* in, void* out, int direction)
+{
+    if (!p || !in || !out || (direction != DFFT_FORWARD && direction != DFFT_BACKWARD)) return fail(DFFT_EINVAL, "bad arguments");
+    if (!p->real) return fail(DFFT_EINVAL, "a complex lines plan runs with dfft_lines_execute");
+    const size_t rsz = p->prec == DFFT_FLOAT ? 4 : 8, csz = 2 * rsz;
+    const bool fwd = direction == DFFT_FORWARD;
+    const uintptr_t ri = (uintptr_t)(fwd ? in : out), ci = (uintptr_t)(fwd ? out : in);
+    if (ri % rsz || ci % csz) return fail(DFFT_EINVAL, "a %s buffer is not aligned to its element size", ri % rsz ? "real" : "complex");
+    const uintptr_t a = (uintptr_t)in, b = (uintptr_t)out;
+    const uintptr_t a_end = a + (fwd ? p->rcount * rsz : p->ccount * csz), b_end = b + (fwd ? p->ccount * csz : p->rcount * rsz);
+    if (a == b || (a < b_end && b < a_end)) return fail(DFFT_EINVAL, "`in` and `out` overlap (real lines are out of place)");
+    CU(cudaSetDevice(p->device));
+    return p->prec == DFFT_DOUBLE ? lines_execute_real_impl<double>(p, in, out, direction) : lines_execute_real_impl<float>(p, in, out, direction);
+}
+
+/* test hook (host only): the passes of a real lines plan for `direction`, JSON as dfft_debug_lines_ops; in = buffer 5, out = 2,
+ * temporary = 4 of device 0.  Real passes carry "nzh" and "pair" as the 3-D plan's Z_R2C / Z_C2R records */
+extern "C" long long dfft_debug_real_lines_ops(int n, int ny, long long batch, int precision, int direction, int two_d, char* buf, long long cap)
+{
+    if (direction != DFFT_FORWARD && direction != DFFT_BACKWARD) return fail(DFFT_EINVAL, "bad direction");
+    dfft_lines_plan_s lp;
+    dfft_plan_s rec;   // only its `ops` vector is used
+    rec.dry = true;
+    const int rc = make_real_lines(&lp, n, ny, batch, precision, two_d != 0, true);
+    if (rc) return rc;
+    static const char* names[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW", "Z_R2C", "Z_C2R"};
+    const int d = direction == DFFT_FORWARD ? 0 : 1;
+    for (int k = 0; k < lp.nreal; k++) {
+        const LinePass& ps = lp.rpass[d][k];
+        RealZArgs<double> r{};
+        real_line_args<double>(ps, line_buf(ps.src, fake_addr(0, 5), fake_addr(0, 2), lp.temp), line_buf(ps.dst, fake_addr(0, 5), fake_addr(0, 2), lp.temp),
+                               direction, r);
+        const bool realk = ps.kind == PK_Z_R2C || ps.kind == PK_Z_C2R;
+        record_op<double>(&rec, names[ps.kind], k, ps.e->N, realk ? ps.e->z_C : ps.e->s_C, false, false, false, r.t);
+        if (realk) {
+            char b[128];
+            snprintf(b, sizeof(b), ", \"nzh\": %d, \"pair\": [%lld, %lld]}", ps.e->N / 2 + 1, ps.ld_in, ps.ld_out);
+            rec.ops.back().pop_back();
+            rec.ops.back() += b;
+        }
     }
     lp.temp = nullptr;
     std::string o = "[";

@@ -74,6 +74,39 @@ static cudaError_t launch_generic(const void* vargs, int sm_count, cudaStream_t 
     return cudaGetLastError();
 }
 
+// real-data passes (fft_generic_r2c_kernel / fft_generic_c2r_kernel): vargs is a RealZArgs<T>, a tile is G.C line pairs
+template <typename T, bool INV>
+static cudaError_t launch_generic_real(const void* vargs, int sm_count, cudaStream_t st)
+{
+    const RealZArgs<T>& a = *reinterpret_cast<const RealZArgs<T>*>(vargs);
+    if (!a.t.gen) return cudaErrorInvalidValue;
+    const GenSched& g = *reinterpret_cast<const GenSched*>(a.t.gen);
+    auto kern = INV ? fft_generic_c2r_kernel<T> : fft_generic_r2c_kernel<T>;
+    const size_t smem = 2 * (size_t)g.C * g.N * sizeof(cx<T>);
+    static std::mutex mu;
+    static size_t attr_set[64] = {0};
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    {
+        std::lock_guard<std::mutex> lk(mu);
+        if (attr_set[dev & 63] < smem) {
+            e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024));
+            if (e != cudaSuccess) return e;
+            attr_set[dev & 63] = 200 * 1024;
+        }
+    }
+    if (a.t.ntiles <= 0) return cudaSuccess;
+    int occ = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, GEN_THREADS, smem);
+    if (e != cudaSuccess) return e;
+    if (occ < 1) return cudaErrorLaunchOutOfResources;
+    long long grid = (long long)sm_count * occ;
+    if (grid > a.t.ntiles) grid = a.t.ntiles;
+    kern<<<(unsigned)grid, GEN_THREADS, smem, st>>>(a, g);
+    return cudaGetLastError();
+}
+
 template <typename T> static void fill_launchers(SizeEntry& e)
 {
     e.launch[PK_Z] = launch_generic<T, MAP_T, MAP_T, false, false>;
@@ -84,6 +117,9 @@ template <typename T> static void fill_launchers(SizeEntry& e)
     e.launch[PK_XB] = launch_generic<T, MAP_T, MAP_C, false, false>;
     e.launch[PK_XB_CO] = launch_generic<T, MAP_T, MAP_C, false, true>;
     e.launch[PK_XF_TW] = launch_generic<T, MAP_C, MAP_T, false, false>;   // the twiddle epilogue is a run-time switch (TileArgs::tw_n)
+    // real lines of the lines engine; the 3-D R2C plan still refuses generic z lengths (plan_create)
+    e.launch[PK_Z_R2C] = launch_generic_real<T, false>;
+    e.launch[PK_Z_C2R] = launch_generic_real<T, true>;
 }
 
 const SizeEntry* generic_size_entry(int N, int prec)

@@ -9,6 +9,7 @@
 // stages, unpadded exchange buffers) -- it exists for API parity, not for the headline sizes.
 #pragma once
 #include "fft_passes.cuh"
+#include "fft_real.cuh"
 
 namespace dfft {
 
@@ -158,6 +159,111 @@ __global__ void __launch_bounds__(GEN_THREADS) fft_generic_kernel(const TileArgs
         }
     }
     signal_when_grid_done<T>(A);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Real-data passes on the run-time schedule: the generic counterparts of fft_z_r2c_kernel / fft_z_c2r_kernel (fft_real.cuh),
+// same RealZArgs addressing (a tile is C line PAIRS, pair (tile, c) at base + tile*SB + c*cs, its second line `ld` further,
+// TileArgs::W = number of lines, points contiguous) and the same split formulas.  A pair occupies one line of each ping-pong
+// buffer, so the shared-memory footprint is that of fft_generic_kernel with the same C.
+
+// every stage of G on C lines starting in buf0; returns the buffer that holds the result
+template <typename T>
+__device__ __forceinline__ cx<T>* generic_stages(cx<T>* buf0, cx<T>* buf1, const cx<T>* __restrict__ lut0, const GenSched& G)
+{
+    cx<T>* src = buf0;
+    cx<T>* dst = buf1;
+    for (int s = 0; s < G.nstages; s++) {
+        const int NS = G.ns[s];
+        const cx<T>* lut = lut0 + G.lut_off[s];
+        switch (G.rad[s]) {
+            case 2: generic_stage<T, 2>(src, dst, lut, G.N, G.C, NS, s > 0); break;
+            case 3: generic_stage<T, 3>(src, dst, lut, G.N, G.C, NS, s > 0); break;
+            case 4: generic_stage<T, 4>(src, dst, lut, G.N, G.C, NS, s > 0); break;
+            case 5: generic_stage<T, 5>(src, dst, lut, G.N, G.C, NS, s > 0); break;
+            case 7: generic_stage<T, 7>(src, dst, lut, G.N, G.C, NS, s > 0); break;
+            case 8: generic_stage<T, 8>(src, dst, lut, G.N, G.C, NS, s > 0); break;
+            case 11: generic_stage<T, 11>(src, dst, lut, G.N, G.C, NS, s > 0); break;
+            case 13: generic_stage<T, 13>(src, dst, lut, G.N, G.C, NS, s > 0); break;
+            default: __trap();
+        }
+        __syncthreads();
+        cx<T>* t = src; src = dst; dst = t;
+    }
+    return src;
+}
+
+// R2C: z = a + i b per pair, the stages, then A / B straight from the transformed line in shared memory
+template <typename T>
+__global__ void __launch_bounds__(GEN_THREADS) fft_generic_r2c_kernel(const RealZArgs<T> R, const GenSched G)
+{
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const TileArgs<T>& A = R.t;
+    const int N = G.N, C = G.C, H = N / 2 + 1;
+    cx<T>* buf0 = reinterpret_cast<cx<T>*>(smem_raw);
+    cx<T>* buf1 = buf0 + (size_t)C * N;
+    const int tid = threadIdx.x;
+    const T h = (T)0.5;
+    for (long long tile = blockIdx.x; tile < A.ntiles; tile += gridDim.x) {
+        __syncthreads();                          // the previous tile's split has read its result buffer
+        for (int i = tid; i < C * N; i += GEN_THREADS) {   // threads along the line: coalesced
+            const int e = i % N, c = i / N;
+            const long long line0 = 2 * (tile * C + c);
+            const T* pa = R.rin + tile * A.ia.SB + c * A.ia.cs + e;
+            buf0[i] = mk<T>(line0 < A.W ? ld_stream(pa) : (T)0, line0 + 1 < A.W ? ld_stream(pa + R.ld_in) : (T)0);
+        }
+        __syncthreads();
+        const cx<T>* z = generic_stages<T>(buf0, buf1, A.lut, G);
+        for (int i = tid; i < C * H; i += GEN_THREADS) {
+            const int j = i % H, c = i / H;
+            const long long line0 = 2 * (tile * C + c);
+            if (line0 >= A.W) continue;
+            const cx<T> p = z[c * N + j], m = z[c * N + (j == 0 ? 0 : N - j)];
+            cx<T>* qa = A.out + tile * A.oa.SB + c * A.oa.cs + j;
+            st_stream(qa, mk<T>(h * (p.x + m.x), h * (p.y - m.y)));
+            if (line0 + 1 < A.W) st_stream(qa + R.ld_out, mk<T>(h * (p.y + m.y), h * (m.x - p.x)));
+        }
+    }
+}
+
+// C2R: Z = A + i B up to N/2, conj A[N-j] + i conj B[N-j] above (Im A, Im B dropped at j = 0 and, even N, j = N/2), loaded
+// swapped as in fft_generic_kernel's inverse; after the stages Re z = v.y goes to line a and Im z = v.x to line b
+template <typename T>
+__global__ void __launch_bounds__(GEN_THREADS) fft_generic_c2r_kernel(const RealZArgs<T> R, const GenSched G)
+{
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const TileArgs<T>& A = R.t;
+    const int N = G.N, C = G.C, H = N / 2 + 1;
+    cx<T>* buf0 = reinterpret_cast<cx<T>*>(smem_raw);
+    cx<T>* buf1 = buf0 + (size_t)C * N;
+    const int tid = threadIdx.x;
+    const T s = A.do_scale ? A.scale : (T)1;
+    for (long long tile = blockIdx.x; tile < A.ntiles; tile += gridDim.x) {
+        __syncthreads();                          // the previous tile's stores have read its result buffer
+        for (int i = tid; i < C * N; i += GEN_THREADS) {
+            const int e = i % N, c = i / N;
+            const long long line0 = 2 * (tile * C + c);
+            const bool mirror = e >= H;
+            const int j = mirror ? N - e : e;
+            const cx<T>* pa = A.in + tile * A.ia.SB + c * A.ia.cs + j;
+            cx<T> a = line0 < A.W ? ld_stream(pa) : mk<T>(0, 0);
+            cx<T> b = line0 + 1 < A.W ? ld_stream(pa + R.ld_in) : mk<T>(0, 0);
+            if (j == 0 || 2 * j == N) { a.y = 0; b.y = 0; }
+            // z = (a.x - b.y, a.y + b.x) below, (a.x + b.y, b.x - a.y) above; stored as (Im z, Re z)
+            buf0[i] = mirror ? mk<T>(b.x - a.y, a.x + b.y) : mk<T>(a.y + b.x, a.x - b.y);
+        }
+        __syncthreads();
+        const cx<T>* z = generic_stages<T>(buf0, buf1, A.lut, G);
+        for (int i = tid; i < C * N; i += GEN_THREADS) {
+            const int e = i % N, c = i / N;
+            const long long line0 = 2 * (tile * C + c);
+            if (line0 >= A.W) continue;
+            const cx<T> v = z[i];
+            T* qa = R.rout + tile * A.oa.SB + c * A.oa.cs + e;
+            st_stream(qa, v.y * s);
+            if (line0 + 1 < A.W) st_stream(qa + R.ld_out, v.x * s);
+        }
+    }
 }
 
 }  // namespace dfft

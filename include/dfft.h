@@ -247,6 +247,24 @@ int dfft_lines_execute(dfft_lines_plan plan, void* data, int direction);
 int dfft_lines_synchronize(dfft_lines_plan plan);
 void* dfft_lines_stream(dfft_lines_plan plan);
 int dfft_lines_destroy(dfft_lines_plan plan);
+/* Real-data lines (R2C forward / C2R backward), out of place, on the same engine:
+ *    1-D: nlines densely packed real lines of n points  <->  nlines densely packed half spectra of n/2+1 complex points.
+ *    2-D: batch row-major ny x nx real matrices (nx fastest)  <->  batch ny x (nx/2+1) complex matrices (numpy.fft.rfft2 layout).
+ * The real axis (n, nx) takes every length with dfft_length_kind(n, precision) >= 1: tuned lengths run on the real kernels of
+ * the 3-D plan's Z pass, other 2..13-smooth lengths up to one shared-memory line on the run-time-scheduled real kernels.  Longer
+ * lines, other prime factors, n < 2, a DFFT_VARIANT kernel entry without real kernels and 2^31 or more real lines are
+ * DFFT_EUNSUPPORTED.  The 2-D plan's ny takes any length a strided C2C lines pass takes; its backward transform uses a
+ * plan-owned temporary of batch*ny*(nx/2+1) complex elements. */
+int dfft_lines_plan_create_r2c(int n, long long nlines, int precision, dfft_lines_plan* plan);
+int dfft_lines_plan_create_r2c_2d(int nx, int ny, long long batch, int precision, dfft_lines_plan* plan);
+/* FORWARD: in = reals -> out = half spectra.  BACKWARD: in = half spectra -> out = reals, unnormalised (numpy.fft.irfft / irfft2
+ * times n / nx*ny; the imaginary parts at bin 0 and, for even n, bin n/2 are ignored, as in the 3-D C2R).  `in` is never
+ * written.  Null or overlapping buffers, a buffer not aligned to its element size, and a complex plan are DFFT_EINVAL (and a
+ * real plan passed to dfft_lines_execute).  Asynchronous on the plan's stream (dfft_lines_synchronize waits). */
+int dfft_lines_execute_real(dfft_lines_plan plan, const void* in, void* out, int direction);
+/* test hook (host only): the passes of a real lines plan (1-D: n, nlines = batch, ny unused; 2-D when two_d != 0), same JSON
+ * as dfft_debug_lines_ops, with "nzh" and "pair" on the real passes; in = buffer 5, out = buffer 2, temporary = buffer 4 */
+long long dfft_debug_real_lines_ops(int n, int ny, long long batch, int precision, int direction, int two_d, char* buf, long long cap);
 /* one-shot convenience (plan + execute + synchronize + destroy), used by the per-axis parity tests */
 int dfft_fft_lines(void* data, int n, long long stride, long long nlines, long long inner, long long inner_dist,
                    long long outer_dist, int direction, int precision);
