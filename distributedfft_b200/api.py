@@ -37,7 +37,7 @@ __all__ = [
     "EXCHANGE_NCCL", "EXCHANGE_STAGED", "SCALE_BACKWARD", "NO_FUSE", "FORCE_FUSE", "OVERLAP_X", "NATURAL_SPECTRUM", "DRY_RUN", "NO_PIPELINE", "NO_TMA", "FORCE_PIPELINE", "DfftError", "lib", "LIB_PATH", "Plan", "LocalComm",
     "BootstrapComm", "fft_mpi_init", "fft_mpi_plan_dft_c2c_3d", "fft_mpi_execute_dft_3d_c2c", "fft_mpi_destroy_plan",
     "fft_mpi_alloc_local_memory", "fft_mpi_local_size_3d", "fft_mpi_cleanup", "getMaxDataCount", "supported_lengths",
-    "fft_mpi_plan_dft_r2c_3d", "local_size_r2c_3d",
+    "fft_mpi_plan_dft_r2c_3d", "local_size_r2c_3d", "fft_mpi_plan_dft_convolve_3d",
     "fft_lines", "lines_ops", "LinesPlan", "RealLinesPlan", "real_lines_ops", "length_kind", "length_schedule", "memcpy_htod", "memcpy_dtoh", "exchange_table", "comm_allgather",
 ]
 
@@ -80,6 +80,9 @@ def lib():
     L.dfft_plan_c2c_3d.argtypes = [ll, ll, ll, vp, vp, vp, i, i, i, i, u, P(vp)]
     L.dfft_plan_r2c_3d.argtypes = [ll, ll, ll, vp, vp, vp, i, i, i, i, u, P(vp)]
     L.dfft_local_size_r2c_3d.argtypes = [ll, ll, ll, i, i, P(ll), P(ll)]
+    L.dfft_plan_convolve_c2c_3d.argtypes = [ll, ll, ll, vp, vp, vp, i, i, i, u, P(vp)]
+    L.dfft_plan_convolve_r2c_3d.argtypes = [ll, ll, ll, vp, vp, vp, i, i, i, u, P(vp)]
+    L.dfft_execute_convolve.argtypes = [vp, vp]
     for name in ("dfft_execute", "dfft_synchronize", "dfft_destroy", "dfft_plan_launches", "dfft_plan_exchange", "dfft_plan_fused", "dfft_plan_pipeline_parts", "dfft_plan_tma_mask", "dfft_plan_pipeline_chain"):
         getattr(L, name).argtypes = [vp]
     L.dfft_execute_stage.argtypes = [vp, i]
@@ -252,6 +255,11 @@ class Plan:
     def execute(self):
         _check(lib().dfft_execute(self.handle), "fft_mpi_execute_dft_3d_c2c")
 
+    def execute_convolve(self, mult_ptr):
+        """convolve plans: out = inverse(m .* forward(bufferDev1)) with the multiplier at `mult_ptr` (see
+        fft_mpi_plan_dft_convolve_3d)"""
+        _check(lib().dfft_execute_convolve(self.handle, mult_ptr), "dfft_execute_convolve")
+
     def execute_stage(self, stage):
         _check(lib().dfft_execute_stage(self.handle, stage), "dfft_execute_stage")
 
@@ -348,6 +356,19 @@ def fft_mpi_plan_dft_r2c_3d(n0, n1, n2, in_ptr, out_ptr, comm, devIdx, totalDevC
     ch = comm.handle if comm is not None else None
     _check(lib().dfft_plan_r2c_3d(n0, n1, n2, in_ptr, out_ptr, ch, devIdx, totalDevCount, direction, precision, flags, ctypes.byref(h)),
            "fft_mpi_plan_dft_r2c_3d")
+    return Plan(h)
+
+
+def fft_mpi_plan_dft_convolve_3d(n0, n1, n2, in_ptr, out_ptr, comm, devIdx, totalDevCount, precision=DOUBLE, flags=0, real=False):
+    """Spectral convolution plan (dfft_plan_convolve_c2c_3d / dfft_plan_convolve_r2c_3d): Plan.execute_convolve(mult_ptr) computes
+    out = ifftn(fftn(in) * m), unnormalised (x n0*n1*n2) unless SCALE_BACKWARD, or with real=True
+    out = irfftn(rfftn(in) * m, s=(n0, n1, n2)) * n0*n1*n2 on real slabs.  `in_ptr` / `out_ptr` hold exactly this device's x-slab
+    [x_l][y][z] (out_ptr None or == in_ptr: in place).  The complex multiplier is m[x][y_l][z'] in natural order over this
+    device's y-slab (fft_mpi_local_size_3d), z' < n2, or n2//2+1 with real=True."""
+    h = ctypes.c_void_p()
+    ch = comm.handle if comm is not None else None
+    fn = lib().dfft_plan_convolve_r2c_3d if real else lib().dfft_plan_convolve_c2c_3d
+    _check(fn(n0, n1, n2, in_ptr, out_ptr, ch, devIdx, totalDevCount, precision, flags, ctypes.byref(h)), "fft_mpi_plan_dft_convolve_3d")
     return Plan(h)
 
 

@@ -441,7 +441,7 @@ struct dfft_plan_s {
     int lag = 0;
     unsigned long long* plane_done = nullptr;
     unsigned int* ticket = nullptr;
-    unsigned long long fuse_epoch = 0;
+    unsigned long long fuse_epoch = 0;   // plane_done value every plane reaches once the last fused launch is done (sum of its GA)
     // describe-only plans (DFFT_DRY_RUN): no CUDA call is made, buffers are symbolic addresses, execute records the
     // passes it would launch (dfft_debug_plan_ops) -- lets the CPU tests interpret the whole multi-device schedule
     bool dry = false;
@@ -471,6 +471,14 @@ struct dfft_plan_s {
     bool r2c = false;
     long long n2r = 0;
     size_t in_esz = 16, out_esz = 16;
+    // spectral convolution plans (dfft_plan_convolve_*): forward half, fused X pass (forward x, multiply, inverse x), backward half.
+    // `direction` is switched to the half being issued, so that every pass helper takes its inverse flag and its t0 kernels from it
+    bool conv = false;
+    bool conv_fuse[2] = {false, false};   // fused t0 of the forward [0] / backward [1] half, chosen as a C2C plan of that direction would
+    bool conv_fuse_tma = false;           // the forward half's t0 is the TMA fused kernel
+    int phase_base = 0;                   // DRY_RUN: added to the recorded phases (the backward half of a convolve plan records from 2)
+    void* work2 = nullptr;                // P2P convolve: the backward exchange's receive buffer (the peers store into it while this
+    std::vector<void*> peer_work2;        // device may still be reading `work`)
 };
 
 // symbolic device address of a describe-only plan: device d (0-based), buffer id b: 1 bufferDev1, 2 bufferDev2 / user out,
@@ -543,7 +551,7 @@ static int share_pointer(dfft_plan p, void* mine, std::vector<void*>& peers)
 }
 
 static int plan_create(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
-                       int P, int direction, int precision, unsigned flags, dfft_plan* plan_out, bool real = false);
+                       int P, int direction, int precision, unsigned flags, dfft_plan* plan_out, bool real = false, bool conv = false);
 
 extern "C" int dfft_plan_c2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
                                 int P, int direction, int precision, unsigned flags, dfft_plan* plan_out)
@@ -563,6 +571,22 @@ extern "C" int dfft_plan_r2c_3d(long long n0, long long n1, long long n2, void* 
     return rc;
 }
 
+extern "C" int dfft_plan_convolve_c2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
+                                         int P, int precision, unsigned flags, dfft_plan* plan_out)
+{
+    const int rc = plan_create(n0, n1, n2, in, out, comm, dev_idx, P, DFFT_FORWARD, precision, flags, plan_out, false, true);
+    if (rc != 0 && P > 1 && comm && comm->local && !(flags & DFFT_DRY_RUN)) comm->poison();
+    return rc;
+}
+
+extern "C" int dfft_plan_convolve_r2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
+                                         int P, int precision, unsigned flags, dfft_plan* plan_out)
+{
+    const int rc = plan_create(n0, n1, n2, in, out, comm, dev_idx, P, DFFT_FORWARD, precision, flags, plan_out, true, true);
+    if (rc != 0 && P > 1 && comm && comm->local && !(flags & DFFT_DRY_RUN)) comm->poison();
+    return rc;
+}
+
 extern "C" int dfft_local_size_r2c_3d(long long n0, long long n1, long long n2, int P, int dev, long long* real_count, long long* complex_count)
 {
     if (P < 1 || dev < 0 || dev >= P || n0 < 1 || n1 < 1 || n2 < 1) return fail(DFFT_EINVAL, "dfft_local_size_r2c_3d: bad arguments");
@@ -574,17 +598,22 @@ extern "C" int dfft_local_size_r2c_3d(long long n0, long long n1, long long n2, 
 }
 
 static int plan_create(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
-                       int P, int direction, int precision, unsigned flags, dfft_plan* plan_out, bool real)
+                       int P, int direction, int precision, unsigned flags, dfft_plan* plan_out, bool real, bool conv)
 {
+    const char* what = conv ? (real ? "dfft_plan_convolve_r2c_3d" : "dfft_plan_convolve_c2c_3d") : (real ? "dfft_plan_r2c_3d" : "dfft_plan_c2c_3d");
     if (!plan_out) return fail(DFFT_EINVAL, "null plan pointer");
     *plan_out = nullptr;
     if (n0 < 1 || n1 < 1 || n2 < 1 || P < 1 || dev_idx < 0 || dev_idx >= P || !in)
-        return fail(DFFT_EINVAL, real ? "dfft_plan_r2c_3d: bad arguments" : "dfft_plan_c2c_3d: bad arguments");
+        return fail(DFFT_EINVAL, "%s: bad arguments", what);
     if (direction != DFFT_FORWARD && direction != DFFT_BACKWARD) return fail(DFFT_EINVAL, "direction must be +1 or -1");
     if (precision != DFFT_DOUBLE && precision != DFFT_FLOAT) return fail(DFFT_EINVAL, "bad precision");
     if (P > DFFT_MAX_CHUNKS) return fail(DFFT_EUNSUPPORTED, "at most %d devices", DFFT_MAX_CHUNKS);
     const bool dry = (flags & DFFT_DRY_RUN) != 0;
-    if (real) {
+    if (conv) {
+        // a convolve plan exposes no spectrum, and its two exchanges are folded into its kernels or handed to NCCL
+        if (flags & DFFT_NATURAL_SPECTRUM) return fail(DFFT_EINVAL, "%s: DFFT_NATURAL_SPECTRUM has no meaning for a convolve plan (no spectrum is exposed)", what);
+        if ((flags & DFFT_EXCHANGE_MASK) == DFFT_EXCHANGE_STAGED) return fail(DFFT_EUNSUPPORTED, "%s: DFFT_EXCHANGE_STAGED is not supported", what);
+    } else if (real) {
         // the real and the complex slab differ in size and layout: no in-place (padded) layout, no stage-by-stage mode
         if (!out || out == in) return fail(DFFT_EINVAL, "dfft_plan_r2c_3d: `out` must be a separate buffer (in-place R2C is not supported)");
         if ((flags & DFFT_EXCHANGE_MASK) == DFFT_EXCHANGE_STAGED) return fail(DFFT_EUNSUPPORTED, "R2C / C2R plans do not support DFFT_EXCHANGE_STAGED");
@@ -600,15 +629,19 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
         return fail(DFFT_EUNSUPPORTED, "unsupported transform length in %lldx%lldx%lld (see dfft_supported_lengths)", n0, n1, n2);
     if (real && (ez->gen || !ez->launch[PK_Z_R2C] || !ez->launch[PK_Z_C2R]))
         return fail(DFFT_EUNSUPPORTED, "R2C / C2R needs a z length with a tuned kernel (dfft_length_kind == 2); %lld has none", n2);
+    if (conv && (ex->gen || !ex->launch[PK_XCONV] || !ex->launch[PK_XCONV_CO]))
+        return fail(DFFT_EUNSUPPORTED, "%s: the x length %lld has no convolution kernel (it needs a tuned length, dfft_length_kind == 2, of the default kernel table)", what, n0);
     // bufferDev2 (`out`, or `in` in place) is written by the pass kernels; an out-of-place `in` is only copied (cudaMemcpy).
     // TMA needs 16-byte-aligned global addresses, and so do the fp64 kernels' double2 accesses: such a buffer is rejected in
     // fp64, and in fp32 (float2 accesses, 8 bytes) it keeps the plan on the register-staged kernels.  R2C plans apply the rule
     // to their complex-side buffer (forward `out`, backward `in`); the real side only needs the alignment of its element type
+    // A real convolve plan keeps every complex array in plan-owned buffers: its user buffers only need their element alignment
     const void* cbuf = real ? (direction == DFFT_FORWARD ? out : in) : ((!out || out == in) ? in : out);
-    const bool buf2_aligned = ((uintptr_t)cbuf & 15) == 0;
+    const bool buf2_aligned = (real && conv) || ((uintptr_t)cbuf & 15) == 0;
     if (precision == DFFT_DOUBLE && !buf2_aligned) return fail(DFFT_EINVAL, "a double-precision output buffer must be 16-byte aligned");
     const size_t rsz = precision == DFFT_FLOAT ? 4 : 8;
-    if (real && ((uintptr_t)(direction == DFFT_FORWARD ? in : out) % rsz) != 0) return fail(DFFT_EINVAL, "the real buffer is not aligned to its element size");
+    if (real && !conv && ((uintptr_t)(direction == DFFT_FORWARD ? in : out) % rsz) != 0) return fail(DFFT_EINVAL, "the real buffer is not aligned to its element size");
+    if (real && conv && (((uintptr_t)in % rsz) != 0 || (out && ((uintptr_t)out % rsz) != 0))) return fail(DFFT_EINVAL, "the real buffers are not aligned to their element size");
 
     dfft_plan p = new dfft_plan_s;
     p->g = g; p->P = P; p->me = dev_idx; p->direction = direction; p->prec = precision; p->flags = flags;
@@ -624,6 +657,12 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
         const long long rcount = p->n0l * n1 * n2;
         if (direction == DFFT_FORWARD) { p->in_count = rcount; p->in_esz = rsz; }
         else { p->out_count = rcount; p->out_esz = rsz; }
+    }
+    if (conv) {
+        // input and output are both exactly this device's x-slab
+        p->conv = true;
+        p->in_count = p->out_count = p->n0l * n1 * n2;
+        p->in_esz = p->out_esz = real ? rsz : p->esz;
     }
     p->ez = ez; p->ey = ey; p->ex = ex; p->comm = comm;
     p->in = in; p->out = out;
@@ -646,7 +685,8 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
     if (dry) p->buf1 = fake_addr(dev_idx, 1);
     else {
         // R2C: bufferDev1 holds exactly the input slab (the user's buffer has only that many elements of its type)
-        const size_t b1 = p->r2c ? (size_t)p->in_count * p->in_esz : (size_t)p->max_count * p->esz;
+        // convolve plans: the user's buffers are exactly the x-slab as well
+        const size_t b1 = (p->r2c || conv) ? (size_t)p->in_count * p->in_esz : (size_t)p->max_count * p->esz;
         CUP(cudaMalloc(&p->buf1, b1));
         CUP(cudaMemcpy(p->buf1, in, b1, cudaMemcpyDeviceToDevice));
         CUP(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
@@ -663,6 +703,10 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
         CUP(upload_lut<float>(&p->lut_z, ez->z_nstages, ez->z_rad));
         CUP(upload_lut<float>(&p->lut_y, ey->s_nstages, ey->s_rad));
         CUP(upload_lut<float>(&p->lut_x, ex->x_nstages, ex->x_rad));
+    }
+    if (conv && !dry) {   // the fused X pass runs the x entry's strided schedule (as the natural-order X pass does)
+        if (precision == DFFT_DOUBLE) CUP(upload_lut<double>(&p->lut_xn, ex->s_nstages, ex->s_rad));
+        else CUP(upload_lut<float>(&p->lut_xn, ex->s_nstages, ex->s_rad));
     }
     if (!dry) CUP(cudaGetLastError());
     if (!dry && !(flags & DFFT_NO_TMA) && buf2_aligned) {
@@ -731,17 +775,28 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
         // instantiated and measured (TmaEntry::use bit TMA_USE_ZY, DESIGN.md 3.4): it is the default forward t0 there.
         // Forced fusion takes the TMA kernel whenever one exists, the register-staged kernel otherwise.
         const char* env = getenv("DFFT_FUSE");
-        const bool tma_zy = P == 1 && direction == DFFT_FORWARD && n1 == n2 && !dry && p->tz && p->tz->fused_zy != nullptr && n2 % p->tz->C == 0;
-        // the register-staged kind this plan would launch (zy_fused, and the part kernels of the pipelined schedules) must exist:
-        // an entry leaves a kind null when its roles do not fit in shared memory together
-        const int kind = direction == DFFT_FORWARD ? (P == 1 ? FK_ZY : FK_ZY_CO) : (P == 1 ? FK_YZ : FK_YZ_CI);
-        const bool can = n1 == n2 && (ez->fused[kind] != nullptr || tma_zy);
-        bool want = (P > 1 && xmode == DFFT_EXCHANGE_P2P) || (tma_zy && (p->tz->use & (1u << TMA_USE_ZY)));
-        if (env) want = strcmp(env, "0") != 0;
-        if (flags & DFFT_FORCE_FUSE) want = true;
-        if (flags & DFFT_NO_FUSE) want = false;
-        p->fuse = can && want && !real;   // R2C: the real Z pass has no fused form; the fusion flags are accepted and do nothing
-        p->fuse_tma = p->fuse && tma_zy;
+        // t0 of one direction; a convolve plan selects each of its halves as the C2C plan of that direction would
+        auto pick = [&](int dir, bool& fuse, bool& fuse_tma) {
+            const bool tma_zy = P == 1 && dir == DFFT_FORWARD && n1 == n2 && !dry && p->tz && p->tz->fused_zy != nullptr && n2 % p->tz->C == 0;
+            // the register-staged kind this plan would launch (zy_fused, and the part kernels of the pipelined schedules) must exist:
+            // an entry leaves a kind null when its roles do not fit in shared memory together
+            const int kind = dir == DFFT_FORWARD ? (P == 1 ? FK_ZY : FK_ZY_CO) : (P == 1 ? FK_YZ : FK_YZ_CI);
+            const bool can = n1 == n2 && (ez->fused[kind] != nullptr || tma_zy);
+            bool want = (P > 1 && xmode == DFFT_EXCHANGE_P2P) || (tma_zy && (p->tz->use & (1u << TMA_USE_ZY)));
+            if (env) want = strcmp(env, "0") != 0;
+            if (flags & DFFT_FORCE_FUSE) want = true;
+            if (flags & DFFT_NO_FUSE) want = false;
+            fuse = can && want && !real;   // R2C: the real Z pass has no fused form; the fusion flags are accepted and do nothing
+            fuse_tma = fuse && tma_zy;
+        };
+        if (conv) {
+            bool unused = false;
+            pick(DFFT_FORWARD, p->conv_fuse[0], p->conv_fuse_tma);
+            pick(DFFT_BACKWARD, p->conv_fuse[1], unused);
+            p->fuse = p->conv_fuse[0] || p->conv_fuse[1];   // execute_convolve sets the flags of the half it issues
+        } else {
+            pick(direction, p->fuse, p->fuse_tma);
+        }
         if (getenv("DFFT_LAG")) p->lag = atoi(getenv("DFFT_LAG"));
         if (p->fuse && !dry) {
             CUP(cudaMalloc((void**)&p->plane_done, (size_t)p->n0l * sizeof(unsigned long long)));
@@ -758,7 +813,7 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
         // opt-in: the whole forward transform of a device as one kernel with t3 overlapped behind per-part arrivals
         const char* env = getenv("DFFT_OVERLAP");
         const bool want = (flags & DFFT_OVERLAP_X) || (env && strcmp(env, "0") != 0);
-        if (want && P > 1 && xmode == DFFT_EXCHANGE_P2P && direction == DFFT_FORWARD && p->fuse && ez->fused3 && ex == ez) {
+        if (want && !conv && P > 1 && xmode == DFFT_EXCHANGE_P2P && direction == DFFT_FORWARD && p->fuse && ez->fused3 && ex == ez) {
             const int cy = ez->p_C, cx_ = ez->x_C;
             int lcm = cy > cx_ ? cy : cx_;   // both are powers of two in the tuned tables
             if (lcm % cy == 0 && lcm % cx_ == 0) {
@@ -793,7 +848,7 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
         //    Default from 4 devices on for axes >= 1024 points, where the X pass that it hides is long enough to pay for the
         //    extra launches and the second read of the intermediate.
         // DFFT_FORCE_PIPELINE / DFFT_PIPELINE=1 pipeline wherever it is possible, DFFT_NO_PIPELINE / DFFT_PIPELINE=0 never.
-        const bool possible = P > 1 && !p->overlap && !real && (xmode == DFFT_EXCHANGE_P2P || xmode == DFFT_EXCHANGE_NCCL);
+        const bool possible = P > 1 && !p->overlap && !real && !conv && (xmode == DFFT_EXCHANGE_P2P || xmode == DFFT_EXCHANGE_NCCL);
         const bool chain_ok = direction == DFFT_FORWARD && xmode == DFFT_EXCHANGE_P2P && p->fuse && ey == ex && ey->fused_yx != nullptr;
         bool want = possible && chain_ok && P >= 4 && n2 >= 1024;
         if (env) want = possible && strcmp(env, "0") != 0;
@@ -843,18 +898,27 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
             }
         }
     }
-    if (real && P > 1) {
-        // R2C scratch where the C2C schedules borrow `out`: the forward Z output / NCCL send buffer, the backward Y output
+    if ((real || conv) && P > 1) {
+        // R2C and convolve scratch where the C2C schedules borrow `out`: the forward Z output / NCCL send buffer, the backward Y output
         if (dry) p->mid = fake_addr(dev_idx, 4);
         else CUP(cudaMalloc(&p->mid, (size_t)p->max_count * p->esz));
+    }
+    if (conv && P > 1 && xmode == DFFT_EXCHANGE_P2P) {
+        if (dry) p->work2 = fake_addr(dev_idx, 7);
+        else CUP(cudaMalloc(&p->work2, (size_t)p->max_count * p->esz));
     }
     if (P > 1 && dry) {
         p->peer_work.resize(P);
         for (int q = 0; q < P; q++) p->peer_work[q] = fake_addr(q, 3);
+        if (p->work2) {
+            p->peer_work2.resize(P);
+            for (int q = 0; q < P; q++) p->peer_work2[q] = fake_addr(q, 7);
+        }
     } else if (P > 1) {
         if (xmode == DFFT_EXCHANGE_P2P || xmode == DFFT_EXCHANGE_STAGED) {
             if (xmode == DFFT_EXCHANGE_P2P) {
                 if ((rc = share_pointer(p, p->work, p->peer_work)) != 0) return bail(rc);
+                if (p->work2 && (rc = share_pointer(p, p->work2, p->peer_work2)) != 0) return bail(rc);
             } else {
                 if ((rc = share_pointer(p, p->buf1, p->peer_buf1)) != 0) return bail(rc);
             }
@@ -902,6 +966,7 @@ extern "C" int dfft_destroy(dfft_plan p)
     if (p->P > 1 && p->comm && !p->comm->local && !p->ipc_opened.empty()) p->comm->host_barrier(p->me);
     if (p->buf1) cudaFree(p->buf1);
     if (p->work) cudaFree(p->work);
+    if (p->work2) cudaFree(p->work2);
     if (p->sync) cudaFree(p->sync);
     if (p->stream2) cudaStreamSynchronize(p->stream2);
     if (p->stream3) cudaStreamSynchronize(p->stream3);
@@ -977,7 +1042,7 @@ template <typename T> struct Pass {
             const int C = kind == PK_Z ? e->z_C : (kind == PK_Y || kind == PK_Y_CI ? e->s_C : (kind == PK_Y_CO ? e->p_C : e->x_C));
             // phase 1 = runs after the exchange has delivered this device's receive buffer
             const bool fwd = p->direction == DFFT_FORWARD;
-            const int phase = fwd ? (axis == 2 ? 1 : 0) : (axis == 2 ? 0 : 1);
+            const int phase = p->phase_base + (fwd ? (axis == 2 ? 1 : 0) : (axis == 2 ? 0 : 1));
             record_op<T>(p, names[kind], phase, e->N, C, kind == PK_Y_CI, kind == PK_Y_CO || kind == PK_XB_CO, kind == PK_XF || kind == PK_XF_TW, a);
             p->launches++;
             return 0;
@@ -1057,7 +1122,7 @@ template <typename T> struct Pass {
         const int kind = fwd ? PK_Z_R2C : PK_Z_C2R;
         if (p->dry) {
             // real-side maps are in real elements; "pair" = distance between the two lines of a pair (input side, output side)
-            record_op<T>(p, fwd ? "Z_R2C" : "Z_C2R", fwd ? 0 : 1, (int)N, C, false, false, false, a);
+            record_op<T>(p, fwd ? "Z_R2C" : "Z_C2R", p->phase_base + (fwd ? 0 : 1), (int)N, C, false, false, false, a);
             char buf[128];
             snprintf(buf, sizeof(buf), ", \"nzh\": %lld, \"pair\": [%lld, %lld]}", H, r.ld_in, r.ld_out);
             p->ops.back().pop_back();
@@ -1124,14 +1189,15 @@ template <typename T> struct Pass {
         FusedCtl c{};
         c.plane_done = p->plane_done; c.ticket = p->ticket; c.planes = p->n0l;
         c.GA = fwd ? z.G : y.G; c.GB = fwd ? y.G : z.G;
-        c.target = ++p->fuse_epoch * (unsigned long long)c.GA;
+        c.target = p->fuse_epoch += (unsigned long long)c.GA;
         c.lag = p->lag;
         const int kind = fwd ? (ymode == 1 ? FK_ZY_CO : FK_ZY) : (ymode == 2 ? FK_YZ_CI : FK_YZ);
         apply_fold<T>(p, fwd ? y : z, fold);   // fft_fused2_kernel gates on / signals through its second role's arguments
         if (p->dry) {
             z.gen = y.gen = nullptr;
-            if (fwd) { record_op<T>(p, "fusedZ", 0, e->N, CZ, false, false, false, z); record_op<T>(p, "fusedY", 0, e->N, CY, false, ymode == 1, false, y); }
-            else { record_op<T>(p, "fusedY", 1, e->N, CY, ymode == 2, false, false, y); record_op<T>(p, "fusedZ", 1, e->N, CZ, false, false, false, z); }
+            const int ph = p->phase_base;
+            if (fwd) { record_op<T>(p, "fusedZ", ph, e->N, CZ, false, false, false, z); record_op<T>(p, "fusedY", ph, e->N, CY, false, ymode == 1, false, y); }
+            else { record_op<T>(p, "fusedY", ph + 1, e->N, CY, ymode == 2, false, false, y); record_op<T>(p, "fusedZ", ph + 1, e->N, CZ, false, false, false, z); }
             p->launches++;
             return 0;
         }
@@ -1157,7 +1223,7 @@ template <typename T> struct Pass {
         FusedCtl c{};
         c.plane_done = p->plane_done; c.ticket = p->ticket; c.planes = p->n0l;
         c.GA = (int)(g.n1 / e->C); c.GB = (int)(g.n2 / e->C);
-        c.target = ++p->fuse_epoch * (unsigned long long)c.GA;
+        c.target = p->fuse_epoch += (unsigned long long)c.GA;
         c.lag = p->lag;
         ev_record(p, p->pev[0][0]);
         cudaError_t err = e->fused_zy(&a, &c, mm, p->sms, p->stream);
@@ -1193,7 +1259,7 @@ template <typename T> struct Pass {
         c.planes = p->n0l; c.rows = p->n1l; c.P = p->P; c.me = p->me;
         c.K = p->parts;
         c.GA = z.G; c.GB = y.G; c.GBk = y.G / c.K; c.GX = x.G; c.GXk = x.G / c.K;
-        c.target = ++p->fuse_epoch * (unsigned long long)c.GA;
+        c.target = p->fuse_epoch += (unsigned long long)c.GA;
         c.epoch = ++p->overlap_epoch;
         c.part_target = c.epoch * (unsigned long long)(p->n0l * c.GBk);
         if (!p->dry) {
@@ -1296,7 +1362,7 @@ template <typename T> struct Pass {
         FusedCtl c{};
         c.plane_done = p->plane_done; c.ticket = p->ticket; c.planes = p->n0l;
         c.GA = z.G; c.GB = y.G;
-        c.target = ++p->fuse_epoch * (unsigned long long)c.GA;
+        c.target = p->fuse_epoch += (unsigned long long)c.GA;
         c.lag = p->lag;
         if (p->dry) {
             record_op<T>(p, "fusedZ", 0, e->N, CZ, false, false, false, z);
@@ -1416,7 +1482,7 @@ template <typename T> struct Pass {
         FusedCtl c{};
         c.plane_done = p->plane_done; c.ticket = p->ticket; c.planes = p->n0l;
         c.GA = y.G; c.GB = z.G;
-        c.target = ++p->fuse_epoch * (unsigned long long)c.GA;
+        c.target = p->fuse_epoch += (unsigned long long)c.GA;
         c.lag = p->lag;
         if (p->dry) {
             record_op<T>(p, "fusedY", 1, e->N, CY, true, false, false, y);
@@ -1452,6 +1518,43 @@ template <typename T> struct Pass {
         }
         if (chunk_base) apply_fold<T>(p, a, fold);
         return launch(p, p->ex, chunk_base ? PK_XB_CO : PK_XB, a);
+    }
+    // fused X pass of a convolve plan (fft_conv_kernel): the [x][y_l][z'] columns of src, transformed along x, multiplied by
+    // mult (same layout), transformed back -> dst in the same layout, or (chunk_base) split by xd into the destinations' receive
+    // buffers [x_l][y_l(me)][z'] as x_bwd's chunked store does.  DFFT_SCALE_BACKWARD's 1/N rides on the multiply
+    static int x_conv(dfft_plan p, const void* src, void* dst, void* const* chunk_base, const void* mult, const Fold* fold = nullptr)
+    {
+        const Geom& g = p->g;
+        const bool co = chunk_base != nullptr;
+        const int C = co ? p->ex->p_C : p->ex->s_C;
+        ConvArgs<T> r{};
+        TileArgs<T>& a = r.t;
+        a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)p->lut_xn;
+        a.G = (int)cdiv(g.n2, C); a.W = (int)g.n2; a.ntiles = p->n1l * a.G;
+        a.ia = Affine{g.n2, C, 1, p->n1l * g.n2}; a.oa = a.ia;
+        const double n2 = p->r2c ? (double)p->n2r : (double)g.n2;
+        a.do_scale = (p->flags & DFFT_SCALE_BACKWARD) ? 1 : 0; a.scale = (T)(1.0 / ((double)g.n0 * (double)g.n1 * n2));
+        if (co) {
+            a.co.ediv = (int)g.xd(); a.co.nchunks = p->P;
+            for (int q = 0; q < p->P; q++) { a.co.cptr[q] = chunk_base[q]; a.co.SAq[q] = g.n2; }
+        }
+        r.mult = (const cx<T>*)mult;
+        apply_fold<T>(p, a, fold);
+        if (p->dry) {
+            record_op<T>(p, co ? "XCONV_CO" : "XCONV", 1, p->ex->N, C, false, co, false, a);
+            char buf[64];
+            snprintf(buf, sizeof(buf), ", \"mult\": %llu}", (unsigned long long)(size_t)mult);
+            p->ops.back().pop_back();
+            p->ops.back() += buf;
+            p->launches++;
+            return 0;
+        }
+        ev_record(p, p->pev[2][0]);
+        cudaError_t err = p->ex->launch[co ? PK_XCONV_CO : PK_XCONV](&r, p->sms, p->stream);
+        ev_record(p, p->pev[2][1]);
+        if (err != cudaSuccess) return fail(DFFT_ECUDA, "convolution X pass launch (N=%d) failed: %s", p->ex->N, cudaGetErrorString(err));
+        p->launches++;
+        return 0;
     }
 };
 
@@ -1516,7 +1619,7 @@ static int nccl_exchange(dfft_plan p, const void* sendbuf, void* recvbuf)
     const int dir = p->direction;
     if (p->dry) {   // describe the all-to-all: element offsets and counts of every chunk this device sends
         char buf[160];
-        std::string o = "{\"op\": \"alltoall\", \"phase\": 0, ";
+        std::string o = "{\"op\": \"alltoall\", \"phase\": " + std::to_string(p->phase_base) + ", ";
         snprintf(buf, sizeof(buf), "\"send\": %llu, \"recv\": %llu, \"esz\": %zu, \"chunks\": [", (unsigned long long)(size_t)sendbuf,
                  (unsigned long long)(size_t)recvbuf, p->esz);
         o += buf;
@@ -1962,6 +2065,132 @@ template <typename T> static int execute_real(dfft_plan p)
     return 0;
 }
 
+// Convolve plans: out = IFFT3(m .* FFT3(in)), never writing bufferDev1.  The forward half is the C2C (R2C) forward schedule up to
+// the arrival of the receive buffer [x][y_l][z'], the fused X pass (fft_conv_kernel) replaces the forward X pass, the multiply and
+// the backward X pass, and the backward half is the C2C (C2R) backward schedule from the exchange on.  Buffers:
+//   P = 1 : work (forward t0 out, fused X pass in place, backward t0 in); bufferDev2 (= out) gets the result
+//   NCCL  : work = both exchanges' receive buffer, mid = forward send buffer, fused X pass output (already grouped by destination:
+//           it is the backward send buffer) and, R2C, the backward Y output
+//   P2P   : work = forward receive buffer, work2 = backward receive buffer (the fused X pass stores into the peers' work2),
+//           mid = forward Z output and, R2C, the backward Y output
+// Epochs (P2P): execute k uses e1 = 2k+1 for the forward exchange and e2 = 2k+2 for the backward one; arrive[s] takes e1 then e2
+// from sender s, ready[r] takes e2 once receiver r's backward Y pass has read its work2.  No device writes a peer buffer before
+// the owner has finished reading that buffer's previous contents:
+//   * the forward Y stores into peer r's work wait for ready[r] >= e1 - 1 (= e2 of the previous execute): r's backward Y pass of
+//     the previous execute is done, and with it r's fused X pass, the only reader of r's work;
+//   * the fused X pass stores into peer r's work2 behind the same gate (it runs later on the same stream): r's backward Y pass of
+//     the previous execute, the only reader of r's work2, is done;
+//   * the waits are >= tests on monotonic words: the previous execute's e2 (= e1 - 1) never satisfies the wait for e1, and a sender
+//     publishes e2 only from its fused X pass, after every store of its forward Y pass.
+template <typename T> static int execute_convolve(dfft_plan p, const void* mult)
+{
+    const Geom& g = p->g;
+    const int P = p->P, me = p->me;
+    const bool p2p = p->xmode == DFFT_EXCHANGE_P2P;
+    int rc;
+    struct Half {
+        dfft_plan p;
+        void set(int h) {   // h = 0 forward half, 1 backward half, -1 between executes
+            p->direction = h == 1 ? DFFT_BACKWARD : DFFT_FORWARD;
+            p->fuse = h < 0 ? (p->conv_fuse[0] || p->conv_fuse[1]) : p->conv_fuse[h];
+            p->fuse_tma = h == 0 && p->conv_fuse_tma;
+            p->phase_base = h == 1 ? 2 : 0;
+        }
+        ~Half() { set(-1); }
+    } half{p};
+    p->launches = 0;
+    CU(ev_record(p, p->ev[0]));
+    half.set(0);
+    const bool fold = p2p && p->done_ctr != nullptr && !p->dry;   // completion signals inside the pass kernels, as in execute_fused
+    unsigned long long e1 = 0, e2 = 0;
+    void* base[DFFT_MAX_CHUNKS];
+    if (P == 1) {
+        if (p->r2c) {
+            if ((rc = Pass<T>::z_real(p, p->buf1, p->work, false))) return rc;
+            if ((rc = Pass<T>::y_pass(p, p->work, p->work, 0, nullptr))) return rc;
+        } else if (p->fuse_tma) {
+            if ((rc = Pass<T>::zy_fused_tma(p, p->buf1, p->work))) return rc;
+        } else if (p->fuse) {
+            if ((rc = Pass<T>::zy_fused(p, p->buf1, p->work, p->work, 0, nullptr, false))) return rc;
+        } else {
+            if ((rc = Pass<T>::z_pass(p, p->buf1, p->work, false))) return rc;
+            if ((rc = Pass<T>::y_pass(p, p->work, p->work, 0, nullptr))) return rc;
+        }
+    } else if (p2p) {
+        e1 = ++p->epoch;
+        e2 = ++p->epoch;
+        for (int q = 0; q < P; q++) base[q] = eoff(p->peer_work[q], recv_off(g, me, q, DFFT_FORWARD), p->esz);
+        Fold fy; fy.sig_which = 1; fy.sig_val = e1; fy.ctr = 0;
+        if (p->r2c) {
+            if ((rc = Pass<T>::z_real(p, p->buf1, p->mid, false))) return rc;
+            if ((rc = flags_wait(p, 0, e1 - 1))) return rc;
+            if ((rc = Pass<T>::y_pass(p, p->mid, nullptr, 1, base, fold ? &fy : nullptr))) return rc;
+        } else if (p->fuse) {
+            if ((rc = flags_wait(p, 0, e1 - 1))) return rc;
+            if ((rc = Pass<T>::zy_fused(p, p->buf1, p->mid, nullptr, 1, base, false, fold ? &fy : nullptr))) return rc;
+        } else {
+            if ((rc = Pass<T>::z_pass(p, p->buf1, p->mid, false))) return rc;
+            if ((rc = flags_wait(p, 0, e1 - 1))) return rc;
+            if ((rc = Pass<T>::y_pass(p, p->mid, nullptr, 1, base, fold ? &fy : nullptr))) return rc;
+        }
+        if (!fold && (rc = flags_signal(p, 1, e1))) return rc;
+        if ((rc = flags_wait(p, 1, e1))) return rc;
+    } else {
+        for (int q = 0; q < P; q++) base[q] = eoff(p->mid, send_off(g, me, q, DFFT_FORWARD), p->esz);
+        if (p->r2c) {
+            if ((rc = Pass<T>::z_real(p, p->buf1, p->work, false))) return rc;
+            if ((rc = Pass<T>::y_pass(p, p->work, nullptr, 1, base))) return rc;
+        } else if (p->fuse) {
+            if ((rc = Pass<T>::zy_fused(p, p->buf1, p->work, nullptr, 1, base, false))) return rc;
+        } else {
+            if ((rc = Pass<T>::z_pass(p, p->buf1, p->work, false))) return rc;
+            if ((rc = Pass<T>::y_pass(p, p->work, nullptr, 1, base))) return rc;
+        }
+        if ((rc = nccl_exchange(p, p->mid, p->work))) return rc;
+    }
+    CU(ev_record(p, p->ev[1]));
+    if (P == 1) {
+        if ((rc = Pass<T>::x_conv(p, p->work, p->work, nullptr, mult))) return rc;
+    } else if (p2p) {
+        for (int q = 0; q < P; q++) base[q] = eoff(p->peer_work2[q], recv_off(g, me, q, DFFT_BACKWARD), p->esz);
+        Fold fc; fc.sig_which = 1; fc.sig_val = e2; fc.ctr = 1;
+        if ((rc = Pass<T>::x_conv(p, p->work, nullptr, base, mult, fold ? &fc : nullptr))) return rc;
+        if (!fold && (rc = flags_signal(p, 1, e2))) return rc;
+    } else {
+        if ((rc = Pass<T>::x_conv(p, p->work, p->mid, nullptr, mult))) return rc;   // [x][y_l][z'] is grouped by destination
+    }
+    CU(ev_record(p, p->ev[2]));
+    half.set(1);
+    if (P == 1) {
+        if (p->r2c) {
+            if ((rc = Pass<T>::y_pass(p, p->work, p->work, 0, nullptr))) return rc;
+            if ((rc = Pass<T>::z_real(p, p->work, p->buf2, false))) return rc;
+        } else if (p->fuse) {
+            if ((rc = Pass<T>::zy_fused(p, p->work, p->buf2, nullptr, 0, nullptr, false))) return rc;
+        } else {
+            if ((rc = Pass<T>::y_pass(p, p->work, p->buf2, 0, nullptr))) return rc;
+            if ((rc = Pass<T>::z_pass(p, p->buf2, p->buf2, false))) return rc;
+        }
+    } else {
+        void* rbuf = p2p ? p->work2 : p->work;
+        if (p2p) { if ((rc = flags_wait(p, 1, e2))) return rc; }
+        else if ((rc = nccl_exchange(p, p->mid, p->work))) return rc;
+        void* cb[DFFT_MAX_CHUNKS];
+        for (int q = 0; q < P; q++) cb[q] = eoff(rbuf, (long long)q * p->n0l * g.yd() * g.n2, p->esz);
+        Fold fyz; fyz.sig_which = 0; fyz.sig_val = e2; fyz.ctr = 1;   // the fused kernel's last CTA signals "work2 consumed"
+        const bool fold_yz = fold && p->fuse && !p->r2c;
+        if (p->fuse && !p->r2c) {
+            if ((rc = Pass<T>::zy_fused(p, nullptr, p->buf2, nullptr, 2, cb, false, fold_yz ? &fyz : nullptr))) return rc;
+        } else if ((rc = Pass<T>::y_pass(p, nullptr, p->r2c ? p->mid : p->buf2, 2, cb))) return rc;
+        if (p2p && !fold_yz && (rc = flags_signal(p, 0, e2))) return rc;
+        if (p->r2c) { if ((rc = Pass<T>::z_real(p, p->mid, p->buf2, false))) return rc; }
+        else if (!p->fuse && (rc = Pass<T>::z_pass(p, p->buf2, p->buf2, false))) return rc;
+    }
+    CU(ev_record(p, p->ev[3]));
+    p->timed = true;
+    return 0;
+}
+
 // reference-like stage-by-stage execution (api.cpp:181-214 with its device-wide syncs)
 template <typename T> static int execute_stage(dfft_plan p, int stage)
 {
@@ -2009,6 +2238,7 @@ template <typename T> static int execute_stage(dfft_plan p, int stage)
 
 extern "C" int dfft_execute_stage(dfft_plan p, int stage)
 {
+    if (p && p->conv) return fail(DFFT_EINVAL, "dfft_execute_stage: a convolve plan runs with dfft_execute_convolve");
     if (p && p->r2c) return fail(DFFT_EUNSUPPORTED, "dfft_execute_stage: R2C / C2R plans have no stage-by-stage mode");
     if (!p || stage < 0 || stage > 3 || p->dry) return fail(DFFT_EINVAL, "dfft_execute_stage: bad arguments");
     if (p->xmode != DFFT_EXCHANGE_STAGED) return fail(DFFT_EINVAL, "dfft_execute_stage needs a plan created with DFFT_EXCHANGE_STAGED");
@@ -2019,6 +2249,7 @@ extern "C" int dfft_execute_stage(dfft_plan p, int stage)
 extern "C" int dfft_execute(dfft_plan p)
 {
     if (!p) return fail(DFFT_EINVAL, "null plan");
+    if (p->conv) return fail(DFFT_EINVAL, "dfft_execute: a convolve plan runs with dfft_execute_convolve");
     if (p->dry) p->ops.clear();
     else CU(cudaSetDevice(p->device));
     if (p->xmode == DFFT_EXCHANGE_STAGED) {
@@ -2034,6 +2265,17 @@ extern "C" int dfft_execute(dfft_plan p)
     }
     if (p->r2c) return p->prec == DFFT_DOUBLE ? execute_real<double>(p) : execute_real<float>(p);
     return p->prec == DFFT_DOUBLE ? execute_fused<double>(p) : execute_fused<float>(p);
+}
+
+extern "C" int dfft_execute_convolve(dfft_plan p, const void* multiplier)
+{
+    if (!p) return fail(DFFT_EINVAL, "null plan");
+    if (!p->conv) return fail(DFFT_EINVAL, "dfft_execute_convolve needs a plan from dfft_plan_convolve_c2c_3d / dfft_plan_convolve_r2c_3d");
+    if (!multiplier) return fail(DFFT_EINVAL, "dfft_execute_convolve: null multiplier");
+    if ((uintptr_t)multiplier % p->esz) return fail(DFFT_EINVAL, "dfft_execute_convolve: the multiplier is not aligned to its complex element size (%zu bytes)", p->esz);
+    if (p->dry) p->ops.clear();
+    else CU(cudaSetDevice(p->device));
+    return p->prec == DFFT_DOUBLE ? execute_convolve<double>(p, multiplier) : execute_convolve<float>(p, multiplier);
 }
 
 extern "C" int dfft_synchronize(dfft_plan p)
@@ -2056,6 +2298,13 @@ extern "C" int dfft_get_timings(dfft_plan p, double t[5])
         for (int s = 0; s < 4; s++) CU(cudaEventElapsedTime(&ms[s], p->ev[s], p->ev[s + 1]));
         if (p->direction == DFFT_BACKWARD) { std::swap(ms[0], ms[3]); std::swap(ms[1], ms[2]); }
         for (int s = 0; s < 4; s++) t[s] = ms[s];
+    } else if (p->conv) {
+        // convolve: t0 = forward half (its t0 and exchange), t3 = fused X pass, t2 = backward half (its exchange and t0)
+        float a, b, c;
+        CU(cudaEventElapsedTime(&a, p->ev[0], p->ev[1]));
+        CU(cudaEventElapsedTime(&b, p->ev[1], p->ev[2]));
+        CU(cudaEventElapsedTime(&c, p->ev[2], p->ev[3]));
+        t[0] = a; t[1] = 0; t[2] = c; t[3] = b;
     } else if (p->pipe) {
         // send side [start, last part issued] = t0 (+t1, + the sends); exposed exchange = from there until the last part has
         // arrived from every sender; t3 = the X pass of the last part (the earlier parts ran under t0)
@@ -2095,6 +2344,7 @@ extern "C" int dfft_get_pass_timings(dfft_plan p, double t[3])
 extern "C" int dfft_execute_host_async(dfft_plan p, const void* host_in, void* host_out)
 {
     if (!p || !host_in || !host_out || p->dry) return fail(DFFT_EINVAL, "bad arguments");
+    if (p->conv) return fail(DFFT_EINVAL, "dfft_execute_host: a convolve plan runs with dfft_execute_convolve");
     CU(cudaSetDevice(p->device));
     CU(cudaMemcpyAsync(p->buf1, host_in, (size_t)p->in_count * p->in_esz, cudaMemcpyHostToDevice, p->stream));
     int rc = dfft_execute(p);

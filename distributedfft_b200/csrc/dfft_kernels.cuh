@@ -21,6 +21,9 @@ enum PassKind {
     PK_XF_TW,      // PK_XF + four-step twiddle epilogue (first pass of a long 1-D transform)
     PK_Z_R2C,      // real lines -> half spectra, two lines per complex transform (fft_real.cuh; args = RealZArgs)
     PK_Z_C2R,      // half spectra -> real lines (fft_real.cuh; args = RealZArgs)
+    PK_XCONV,      // spectral convolution along x: forward, multiply, inverse in one column pass (fft_conv_kernel; args = ConvArgs),
+                   // strided local configuration, local store
+    PK_XCONV_CO,   // + chunked (peer) store split by xd, in the peer-store configuration
     PK_COUNT
 };
 

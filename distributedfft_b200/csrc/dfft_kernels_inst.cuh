@@ -64,6 +64,33 @@ cudaError_t launch_real(const void* vargs, int sm_count, cudaStream_t st)
     return cudaGetLastError();
 }
 
+// spectral convolution column pass (fft_conv_kernel): vargs is a ConvArgs<T>
+template <class S, typename T, int C, bool TW, bool CO, int MINB, bool PP>
+cudaError_t launch_conv(const void* vargs, int sm_count, cudaStream_t st)
+{
+    const ConvArgs<T>& a = *reinterpret_cast<const ConvArgs<T>*>(vargs);
+    auto kern = fft_conv_kernel<S, T, C, TW, CO, MINB, PP>;
+    constexpr size_t smem = TileSmem<S, T, C, PP>::bytes(CO);
+    static std::atomic<int> occ_cache[64];
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    int occ = occ_cache[dev & 63].load();
+    if (occ == 0) {
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, S::T * C, smem);
+        if (e != cudaSuccess) return e;
+        if (occ < 1) return cudaErrorLaunchOutOfResources;
+        occ_cache[dev & 63].store(occ);
+    }
+    if (a.t.ntiles <= 0) return cudaSuccess;
+    long long grid = (long long)sm_count * occ;
+    if (grid > a.t.ntiles) grid = a.t.ntiles;
+    kern<<<(unsigned)grid, S::T * C, smem, st>>>(a);
+    return cudaGetLastError();
+}
+
 template <class OpA, class OpB, typename T, int MINB>
 cudaError_t launch_fused(const void* va, const void* vb, const FusedCtl* ctl, int sm_count, cudaStream_t st)
 {
@@ -229,6 +256,9 @@ SizeEntry make_entry(int variant = 0)
         constexpr int MBI = Z::MB > 3 ? 3 : Z::MB;
         e.launch[PK_Z_R2C] = launch_real<ZS, T, Z::C, false, Z::MB, Z::PP, false>;
         e.launch[PK_Z_C2R] = launch_real<ZS, T, Z::C, false, MBI, Z::PP, true>;
+        // spectral convolution along x (the X axis of a convolve plan uses this entry's strided schedule and twiddle table)
+        e.launch[PK_XCONV] = launch_conv<SS, T, Y::C, Y::TW, false, Y::MB, Y::PP>;
+        e.launch[PK_XCONV_CO] = launch_conv<SS, T, PEER::C, PEER::TW, true, PEER::MB, PEER::PP>;
     }
     // fused two-pass kernels: the contiguous role is re-tiled so that both roles fill the same CTA
     constexpr int NT = SS::T * Y::C, NTP = SS::T * PEER::C;

@@ -421,6 +421,72 @@ __global__ void __launch_bounds__(S::T* C, MINB) fft_tile_kernel(const TileArgs<
 }
 
 // ------------------------------------------------------------------------------------------
+// Spectral convolution column pass: forward FFT along x, pointwise multiply, inverse FFT along x, in ONE pass over a tile of
+// x-columns (MAP_C on both sides).  The spectrum of a column never leaves the registers: after the last stage thread (t, c) holds
+// the points t + u*T of column c, exactly the points it loaded, so the multiplier element of each register is read through the
+// input map with the multiplier's own base (its layout is the receive buffer's [x][y_l][z']) and the inverse run starts from the
+// same register layout.  Unnormalised (x N per axis); TileArgs::do_scale folds 1/scale into the multiply.  TileArgs::inv is unused.
+// CHUNK_OUT: the store is split by x (ChunkTab co, the PK_XB_CO addressing) into the peers' receive buffers.
+// ------------------------------------------------------------------------------------------
+template <typename T> struct ConvArgs {
+    TileArgs<T> t;
+    const cx<T>* mult;
+};
+
+template <class S, typename T, int C, bool TWREG, bool CHUNK_OUT, int MINB, bool PINGPONG>
+__global__ void __launch_bounds__(S::T* C, MINB) fft_conv_kernel(const ConvArgs<T> R)
+{
+    static_assert(S::valid(), "bad schedule");
+    using Op = TileOp<S, T, C, MAP_C, MAP_C, TWREG, false, CHUNK_OUT, PINGPONG>;
+    constexpr int RR = S::R, TT = S::T;
+    const TileArgs<T>& A = R.t;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    typename Op::Ctx k;
+    Op::setup(A, smem_raw, smem_raw + Op::SM::exch_bytes, k);
+    cx<T> twr[Op::NTW];
+    Op::load_twiddles(k, twr);
+    wait_flags_at_start<T>(A);
+    const int t = k.t_in, c = k.c_in;   // MAP_C on both sides: t_out == t_in, c_out == c_in
+    const bool do_scale = A.do_scale != 0;
+    for (long long tile = blockIdx.x; tile < A.ntiles; tile += gridDim.x) {
+        const long long a = tile / A.G;
+        const int b = (int)(tile - a * A.G);
+        const bool ok = b * C + c < A.W;
+        const long long off = a * A.ia.SA + b * A.ia.SB + c * A.ia.cs + (long long)t * A.ia.es;
+        cx<T> v[RR];
+#pragma unroll
+        for (int u = 0; u < RR; u++) v[u] = ok ? ld_stream(A.in + off + (long long)u * TT * A.ia.es) : mk<T>(0, 0);
+        StageRunner<S, 0, T, C, MAP_C, MAP_C, TWREG, PINGPONG>::run(v, t, c, t, c, k.exch, k.pp, k.lut_s, twr, [] {});
+        // multiply, then the inverse as swap -> forward -> swap (the swap-in is folded into the multiply's result)
+#pragma unroll
+        for (int u = 0; u < RR; u++) {
+            cx<T> m = ok ? ld_stream(R.mult + off + (long long)u * TT * A.ia.es) : mk<T>(0, 0);
+            if (do_scale) { m.x *= A.scale; m.y *= A.scale; }
+            v[u] = cswap(cmul(v[u], m));
+        }
+        // the inverse run's first scatter reuses the exchange buffer: every thread's last gather of the forward run is done
+        __syncthreads();
+        StageRunner<S, 0, T, C, MAP_C, MAP_C, TWREG, PINGPONG>::run(v, t, c, t, c, k.exch, k.pp, k.lut_s, twr, [] {});
+        if (ok) {
+            if constexpr (!CHUNK_OUT) {
+                cx<T>* p = A.out + a * A.oa.SA + b * A.oa.SB + c * A.oa.cs + (long long)t * A.oa.es;
+#pragma unroll
+                for (int u = 0; u < RR; u++) st_stream(p + (long long)u * TT * A.oa.es, cswap(v[u]));
+            } else {
+                const long long o = b * A.oa.SB + c * A.oa.cs;
+#pragma unroll
+                for (int u = 0; u < RR; u++) {
+                    const int2 qe = k.etab_o[t + u * TT];
+                    cx<T>* p = reinterpret_cast<cx<T>*>(k.cptr_o[qe.x]) + a * k.saq_o[qe.x] + o + (long long)qe.y * A.oa.es;
+                    st_stream(p, cswap(v[u]));
+                }
+            }
+        }
+    }
+    signal_when_grid_done<T>(A);
+}
+
+// ------------------------------------------------------------------------------------------
 // Two dependent passes over the same planes in ONE persistent kernel (t0 = Z then Y forward, Y then Z
 // backward): the reference runs them as two launches per plane (fft_mpi_3d_api.cpp:496-502), we ran
 // them as two full HBM sweeps; here a plane's intermediate is produced and consumed while it is still

@@ -179,6 +179,32 @@ int dfft_plan_r2c_3d(long long n0, long long n1, long long n2, void* in, void* o
 /* element counts of one device: reals of its x-slab, complex elements of its half-spectrum slab */
 int dfft_local_size_r2c_3d(long long n0, long long n1, long long n2, int total_devices, int dev_idx,
                            long long* real_count, long long* complex_count);
+/* Spectral convolution plans: forward transform, pointwise multiply, inverse transform in one plan, with the multiply folded into
+ * one x-column pass (forward FFT along x, multiply, inverse FFT along x) so the spectrum never reaches memory in transposed order.
+ *   C2C: out = IFFT3( m .* FFT3(in) ), unnormalised (x n0*n1*n2) unless DFFT_SCALE_BACKWARD.
+ *   R2C: out = irfftn( m .* rfftn(in), s=(n0,n1,n2) ) * n0*n1*n2 (numpy's C2R convention), real in / real out.
+ * `in` and `out` are this device's x-slab [x_l][y][z], exactly local_n0*n1*n2 elements (complex for C2C, reals for R2C); the plan
+ * never touches anything past them.  Ownership as for the other plans: `in` is snapshotted into bufferDev1 at creation and every
+ * execute transforms that snapshot (refill it through dfft_plan_buffers for new data; it is never written); out == NULL or
+ * out == in means in place; creation, execute and destroy are collective when P > 1.
+ * The multiplier is given at each execute (one plan serves many multipliers): read-only, complex in the plan's precision, aligned to
+ * its element size, in NATURAL order over this device's y-slab: m[x][y_l][z'], x < n0, y_l < local_n1 starting at local_1_start
+ * (dfft_local_size_3d), z' < n2 (C2C) or n2/2+1 (R2C).  With one device that is the natural [x][y][z] array.
+ * Flags: DFFT_SCALE_BACKWARD, DFFT_EXCHANGE_AUTO / P2P / NCCL and DFFT_DRY_RUN (the multiplier is then a symbolic address too)
+ * are honoured; DFFT_NO_TMA, DFFT_NO_FUSE and DFFT_FORCE_FUSE select the forward and the backward t0 exactly as for C2C plans of
+ * the same shape; the pipeline and overlap flags are accepted and have no effect.
+ * DFFT_EUNSUPPORTED: DFFT_EXCHANGE_STAGED; an x length without a tuned kernel (dfft_length_kind(n0, precision) != 2) or a
+ * DFFT_VARIANT entry without the convolution kernels; y / z lengths the C2C (R2C) plan rejects.
+ * DFFT_EINVAL: DFFT_NATURAL_SPECTRUM (no spectrum is exposed); dfft_execute, dfft_execute_stage and dfft_execute_host* on a
+ * convolve plan; dfft_execute_convolve on any other plan; a null or misaligned multiplier.
+ * dfft_get_timings after dfft_execute_convolve: t[0] = forward half (its t0 and, P > 1, its exchange), t[1] = 0, t[2] = backward
+ * half (its exchange and t0), t[3] = the fused X pass, t[4] = total. */
+int dfft_plan_convolve_c2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
+                              int total_devices, int precision, unsigned flags, dfft_plan* plan);
+int dfft_plan_convolve_r2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
+                              int total_devices, int precision, unsigned flags, dfft_plan* plan);
+/* Asynchronous on the plan's stream, like dfft_execute; result in bufferDev2 (= out) */
+int dfft_execute_convolve(dfft_plan plan, const void* multiplier);
 /* fft_mpi_execute_dft_3d_c2c, fft_mpi_3d_api.cpp:181-214.  Asynchronous on the plan's stream;
  * dfft_synchronize() or dfft_get_timings() waits.  Result in bufferDev2 (= out). */
 int dfft_execute(dfft_plan plan);
