@@ -471,14 +471,18 @@ struct dfft_plan_s {
     bool r2c = false;
     long long n2r = 0;
     size_t in_esz = 16, out_esz = 16;
-    // spectral convolution plans (dfft_plan_convolve_*): forward half, fused X pass (forward x, multiply, inverse x), backward half.
-    // `direction` is switched to the half being issued, so that every pass helper takes its inverse flag and its t0 kernels from it
+    // spectral convolution plans (dfft_plan_convolve_*): forward half, fused X pass (forward x, multiply, inverse x), backward half,
+    // each half run with its own direction and fused choice (`direction` stays DFFT_FORWARD)
     bool conv = false;
     bool conv_fuse[2] = {false, false};   // fused t0 of the forward [0] / backward [1] half, chosen as a C2C plan of that direction would
     bool conv_fuse_tma = false;           // the forward half's t0 is the TMA fused kernel
-    int phase_base = 0;                   // DRY_RUN: added to the recorded phases (the backward half of a convolve plan records from 2)
     void* work2 = nullptr;                // P2P convolve: the backward exchange's receive buffer (the peers store into it while this
     std::vector<void*> peer_work2;        // device may still be reading `work`)
+    // buffer roles of the slab schedule (execute_slabs): `stage` = the P2P forward Z output and the NCCL send buffer of either
+    // direction, `ybwd` = the backward Y output.  C2C plans borrow bufferDev2; R2C and convolve plans use `mid`, so that a user's
+    // real buffer never holds complex data (a one-device R2C plan runs its backward Y in place in `work`)
+    void* stage = nullptr;
+    void* ybwd = nullptr;
 };
 
 // symbolic device address of a describe-only plan: device d (0-based), buffer id b: 1 bufferDev1, 2 bufferDev2 / user out,
@@ -489,8 +493,12 @@ static inline cudaError_t ev_record(dfft_plan p, cudaEvent_t e) { return p->dry 
 static inline cudaError_t ev_record_on(dfft_plan p, cudaEvent_t e, cudaStream_t st) { return p->dry ? cudaSuccess : cudaEventRecord(e, st); }
 static inline cudaError_t stream_wait(dfft_plan p, cudaStream_t st, cudaEvent_t e) { return p->dry ? cudaSuccess : cudaStreamWaitEvent(st, e, 0); }
 
+static const char* const kPassNames[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW", "Z_R2C", "Z_C2R", "XCONV", "XCONV_CO"};
+
+// `extra`: further fields of the record, each starting with ", "
 template <typename T>
-static void record_op(dfft_plan p, const char* name, int phase, int N, int C, bool chunk_in, bool chunk_out, bool transposed_store, const TileArgs<T>& a)
+static void record_op(std::vector<std::string>& ops, const char* name, int phase, int N, int C, bool chunk_in, bool chunk_out, bool transposed_store,
+                      const TileArgs<T>& a, const char* extra = "")
 {
     char buf[256];
     std::string o = "{";
@@ -512,8 +520,19 @@ static void record_op(dfft_plan p, const char* name, int phase, int N, int C, bo
         for (int q = 0; q < ct.nchunks; q++) { snprintf(buf, sizeof(buf), "%s%lld", q ? ", " : "", ct.SAq[q]); o += buf; }
         o += "]}";
     }
+    o += extra;
     o += "}";
-    p->ops.push_back(o);
+    ops.push_back(o);
+}
+
+// the records as one JSON array (the debug hooks' format); returns the bytes needed, copied into buf when cap suffices
+static long long ops_json(const std::vector<std::string>& ops, char* buf, long long cap)
+{
+    std::string o = "[";
+    for (size_t i = 0; i < ops.size(); i++) { if (i) o += ", "; o += ops[i]; }
+    o += "]";
+    if (buf && cap > (long long)o.size()) memcpy(buf, o.c_str(), o.size() + 1);
+    return (long long)o.size() + 1;
 }
 
 template <typename T> static cudaError_t upload_lut(void** dst, int nstages, const int* rad)
@@ -551,40 +570,40 @@ static int share_pointer(dfft_plan p, void* mine, std::vector<void*>& peers)
 }
 
 static int plan_create(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
-                       int P, int direction, int precision, unsigned flags, dfft_plan* plan_out, bool real = false, bool conv = false);
+                       int P, int direction, int precision, unsigned flags, dfft_plan* plan_out, bool real, bool conv);
+
+// a participant that fails (bad argument, allocation, peer mapping ...) must not leave the others waiting for it in the collective
+// part of plan creation: the local communicator is poisoned and their barriers return an error
+static int plan_create_collective(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx, int P,
+                                  int direction, int precision, unsigned flags, dfft_plan* plan_out, bool real, bool conv)
+{
+    const int rc = plan_create(n0, n1, n2, in, out, comm, dev_idx, P, direction, precision, flags, plan_out, real, conv);
+    if (rc != 0 && P > 1 && comm && comm->local && !(flags & DFFT_DRY_RUN)) comm->poison();
+    return rc;
+}
 
 extern "C" int dfft_plan_c2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
                                 int P, int direction, int precision, unsigned flags, dfft_plan* plan_out)
 {
-    const int rc = plan_create(n0, n1, n2, in, out, comm, dev_idx, P, direction, precision, flags, plan_out);
-    // a participant that fails (bad argument, allocation, peer mapping ...) must not leave the others waiting for it
-    // in the collective part of plan creation: the local communicator is poisoned and their barriers return an error
-    if (rc != 0 && P > 1 && comm && comm->local && !(flags & DFFT_DRY_RUN)) comm->poison();
-    return rc;
+    return plan_create_collective(n0, n1, n2, in, out, comm, dev_idx, P, direction, precision, flags, plan_out, false, false);
 }
 
 extern "C" int dfft_plan_r2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
                                 int P, int direction, int precision, unsigned flags, dfft_plan* plan_out)
 {
-    const int rc = plan_create(n0, n1, n2, in, out, comm, dev_idx, P, direction, precision, flags, plan_out, true);
-    if (rc != 0 && P > 1 && comm && comm->local && !(flags & DFFT_DRY_RUN)) comm->poison();
-    return rc;
+    return plan_create_collective(n0, n1, n2, in, out, comm, dev_idx, P, direction, precision, flags, plan_out, true, false);
 }
 
 extern "C" int dfft_plan_convolve_c2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
                                          int P, int precision, unsigned flags, dfft_plan* plan_out)
 {
-    const int rc = plan_create(n0, n1, n2, in, out, comm, dev_idx, P, DFFT_FORWARD, precision, flags, plan_out, false, true);
-    if (rc != 0 && P > 1 && comm && comm->local && !(flags & DFFT_DRY_RUN)) comm->poison();
-    return rc;
+    return plan_create_collective(n0, n1, n2, in, out, comm, dev_idx, P, DFFT_FORWARD, precision, flags, plan_out, false, true);
 }
 
 extern "C" int dfft_plan_convolve_r2c_3d(long long n0, long long n1, long long n2, void* in, void* out, dfft_comm comm, int dev_idx,
                                          int P, int precision, unsigned flags, dfft_plan* plan_out)
 {
-    const int rc = plan_create(n0, n1, n2, in, out, comm, dev_idx, P, DFFT_FORWARD, precision, flags, plan_out, true, true);
-    if (rc != 0 && P > 1 && comm && comm->local && !(flags & DFFT_DRY_RUN)) comm->poison();
-    return rc;
+    return plan_create_collective(n0, n1, n2, in, out, comm, dev_idx, P, DFFT_FORWARD, precision, flags, plan_out, true, true);
 }
 
 extern "C" int dfft_local_size_r2c_3d(long long n0, long long n1, long long n2, int P, int dev, long long* real_count, long long* complex_count)
@@ -793,7 +812,7 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
             bool unused = false;
             pick(DFFT_FORWARD, p->conv_fuse[0], p->conv_fuse_tma);
             pick(DFFT_BACKWARD, p->conv_fuse[1], unused);
-            p->fuse = p->conv_fuse[0] || p->conv_fuse[1];   // execute_convolve sets the flags of the half it issues
+            p->fuse = p->conv_fuse[0] || p->conv_fuse[1];   // the plan holds the state a fused t0 of either half needs
         } else {
             pick(direction, p->fuse, p->fuse_tma);
         }
@@ -948,6 +967,8 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
         }
         if (comm->host_barrier(p->me) != 0) return bail(fail(DFFT_ECOMM, "a peer failed during plan creation"));
     }
+    p->stage = (real || conv) ? p->mid : p->buf2;
+    p->ybwd = real ? (P == 1 ? p->work : p->mid) : p->buf2;
     if (!dry) CUP(cudaDeviceSynchronize());
 #undef CUP
     *plan_out = p;
@@ -1030,34 +1051,104 @@ template <typename T> static void apply_fold(dfft_plan p, TileArgs<T>& a, const 
     }
 }
 
+// whether the pass of TMA mode `mode` over `extent` lines (Z) / columns (Y, X) runs on the TMA-pipelined kernel
+static bool tma_ok(dfft_plan p, int mode, long long extent)
+{
+    const TmaEntry* e = mode == TMA_Z ? p->tz : (mode == TMA_Y ? p->ty : p->tx);
+    return e && (e->use & (1u << mode)) && !p->dry && extent % e->C == 0;
+}
+
 template <typename T> struct Pass {
-    static int launch(dfft_plan p, const SizeEntry* e, int kind, TileArgs<T>& a, int axis_override = -1, cudaStream_t st = nullptr)
+    // one launch: in a describe-only plan `rec` records what would run; otherwise `go` launches between the per-pass event
+    // brackets of the axes ax0..ax1 it covers (none inside the pipelined schedules, which bracket their parts themselves)
+    template <class Rec, class Go> static int issue(dfft_plan p, int ax0, int ax1, Rec&& rec, Go&& go, const char* what, int N)
     {
-        if (!st) st = p->stream;
-        a.inv = p->direction == DFFT_BACKWARD ? 1 : 0;
-        a.gen = e->gen;
-        const int axis = axis_override >= 0 ? axis_override : (kind == PK_Z ? 0 : (kind == PK_Y || kind == PK_Y_CO || kind == PK_Y_CI ? 1 : 2));
         if (p->dry) {
-            static const char* names[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW", "Z_R2C", "Z_C2R"};
-            const int C = kind == PK_Z ? e->z_C : (kind == PK_Y || kind == PK_Y_CI ? e->s_C : (kind == PK_Y_CO ? e->p_C : e->x_C));
-            // phase 1 = runs after the exchange has delivered this device's receive buffer
-            const bool fwd = p->direction == DFFT_FORWARD;
-            const int phase = p->phase_base + (fwd ? (axis == 2 ? 1 : 0) : (axis == 2 ? 0 : 1));
-            record_op<T>(p, names[kind], phase, e->N, C, kind == PK_Y_CI, kind == PK_Y_CO || kind == PK_XB_CO, kind == PK_XF || kind == PK_XF_TW, a);
+            rec();
             p->launches++;
             return 0;
         }
-        if (!p->in_pipe) ev_record(p, p->pev[axis][0]);
-        cudaError_t err = e->launch[kind](&a, p->sms, st);
-        if (!p->in_pipe) ev_record(p, p->pev[axis][1]);
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "pass launch (kind %d, N=%d) failed: %s", kind, e->N, cudaGetErrorString(err));
+        if (!p->in_pipe) ev_record(p, p->pev[ax0][0]);
+        const cudaError_t err = go();
+        if (!p->in_pipe) {
+            ev_record(p, p->pev[ax0][1]);
+            for (int ax = ax0 + 1; ax <= ax1; ax++) { ev_record(p, p->pev[ax][0]); ev_record(p, p->pev[ax][1]); }
+        }
+        if (err != cudaSuccess) return fail(DFFT_ECUDA, "%s launch (N=%d) failed: %s", what, N, cudaGetErrorString(err));
         p->launches++;
         return 0;
+    }
+    static T scale_factor(dfft_plan p)
+    {
+        const Geom& g = p->g;
+        return (T)(1.0 / ((double)g.n0 * (double)g.n1 * (p->r2c ? (double)p->n2r : (double)g.n2)));
+    }
+    // contiguous Z lines of every local plane, C lines per tile: per plane (the fused kernels' role) or as one run of n0l*N1 lines
+    static void z_lines(dfft_plan p, TileArgs<T>& a, int C, bool per_plane)
+    {
+        const Geom& g = p->g;
+        const long long nlines = per_plane ? g.n1 : p->n0l * g.n1;
+        a.G = (int)cdiv(nlines, C); a.W = (int)std::min<long long>(nlines, 0x7fffffff); a.ntiles = per_plane ? p->n0l * a.G : a.G;
+        a.ia = Affine{per_plane ? g.n1 * g.n2 : 0, (long long)C * g.n2, g.n2, 1}; a.oa = a.ia;
+    }
+    // Y columns (length N1, stride N2) of every local plane over the z-extent zk (N2: whole planes); returns the map of the
+    // [x_l][y][z] side
+    static Affine y_cols(dfft_plan p, TileArgs<T>& a, int C, long long zk)
+    {
+        const Geom& g = p->g;
+        a.G = (int)cdiv(zk, C); a.W = (int)zk; a.ntiles = p->n0l * a.G;
+        return Affine{g.n1 * g.n2, C, 1, g.n2};
+    }
+    // X columns over the z-extent zk: the [x][y_l][z'] side (row length zk) and the transposed [y_l][z][x] side; forward loads
+    // the former and stores the latter, backward the reverse
+    static void x_tiles(dfft_plan p, TileArgs<T>& a, int C, long long zk, bool fwd)
+    {
+        const Geom& g = p->g;
+        a.G = (int)cdiv(zk, C); a.W = (int)zk; a.ntiles = p->n1l * a.G;
+        const Affine slab{zk, C, 1, p->n1l * zk}, tr{g.n2 * g.n0, (long long)C * g.n0, g.n0, 1};
+        a.ia = fwd ? slab : tr; a.oa = fwd ? tr : slab;
+    }
+    // chunk q = the rows of destination / source device q at base[q]: split along y (ediv yd, n1_l(q) rows of zk points per
+    // plane) or along x (ediv xd, planes of zk points)
+    static void chunk_table(dfft_plan p, ChunkTab& ct, bool by_y, long long zk, void* const* base)
+    {
+        const Geom& g = p->g;
+        ct.ediv = (int)(by_y ? g.yd() : g.xd()); ct.nchunks = p->P;
+        for (int q = 0; q < p->P; q++) { ct.cptr[q] = base[q]; ct.SAq[q] = by_y ? g.n1l(q) * zk : zk; }
+    }
+    // controls of a two-role t0 kernel: every plane's first role (GA tiles) completes before its second role (GB tiles) reads it
+    static FusedCtl fused_ctl(dfft_plan p, int GA, int GB)
+    {
+        FusedCtl c{};
+        c.plane_done = p->plane_done; c.ticket = p->ticket; c.planes = p->n0l;
+        c.GA = GA; c.GB = GB;
+        c.target = p->fuse_epoch += (unsigned long long)GA;
+        c.lag = p->lag;
+        return c;
+    }
+    // DRY_RUN phase of a pass: 1 = runs after the exchange has delivered this device's receive buffer (a convolve plan's
+    // backward half records from 2)
+    static int phase(dfft_plan p, int dir, bool after_exchange) { return (p->conv && dir == DFFT_BACKWARD ? 2 : 0) + (after_exchange ? 1 : 0); }
+
+    static int launch(dfft_plan p, const SizeEntry* e, int kind, TileArgs<T>& a, int dir, int axis_override = -1, cudaStream_t st = nullptr)
+    {
+        if (!st) st = p->stream;
+        a.inv = dir == DFFT_BACKWARD ? 1 : 0;
+        a.gen = e->gen;
+        const int axis = axis_override >= 0 ? axis_override : (kind == PK_Z ? 0 : (kind == PK_Y || kind == PK_Y_CO || kind == PK_Y_CI ? 1 : 2));
+        const int C = kind == PK_Z ? e->z_C : (kind == PK_Y || kind == PK_Y_CI ? e->s_C : (kind == PK_Y_CO ? e->p_C : e->x_C));
+        auto rec = [&] {
+            record_op<T>(p->ops, kPassNames[kind], phase(p, dir, dir == DFFT_FORWARD ? axis == 2 : axis != 2), e->N, C, kind == PK_Y_CI,
+                         kind == PK_Y_CO || kind == PK_XB_CO, kind == PK_XF || kind == PK_XF_TW, a);
+        };
+        char what[32];
+        snprintf(what, sizeof(what), "pass (kind %d)", kind);
+        return issue(p, axis, axis, rec, [&] { return e->launch[kind](&a, p->sms, st); }, what, e->N);
     }
     // one TMA-pipelined pass (fft_tma.cuh).  Tensor sides are described as (base, d1, d2, s1, s2, axis): a 3-D tensor of
     // complex elements, row length `d0`, dim1/dim2 extents and element strides, transform axis = tensor dim `axis` (1 or 2)
     struct TmaTensor { void* base; long long d0, d1, d2, s1, s2; };
-    static int launch_tma(dfft_plan p, const TmaEntry* e, int mode, TmaArgs<T>& a, const TmaTensor* tin, const TmaTensor* tout, int axis,
+    static int launch_tma(dfft_plan p, const TmaEntry* e, int mode, TmaArgs<T>& a, const TmaTensor* tin, const TmaTensor* tout, int axis, int dir,
                           cudaStream_t st = nullptr)
     {
         if (!st) st = p->stream;
@@ -1071,41 +1162,35 @@ template <typename T> struct Pass {
             const int rc = tma_encode_3d(ms[k], ts[k]->base, p->prec, ts[k]->d0, ts[k]->d1, ts[k]->d2, ts[k]->s1, ts[k]->s2, e->C, b1, b2);
             if (rc != 0) return fail(DFFT_ECUDA, "cuTensorMapEncodeTiled failed (%d) for a %lldx%lldx%lld tensor", rc, ts[k]->d0, ts[k]->d1, ts[k]->d2);
         }
-        a.inv = p->direction == DFFT_BACKWARD ? 1 : 0;
-        if (!p->in_pipe) ev_record(p, p->pev[axis][0]);
-        cudaError_t err = e->launch(mode, &a, tin ? mi : nullptr, tout ? mo : nullptr, p->sms, st);
-        if (!p->in_pipe) ev_record(p, p->pev[axis][1]);
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "TMA pass launch (mode %d, N=%d) failed: %s", mode, e->N, cudaGetErrorString(err));
-        p->launches++;
-        return 0;
+        a.inv = dir == DFFT_BACKWARD ? 1 : 0;
+        char what[32];
+        snprintf(what, sizeof(what), "TMA pass (mode %d)", mode);
+        return issue(p, axis, axis, [] {}, [&] { return e->launch(mode, &a, tin ? mi : nullptr, tout ? mo : nullptr, p->sms, st); }, what, e->N);
     }
     // contiguous lines of length N2 (n0l*N1 lines), src -> dst (in place when equal)
-    static int z_pass(dfft_plan p, const void* src, void* dst, bool scale)
+    static int z_pass(dfft_plan p, const void* src, void* dst, bool scale, int dir)
     {
         const Geom& g = p->g;
-        if (p->tz && (p->tz->use & (1u << TMA_Z)) && !p->dry && (p->n0l * g.n1) % p->tz->C == 0) {
+        if (tma_ok(p, TMA_Z, p->n0l * g.n1)) {
             TmaArgs<T> t{};
             t.in = (const cx<T>*)src; t.out = (cx<T>*)dst; t.lut = (const cx<T>*)p->lut_tz;
             t.ntiles = p->n0l * g.n1 / p->tz->C; t.G = (int)std::min<long long>(t.ntiles, 0x7fffffff);
             t.in_SA = t.out_SA = (long long)t.G * p->tz->C * g.n2;   // a = tile / G: only needed beyond 2^31 tiles
-            t.do_scale = scale ? 1 : 0; t.scale = (T)(1.0 / ((double)g.n0 * (double)g.n1 * (double)g.n2));
-            return launch_tma(p, p->tz, TMA_Z, t, nullptr, nullptr, 0);
+            t.do_scale = scale ? 1 : 0; t.scale = scale_factor(p);
+            return launch_tma(p, p->tz, TMA_Z, t, nullptr, nullptr, 0, dir);
         }
         TileArgs<T> a{};
-        const int C = p->ez->z_C;
-        const long long nlines = p->n0l * g.n1;
+        z_lines(p, a, p->ez->z_C, false);
         a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)p->lut_z;
-        a.G = (int)cdiv(nlines, C); a.W = (int)std::min<long long>(nlines, 0x7fffffff); a.ntiles = a.G;
-        a.ia = Affine{0, (long long)C * g.n2, g.n2, 1}; a.oa = a.ia;
-        a.do_scale = scale ? 1 : 0; a.scale = (T)(1.0 / ((double)g.n0 * (double)g.n1 * (double)g.n2));
-        return launch(p, p->ez, PK_Z, a);
+        a.do_scale = scale ? 1 : 0; a.scale = scale_factor(p);
+        return launch(p, p->ez, PK_Z, a, dir);
     }
     // real-data Z pass of an R2C plan (fft_real.cuh): the n0l*N1 real lines of N2r points, two per complex transform, <-> as many
     // half-spectrum lines of nzh = g.n2 points.  Forward: src real -> dst complex; backward: src complex -> dst real (+ scale)
-    static int z_real(dfft_plan p, const void* src, void* dst, bool scale)
+    static int z_real(dfft_plan p, const void* src, void* dst, bool scale, int dir)
     {
         const Geom& g = p->g;
-        const bool fwd = p->direction == DFFT_FORWARD;
+        const bool fwd = dir == DFFT_FORWARD;
         const int C = p->ez->z_C;
         const long long nlines = p->n0l * g.n1, N = p->n2r, H = g.n2;
         RealZArgs<T> r{};
@@ -1118,97 +1203,62 @@ template <typename T> struct Pass {
         if (fwd) r.rin = (const T*)src;
         else r.rout = (T*)dst;
         a.inv = fwd ? 0 : 1;
-        a.do_scale = scale ? 1 : 0; a.scale = (T)(1.0 / ((double)g.n0 * (double)g.n1 * (double)N));
+        a.do_scale = scale ? 1 : 0; a.scale = scale_factor(p);
         const int kind = fwd ? PK_Z_R2C : PK_Z_C2R;
-        if (p->dry) {
+        auto rec = [&] {
             // real-side maps are in real elements; "pair" = distance between the two lines of a pair (input side, output side)
-            record_op<T>(p, fwd ? "Z_R2C" : "Z_C2R", p->phase_base + (fwd ? 0 : 1), (int)N, C, false, false, false, a);
-            char buf[128];
-            snprintf(buf, sizeof(buf), ", \"nzh\": %lld, \"pair\": [%lld, %lld]}", H, r.ld_in, r.ld_out);
-            p->ops.back().pop_back();
-            p->ops.back() += buf;
-            p->launches++;
-            return 0;
-        }
-        ev_record(p, p->pev[0][0]);
-        cudaError_t err = p->ez->launch[kind](&r, p->sms, p->stream);
-        ev_record(p, p->pev[0][1]);
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "real Z pass launch (N=%lld) failed: %s", N, cudaGetErrorString(err));
-        p->launches++;
-        return 0;
+            char extra[128];
+            snprintf(extra, sizeof(extra), ", \"nzh\": %lld, \"pair\": [%lld, %lld]", H, r.ld_in, r.ld_out);
+            record_op<T>(p->ops, kPassNames[kind], phase(p, dir, !fwd), (int)N, C, false, false, false, a, extra);
+        };
+        return issue(p, 0, 0, rec, [&] { return p->ez->launch[kind](&r, p->sms, p->stream); }, "real Z pass", (int)N);
     }
     // columns of length N1 (stride N2) of every local plane.  mode 0: src -> dst natural (in place when equal)
     // mode 1: chunked (packed / peer) store, mode 2: chunked (unpack) load
-    static int y_pass(dfft_plan p, const void* src, void* dst, int mode, void* const* chunk_base, const Fold* fold = nullptr)
+    static int y_pass(dfft_plan p, const void* src, void* dst, int mode, void* const* chunk_base, const Fold* fold, int dir)
     {
         const Geom& g = p->g;
-        if (mode == 0 && p->ty && (p->ty->use & (1u << TMA_Y)) && !p->dry && g.n2 % p->ty->C == 0) {
+        if (mode == 0 && tma_ok(p, TMA_Y, g.n2)) {
             TmaArgs<T> t{};
             t.lut = (const cx<T>*)p->lut_ty;
             t.G = (int)(g.n2 / p->ty->C); t.ntiles = p->n0l * t.G;
             TmaTensor ti{(void*)src, g.n2, g.n1, p->n0l, g.n2, g.n1 * g.n2}, to{dst, g.n2, g.n1, p->n0l, g.n2, g.n1 * g.n2};
-            return launch_tma(p, p->ty, TMA_Y, t, &ti, &to, 1);
+            return launch_tma(p, p->ty, TMA_Y, t, &ti, &to, 1, dir);
         }
         TileArgs<T> a{};
-        const int C = mode == 1 ? p->ey->p_C : p->ey->s_C;
         a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)p->lut_y;
-        a.G = (int)cdiv(g.n2, C); a.W = (int)g.n2; a.ntiles = p->n0l * a.G;
-        a.ia = Affine{g.n1 * g.n2, C, 1, g.n2}; a.oa = a.ia;
-        if (mode != 0) {
-            ChunkTab& ct = mode == 1 ? a.co : a.ci;
-            ct.ediv = (int)g.yd(); ct.nchunks = p->P;
-            for (int q = 0; q < p->P; q++) { ct.cptr[q] = chunk_base[q]; ct.SAq[q] = g.n1l(q) * g.n2; }
-        }
+        a.ia = a.oa = y_cols(p, a, mode == 1 ? p->ey->p_C : p->ey->s_C, g.n2);
+        if (mode != 0) chunk_table(p, mode == 1 ? a.co : a.ci, true, g.n2, chunk_base);
         apply_fold<T>(p, a, fold);
-        return launch(p, p->ey, mode == 0 ? PK_Y : (mode == 1 ? PK_Y_CO : PK_Y_CI), a);
+        return launch(p, p->ey, mode == 0 ? PK_Y : (mode == 1 ? PK_Y_CO : PK_Y_CI), a, dir);
     }
     // t0 in one persistent kernel (square planes): forward Z (zsrc -> mid) then Y (mid -> ydst, or chunked);
     // backward Y (ysrc or chunked -> mid) then Z (mid -> mid).  ymode as in y_pass.
-    static int zy_fused(dfft_plan p, const void* src, void* mid, void* dst, int ymode, void* const* chunk_base, bool scale, const Fold* fold = nullptr)
+    static int zy_fused(dfft_plan p, const void* src, void* mid, void* dst, int ymode, void* const* chunk_base, bool scale, const Fold* fold, int dir)
     {
         const Geom& g = p->g;
         const SizeEntry* e = p->ez;
-        const bool fwd = p->direction == DFFT_FORWARD;
+        const bool fwd = dir == DFFT_FORWARD;
         TileArgs<T> z{}, y{};
         const int CZ = (fwd && ymode == 1) ? e->f_zCp : e->f_zC, CY = (fwd && ymode == 1) ? e->p_C : e->s_C;
         z.lut = (const cx<T>*)p->lut_z; y.lut = (const cx<T>*)p->lut_y;
         z.inv = y.inv = fwd ? 0 : 1;
-        // contiguous role, tiled per plane: tile (plane, b) = CZ lines starting at line b*CZ of the plane
-        z.G = (int)cdiv(g.n1, CZ); z.W = (int)g.n1; z.ntiles = p->n0l * z.G;
-        z.ia = Affine{g.n1 * g.n2, (long long)CZ * g.n2, g.n2, 1}; z.oa = z.ia;
-        z.do_scale = scale ? 1 : 0; z.scale = (T)(1.0 / ((double)g.n0 * (double)g.n1 * (double)g.n2));
-        y.G = (int)cdiv(g.n2, CY); y.W = (int)g.n2; y.ntiles = p->n0l * y.G;
-        y.ia = Affine{g.n1 * g.n2, CY, 1, g.n2}; y.oa = y.ia;
-        if (ymode != 0) {
-            ChunkTab& ct = ymode == 1 ? y.co : y.ci;
-            ct.ediv = (int)g.yd(); ct.nchunks = p->P;
-            for (int q = 0; q < p->P; q++) { ct.cptr[q] = chunk_base[q]; ct.SAq[q] = g.n1l(q) * g.n2; }
-        }
+        z_lines(p, z, CZ, true);   // contiguous role, tiled per plane: tile (plane, b) = CZ lines starting at line b*CZ of the plane
+        z.do_scale = scale ? 1 : 0; z.scale = scale_factor(p);
+        y.ia = y.oa = y_cols(p, y, CY, g.n2);
+        if (ymode != 0) chunk_table(p, ymode == 1 ? y.co : y.ci, true, g.n2, chunk_base);
         if (fwd) { z.in = (const cx<T>*)src; z.out = (cx<T>*)mid; y.in = (const cx<T>*)mid; y.out = (cx<T>*)dst; }
         else { y.in = (const cx<T>*)src; y.out = (cx<T>*)mid; z.in = (const cx<T>*)mid; z.out = (cx<T>*)mid; }
-        FusedCtl c{};
-        c.plane_done = p->plane_done; c.ticket = p->ticket; c.planes = p->n0l;
-        c.GA = fwd ? z.G : y.G; c.GB = fwd ? y.G : z.G;
-        c.target = p->fuse_epoch += (unsigned long long)c.GA;
-        c.lag = p->lag;
+        FusedCtl c = fused_ctl(p, fwd ? z.G : y.G, fwd ? y.G : z.G);
         const int kind = fwd ? (ymode == 1 ? FK_ZY_CO : FK_ZY) : (ymode == 2 ? FK_YZ_CI : FK_YZ);
         apply_fold<T>(p, fwd ? y : z, fold);   // fft_fused2_kernel gates on / signals through its second role's arguments
-        if (p->dry) {
-            z.gen = y.gen = nullptr;
-            const int ph = p->phase_base;
-            if (fwd) { record_op<T>(p, "fusedZ", ph, e->N, CZ, false, false, false, z); record_op<T>(p, "fusedY", ph, e->N, CY, false, ymode == 1, false, y); }
-            else { record_op<T>(p, "fusedY", ph + 1, e->N, CY, ymode == 2, false, false, y); record_op<T>(p, "fusedZ", ph + 1, e->N, CZ, false, false, false, z); }
-            p->launches++;
-            return 0;
-        }
-        ev_record(p, p->pev[0][0]);
-        cudaError_t err = fwd ? e->fused[kind](&z, &y, &c, p->sms, p->stream) : e->fused[kind](&y, &z, &c, p->sms, p->stream);
-        ev_record(p, p->pev[0][1]);
-        ev_record(p, p->pev[1][0]);
-        ev_record(p, p->pev[1][1]);
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "fused t0 launch (kind %d, N=%d) failed: %s", kind, e->N, cudaGetErrorString(err));
-        p->launches++;
-        return 0;
+        auto rec = [&] {
+            const int ph = phase(p, dir, !fwd);
+            if (fwd) { record_op<T>(p->ops, "fusedZ", ph, e->N, CZ, false, false, false, z); record_op<T>(p->ops, "fusedY", ph, e->N, CY, false, ymode == 1, false, y); }
+            else { record_op<T>(p->ops, "fusedY", ph, e->N, CY, ymode == 2, false, false, y); record_op<T>(p->ops, "fusedZ", ph, e->N, CZ, false, false, false, z); }
+        };
+        auto go = [&] { return fwd ? e->fused[kind](&z, &y, &c, p->sms, p->stream) : e->fused[kind](&y, &z, &c, p->sms, p->stream); };
+        return issue(p, 0, 1, rec, go, "fused t0", e->N);
     }
     // forward t0 of one device in one TMA-pipelined kernel (square planes): Z: src -> mid, Y: mid -> mid in place
     static int zy_fused_tma(dfft_plan p, const void* src, void* mid)
@@ -1220,19 +1270,8 @@ template <typename T> struct Pass {
         if (rc != 0) return fail(DFFT_ECUDA, "cuTensorMapEncodeTiled failed (%d) for a %lldx%lldx%lld tensor", rc, g.n2, g.n1, p->n0l);
         TmaFusedArgs<T> a{};
         a.src = (const cx<T>*)src; a.mid = (cx<T>*)mid; a.lut = (const cx<T>*)p->lut_tz;
-        FusedCtl c{};
-        c.plane_done = p->plane_done; c.ticket = p->ticket; c.planes = p->n0l;
-        c.GA = (int)(g.n1 / e->C); c.GB = (int)(g.n2 / e->C);
-        c.target = p->fuse_epoch += (unsigned long long)c.GA;
-        c.lag = p->lag;
-        ev_record(p, p->pev[0][0]);
-        cudaError_t err = e->fused_zy(&a, &c, mm, p->sms, p->stream);
-        ev_record(p, p->pev[0][1]);
-        ev_record(p, p->pev[1][0]);
-        ev_record(p, p->pev[1][1]);
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "TMA fused t0 launch (N=%d) failed: %s", e->N, cudaGetErrorString(err));
-        p->launches++;
-        return 0;
+        FusedCtl c = fused_ctl(p, (int)(g.n1 / e->C), (int)(g.n2 / e->C));
+        return issue(p, 0, 1, [] {}, [&] { return e->fused_zy(&a, &c, mm, p->sms, p->stream); }, "TMA fused t0", e->N);
     }
     // forward t0 + t1 + t2 + t3 in one kernel (P2P, square planes): Z: buf1 -> mid, Y: mid -> peers' work, X: work -> buf2
     static int fwd_overlapped(dfft_plan p, void* const* peer_base)
@@ -1242,17 +1281,12 @@ template <typename T> struct Pass {
         TileArgs<T> z{}, y{}, x{};
         const int CZ = e->f_zCp, CY = e->p_C, CX = e->x_C;
         z.lut = (const cx<T>*)p->lut_z; y.lut = (const cx<T>*)p->lut_y; x.lut = (const cx<T>*)p->lut_x;
-        z.G = (int)cdiv(g.n1, CZ); z.W = (int)g.n1; z.ntiles = p->n0l * z.G;
-        z.ia = Affine{g.n1 * g.n2, (long long)CZ * g.n2, g.n2, 1}; z.oa = z.ia;
+        z_lines(p, z, CZ, true);
         z.in = (const cx<T>*)p->buf1; z.out = (cx<T>*)p->mid;
-        y.G = (int)cdiv(g.n2, CY); y.W = (int)g.n2; y.ntiles = p->n0l * y.G;
-        y.ia = Affine{g.n1 * g.n2, CY, 1, g.n2}; y.oa = y.ia;
+        y.ia = y.oa = y_cols(p, y, CY, g.n2);
         y.in = (const cx<T>*)p->mid; y.out = nullptr;
-        y.co.ediv = (int)g.yd(); y.co.nchunks = p->P;
-        for (int q = 0; q < p->P; q++) { y.co.cptr[q] = peer_base[q]; y.co.SAq[q] = g.n1l(q) * g.n2; }
-        x.G = (int)cdiv(g.n2, CX); x.W = (int)g.n2; x.ntiles = p->n1l * x.G;
-        x.ia = Affine{g.n2, CX, 1, p->n1l * g.n2};
-        x.oa = Affine{g.n2 * g.n0, (long long)CX * g.n0, g.n0, 1};
+        chunk_table(p, y.co, true, g.n2, peer_base);
+        x_tiles(p, x, CX, g.n2, true);
         x.in = (const cx<T>*)p->work; x.out = (cx<T>*)p->buf2;
         Fused3Ctl c{};
         c.plane_done = p->plane_done; c.ticket = p->ticket; c.part_done = p->part_done;
@@ -1274,20 +1308,12 @@ template <typename T> struct Pass {
             cudaMemsetAsync(p->dbg + 4, 0, 12 * sizeof(unsigned long long), p->stream);
             c.dbg = p->dbg;
         }
-        if (p->dry) {
-            record_op<T>(p, "ovlZ", 0, e->N, CZ, false, false, false, z);
-            record_op<T>(p, "ovlY", 0, e->N, CY, false, true, false, y);
-            record_op<T>(p, "ovlX", 1, e->N, CX, false, false, true, x);
-            p->launches++;
-            return 0;
-        }
-        ev_record(p, p->pev[0][0]);
-        cudaError_t err = e->fused3(&z, &y, &x, &c, p->sms, p->stream);
-        ev_record(p, p->pev[0][1]);
-        for (int a = 1; a < 3; a++) { ev_record(p, p->pev[a][0]); ev_record(p, p->pev[a][1]); }
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "overlapped forward launch (N=%d) failed: %s", e->N, cudaGetErrorString(err));
-        p->launches++;
-        return 0;
+        auto rec = [&] {
+            record_op<T>(p->ops, "ovlZ", 0, e->N, CZ, false, false, false, z);
+            record_op<T>(p->ops, "ovlY", 0, e->N, CY, false, true, false, y);
+            record_op<T>(p->ops, "ovlX", 1, e->N, CX, false, false, true, x);
+        };
+        return issue(p, 0, 2, rec, [&] { return e->fused3(&z, &y, &x, &c, p->sms, p->stream); }, "overlapped forward", e->N);
     }
     // X transform that keeps the natural [x][y][z] layout (single device): columns along x, stride N1*N2, src -> dst
     static int x_natural(dfft_plan p, const void* src, void* dst)
@@ -1298,41 +1324,35 @@ template <typename T> struct Pass {
         a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)p->lut_xn;
         a.G = (int)cdiv(g.n2, C); a.W = (int)g.n2; a.ntiles = g.n1 * a.G;
         a.ia = Affine{g.n2, C, 1, g.n1 * g.n2}; a.oa = a.ia;
-        return launch(p, p->ex, PK_Y, a, 2);   // a strided-local kernel, timed as the X pass
+        return launch(p, p->ex, PK_Y, a, p->direction, 2);   // a strided-local kernel, timed as the X pass
     }
     // forward X: src = [x][y_l][z] -> dst = [y_l][z][x]
-    static bool x_fwd_folds(dfft_plan p) { return !(p->tx && (p->tx->use & (1u << TMA_XF)) && !p->dry && p->g.n2 % p->tx->C == 0); }
+    static bool x_fwd_folds(dfft_plan p) { return !tma_ok(p, TMA_XF, p->g.n2); }
     static int x_fwd(dfft_plan p, const void* src, void* dst, const Fold* fold = nullptr)
     {
         const Geom& g = p->g;
-        if (p->tx && (p->tx->use & (1u << TMA_XF)) && !p->dry && g.n2 % p->tx->C == 0) {
+        if (tma_ok(p, TMA_XF, g.n2)) {
             TmaArgs<T> t{};
             t.lut = (const cx<T>*)p->lut_tx; t.out = (cx<T>*)dst;
             t.G = (int)(g.n2 / p->tx->C); t.ntiles = p->n1l * t.G; t.out_SA = g.n2 * g.n0;
             TmaTensor ti{(void*)src, g.n2, p->n1l, g.n0, g.n2, p->n1l * g.n2};
-            return launch_tma(p, p->tx, TMA_XF, t, &ti, nullptr, 2);
+            return launch_tma(p, p->tx, TMA_XF, t, &ti, nullptr, 2, DFFT_FORWARD);
         }
         TileArgs<T> a{};
-        const int C = p->ex->x_C;
+        x_tiles(p, a, p->ex->x_C, g.n2, true);
         a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)p->lut_x;
-        a.G = (int)cdiv(g.n2, C); a.W = (int)g.n2; a.ntiles = p->n1l * a.G;
-        a.ia = Affine{g.n2, C, 1, p->n1l * g.n2};
-        a.oa = Affine{g.n2 * g.n0, (long long)C * g.n0, g.n0, 1};
         apply_fold<T>(p, a, fold);
-        return launch(p, p->ex, PK_XF, a);
+        return launch(p, p->ex, PK_XF, a, DFFT_FORWARD);
     }
     // ---- z-part variants (stream-pipelined forward): part k of K covers the columns z in [k*zk, (k+1)*zk) ----------
     // Y pass of one z-part: mid[x_l][y][z in part] -> chunk q (the rows of destination device q) at chunk_base[q], laid out
     // [x_l][y_l(q)][z'] with row length zk: the part-major receive (P2P) / send (NCCL) layout
     static void y_part_args(dfft_plan p, TileArgs<T>& a, const void* src, long long zk, int k, void* const* chunk_base, int C)
     {
-        const Geom& g = p->g;
         a.in = (const cx<T>*)src + k * zk; a.out = nullptr; a.lut = (const cx<T>*)p->lut_y;
-        a.G = (int)cdiv(zk, C); a.W = (int)zk; a.ntiles = p->n0l * a.G;
-        a.ia = Affine{g.n1 * g.n2, C, 1, g.n2};
+        a.ia = y_cols(p, a, C, zk);
         a.oa = Affine{0, C, 1, zk};
-        a.co.ediv = (int)g.yd(); a.co.nchunks = p->P;
-        for (int q = 0; q < p->P; q++) { a.co.cptr[q] = chunk_base[q]; a.co.SAq[q] = g.n1l(q) * zk; }
+        chunk_table(p, a.co, true, zk, chunk_base);
         if (p->xmode == DFFT_EXCHANGE_P2P && !p->dry && p->done_ctr) {
             // the kernel's last CTA publishes "part k of sender me has arrived" (epoch) on every receiving device
             a.sig_n = p->P; a.sig_val = p->epoch; a.done_ctr = p->done_ctr + k;
@@ -1344,46 +1364,31 @@ template <typename T> struct Pass {
         TileArgs<T> a{};
         y_part_args(p, a, src, zk, k, chunk_base, p->ey->p_C);
         a.max_ctas_per_sm = cap;
-        return launch(p, p->ey, PK_Y_CO, a);
+        return launch(p, p->ey, PK_Y_CO, a, DFFT_FORWARD);
     }
     // part 0 together with the Z pass of every plane in one persistent kernel (fft_fused2_kernel): Z: src -> mid (L2),
     // Y part 0: mid -> chunks
     static int zy_fused_part0(dfft_plan p, const void* src, void* mid, long long zk, void* const* chunk_base)
     {
-        const Geom& g = p->g;
         const SizeEntry* e = p->ez;
         TileArgs<T> z{}, y{};
         const int CZ = e->f_zCp, CY = e->p_C;
         z.lut = (const cx<T>*)p->lut_z;
-        z.G = (int)cdiv(g.n1, CZ); z.W = (int)g.n1; z.ntiles = p->n0l * z.G;
-        z.ia = Affine{g.n1 * g.n2, (long long)CZ * g.n2, g.n2, 1}; z.oa = z.ia;
+        z_lines(p, z, CZ, true);
         z.in = (const cx<T>*)src; z.out = (cx<T>*)mid;
         y_part_args(p, y, mid, zk, 0, chunk_base, CY);
-        FusedCtl c{};
-        c.plane_done = p->plane_done; c.ticket = p->ticket; c.planes = p->n0l;
-        c.GA = z.G; c.GB = y.G;
-        c.target = p->fuse_epoch += (unsigned long long)c.GA;
-        c.lag = p->lag;
-        if (p->dry) {
-            record_op<T>(p, "fusedZ", 0, e->N, CZ, false, false, false, z);
-            record_op<T>(p, "fusedY", 0, e->N, CY, false, true, false, y);
-            p->launches++;
-            return 0;
-        }
-        cudaError_t err = e->fused[FK_ZY_CO](&z, &y, &c, p->sms, p->stream);
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "fused t0 (part 0) launch (N=%d) failed: %s", e->N, cudaGetErrorString(err));
-        p->launches++;
-        return 0;
+        FusedCtl c = fused_ctl(p, z.G, y.G);
+        auto rec = [&] {
+            record_op<T>(p->ops, "fusedZ", 0, e->N, CZ, false, false, false, z);
+            record_op<T>(p->ops, "fusedY", 0, e->N, CY, false, true, false, y);
+        };
+        return issue(p, 0, 1, rec, [&] { return e->fused[FK_ZY_CO](&z, &y, &c, p->sms, p->stream); }, "fused t0 (part 0)", e->N);
     }
     // X pass of one z-part on the receive side: rpart = [x (all N0)][y_l][z'] (row length zk) -> dst[y_l][z in part][x]
     static void x_part_args(dfft_plan p, TileArgs<T>& a, const void* rpart, void* dst, long long zk, int k)
     {
-        const Geom& g = p->g;
-        const int C = p->ex->x_C;
-        a.in = (const cx<T>*)rpart; a.out = (cx<T>*)dst + k * zk * g.n0; a.lut = (const cx<T>*)p->lut_x;
-        a.G = (int)cdiv(zk, C); a.W = (int)zk; a.ntiles = p->n1l * a.G;
-        a.ia = Affine{zk, C, 1, p->n1l * zk};
-        a.oa = Affine{g.n2 * g.n0, (long long)C * g.n0, g.n0, 1};
+        x_tiles(p, a, p->ex->x_C, zk, true);
+        a.in = (const cx<T>*)rpart; a.out = (cx<T>*)dst + k * zk * p->g.n0; a.lut = (const cx<T>*)p->lut_x;
     }
     // Y pass of part k (stores to the peers) and X pass of part k-1 (already arrived) in one two-role kernel
     static int yx_fused(dfft_plan p, const void* mid, long long zk, int k, void* const* chunk_base, const void* rpart_prev, void* dst)
@@ -1395,134 +1400,106 @@ template <typename T> struct Pass {
         YxCtl c{};
         c.ticket = p->ticket;
         c.TA = (unsigned)y.ntiles; c.TB = (unsigned)x.ntiles;
-        if (p->dry) {
-            record_op<T>(p, "Y_CO", 0, e->N, e->p_C, false, true, false, y);
-            record_op<T>(p, "XF", 1, e->N, e->x_C, false, false, true, x);
-            p->launches++;
-            return 0;
-        }
-        cudaError_t err = e->fused_yx(&y, &x, &c, p->sms, p->stream);
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "fused Y+X part launch (N=%d, part %d) failed: %s", e->N, k, cudaGetErrorString(err));
-        p->launches++;
-        return 0;
+        auto rec = [&] {
+            record_op<T>(p->ops, "Y_CO", 0, e->N, e->p_C, false, true, false, y);
+            record_op<T>(p->ops, "XF", 1, e->N, e->x_C, false, false, true, x);
+        };
+        return issue(p, 1, 2, rec, [&] { return e->fused_yx(&y, &x, &c, p->sms, p->stream); }, "fused Y+X part", e->N);
     }
     static int x_part(dfft_plan p, const void* rpart, void* dst, long long zk, int k, int cap, cudaStream_t st)
     {
         const Geom& g = p->g;
         // the TMA kernel takes the whole SM (one CTA, 3-slot ring): only for a part that overlaps nothing (the last one)
-        if (cap == 0 && p->tx && (p->tx->use & (1u << TMA_XF)) && !p->dry && zk % p->tx->C == 0) {
+        if (cap == 0 && tma_ok(p, TMA_XF, zk)) {
             TmaArgs<T> t{};
             t.lut = (const cx<T>*)p->lut_tx; t.out = (cx<T>*)dst + k * zk * g.n0;
             t.G = (int)(zk / p->tx->C); t.ntiles = p->n1l * t.G; t.out_SA = g.n2 * g.n0;
             TmaTensor ti{(void*)rpart, zk, p->n1l, g.n0, zk, p->n1l * zk};
-            return launch_tma(p, p->tx, TMA_XF, t, &ti, nullptr, 2, st);
+            return launch_tma(p, p->tx, TMA_XF, t, &ti, nullptr, 2, DFFT_FORWARD, st);
         }
         TileArgs<T> a{};
-        const int C = p->ex->x_C;
-        a.in = (const cx<T>*)rpart; a.out = (cx<T>*)dst + k * zk * g.n0; a.lut = (const cx<T>*)p->lut_x;
-        a.G = (int)cdiv(zk, C); a.W = (int)zk; a.ntiles = p->n1l * a.G;
-        a.ia = Affine{zk, C, 1, p->n1l * zk};
-        a.oa = Affine{g.n2 * g.n0, (long long)C * g.n0, g.n0, 1};
+        x_part_args(p, a, rpart, dst, zk, k);
         a.max_ctas_per_sm = cap;
-        return launch(p, p->ex, PK_XF, a, -1, st);
+        return launch(p, p->ex, PK_XF, a, DFFT_FORWARD, -1, st);
     }
     // ---- z-part variants of the BACKWARD passes (stream-pipelined backward) --------------------------------------------------
     // inverse X pass of one z-part: src[y_l][z in part][x] -> chunk p (= the x-planes of destination device p) at chunk_base[p],
     // laid out [x_l][y_l][z'] with row length zk
     static int xb_part(dfft_plan p, const void* src, long long zk, int k, void* const* chunk_base, int cap)
     {
-        const Geom& g = p->g;
         TileArgs<T> a{};
-        const int C = p->ex->x_C;
-        a.in = (const cx<T>*)src + k * zk * g.n0; a.out = nullptr; a.lut = (const cx<T>*)p->lut_x;
-        a.G = (int)cdiv(zk, C); a.W = (int)zk; a.ntiles = p->n1l * a.G;
-        a.ia = Affine{g.n2 * g.n0, (long long)C * g.n0, g.n0, 1};
-        a.oa = Affine{0, C, 1, p->n1l * zk};
-        a.co.ediv = (int)g.xd(); a.co.nchunks = p->P;
-        for (int q = 0; q < p->P; q++) { a.co.cptr[q] = chunk_base[q]; a.co.SAq[q] = zk; }
+        x_tiles(p, a, p->ex->x_C, zk, false);
+        a.oa.SA = 0;   // the chunk table's SAq places the planes
+        a.in = (const cx<T>*)src + k * zk * p->g.n0; a.out = nullptr; a.lut = (const cx<T>*)p->lut_x;
+        chunk_table(p, a.co, false, zk, chunk_base);
         if (p->xmode == DFFT_EXCHANGE_P2P && !p->dry && p->done_ctr) {
             a.sig_n = p->P; a.sig_val = p->epoch; a.done_ctr = p->done_ctr + k;
             for (int q = 0; q < p->P; q++) a.sig[q] = &p->peer_sync[q]->part_arrive[k][p->me];
         }
         a.max_ctas_per_sm = cap;
-        return launch(p, p->ex, PK_XB_CO, a);
+        return launch(p, p->ex, PK_XB_CO, a, DFFT_BACKWARD);
     }
     // inverse Y pass of one z-part on the receive side: rpart = [sender q][x_l][y_l(q)][z'] -> dst[x_l][y][z in part]
     static void yinv_part_args(dfft_plan p, TileArgs<T>& a, const void* rpart, void* dst, long long zk, int k, int C)
     {
         const Geom& g = p->g;
         a.in = nullptr; a.out = (cx<T>*)dst + k * zk; a.lut = (const cx<T>*)p->lut_y;
-        a.G = (int)cdiv(zk, C); a.W = (int)zk; a.ntiles = p->n0l * a.G;
+        a.oa = y_cols(p, a, C, zk);
         a.ia = Affine{0, C, 1, zk};
-        a.oa = Affine{g.n1 * g.n2, C, 1, g.n2};
-        a.ci.ediv = (int)g.yd(); a.ci.nchunks = p->P;
-        for (int q = 0; q < p->P; q++) { a.ci.cptr[q] = eoff((void*)rpart, (long long)q * p->n0l * g.yd() * zk, p->esz); a.ci.SAq[q] = g.n1l(q) * zk; }
+        void* base[DFFT_MAX_CHUNKS];
+        for (int q = 0; q < p->P; q++) base[q] = eoff((void*)rpart, (long long)q * p->n0l * g.yd() * zk, p->esz);
+        chunk_table(p, a.ci, true, zk, base);
     }
     static int yinv_part(dfft_plan p, const void* rpart, void* dst, long long zk, int k, int cap, cudaStream_t st)
     {
         TileArgs<T> a{};
         yinv_part_args(p, a, rpart, dst, zk, k, p->ey->s_C);
         a.max_ctas_per_sm = cap;
-        return launch(p, p->ey, PK_Y_CI, a, -1, st);
+        return launch(p, p->ey, PK_Y_CI, a, DFFT_BACKWARD, -1, st);
     }
     // the LAST part's inverse Y pass completes every plane: it runs fused with the inverse Z pass (fft_fused2_kernel, Y then Z)
     static int yz_fused_last_part(dfft_plan p, const void* rpart, void* dst, long long zk, int k, bool scale, cudaStream_t st)
     {
-        const Geom& g = p->g;
         const SizeEntry* e = p->ez;
         TileArgs<T> z{}, y{};
         const int CZ = e->f_zC, CY = e->s_C;
         yinv_part_args(p, y, rpart, dst, zk, k, CY);
         y.inv = 1;
         z.lut = (const cx<T>*)p->lut_z; z.inv = 1;
-        z.G = (int)cdiv(g.n1, CZ); z.W = (int)g.n1; z.ntiles = p->n0l * z.G;
-        z.ia = Affine{g.n1 * g.n2, (long long)CZ * g.n2, g.n2, 1}; z.oa = z.ia;
+        z_lines(p, z, CZ, true);
         z.in = (const cx<T>*)dst; z.out = (cx<T>*)dst;
-        z.do_scale = scale ? 1 : 0; z.scale = (T)(1.0 / ((double)g.n0 * (double)g.n1 * (double)g.n2));
-        FusedCtl c{};
-        c.plane_done = p->plane_done; c.ticket = p->ticket; c.planes = p->n0l;
-        c.GA = y.G; c.GB = z.G;
-        c.target = p->fuse_epoch += (unsigned long long)c.GA;
-        c.lag = p->lag;
-        if (p->dry) {
-            record_op<T>(p, "fusedY", 1, e->N, CY, true, false, false, y);
-            record_op<T>(p, "fusedZ", 1, e->N, CZ, false, false, false, z);
-            p->launches++;
-            return 0;
-        }
-        cudaError_t err = e->fused[FK_YZ_CI](&y, &z, &c, p->sms, st);
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "fused inverse t0 (last part) launch (N=%d) failed: %s", e->N, cudaGetErrorString(err));
-        p->launches++;
-        return 0;
+        z.do_scale = scale ? 1 : 0; z.scale = scale_factor(p);
+        FusedCtl c = fused_ctl(p, y.G, z.G);
+        auto rec = [&] {
+            record_op<T>(p->ops, "fusedY", 1, e->N, CY, true, false, false, y);
+            record_op<T>(p->ops, "fusedZ", 1, e->N, CZ, false, false, false, z);
+        };
+        return issue(p, 0, 1, rec, [&] { return e->fused[FK_YZ_CI](&y, &z, &c, p->sms, st); }, "fused inverse t0 (last part)", e->N);
     }
     // backward X: src = [y_l][z][x] -> dst = [x][y_l][z] (chunked by destination device when chunk_base)
     static int x_bwd(dfft_plan p, const void* src, void* dst, void* const* chunk_base, const Fold* fold = nullptr)
     {
         const Geom& g = p->g;
-        if (!chunk_base && p->tx && (p->tx->use & (1u << TMA_XB)) && !p->dry && g.n2 % p->tx->C == 0) {
+        if (!chunk_base && tma_ok(p, TMA_XB, g.n2)) {
             TmaArgs<T> t{};
             t.lut = (const cx<T>*)p->lut_tx; t.in = (const cx<T>*)src;
             t.G = (int)(g.n2 / p->tx->C); t.ntiles = p->n1l * t.G; t.in_SA = g.n2 * g.n0;
             TmaTensor to{dst, g.n2, p->n1l, g.n0, g.n2, p->n1l * g.n2};
-            return launch_tma(p, p->tx, TMA_XB, t, nullptr, &to, 2);
+            return launch_tma(p, p->tx, TMA_XB, t, nullptr, &to, 2, DFFT_BACKWARD);
         }
         TileArgs<T> a{};
-        const int C = p->ex->x_C;
+        x_tiles(p, a, p->ex->x_C, g.n2, false);
         a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)p->lut_x;
-        a.G = (int)cdiv(g.n2, C); a.W = (int)g.n2; a.ntiles = p->n1l * a.G;
-        a.ia = Affine{g.n2 * g.n0, (long long)C * g.n0, g.n0, 1};
-        a.oa = Affine{g.n2, C, 1, p->n1l * g.n2};
         if (chunk_base) {
-            a.co.ediv = (int)g.xd(); a.co.nchunks = p->P;
-            for (int q = 0; q < p->P; q++) { a.co.cptr[q] = chunk_base[q]; a.co.SAq[q] = g.n2; }
+            chunk_table(p, a.co, false, g.n2, chunk_base);
+            apply_fold<T>(p, a, fold);
         }
-        if (chunk_base) apply_fold<T>(p, a, fold);
-        return launch(p, p->ex, chunk_base ? PK_XB_CO : PK_XB, a);
+        return launch(p, p->ex, chunk_base ? PK_XB_CO : PK_XB, a, DFFT_BACKWARD);
     }
     // fused X pass of a convolve plan (fft_conv_kernel): the [x][y_l][z'] columns of src, transformed along x, multiplied by
     // mult (same layout), transformed back -> dst in the same layout, or (chunk_base) split by xd into the destinations' receive
     // buffers [x_l][y_l(me)][z'] as x_bwd's chunked store does.  DFFT_SCALE_BACKWARD's 1/N rides on the multiply
-    static int x_conv(dfft_plan p, const void* src, void* dst, void* const* chunk_base, const void* mult, const Fold* fold = nullptr)
+    static int x_conv(dfft_plan p, const void* src, void* dst, void* const* chunk_base, const void* mult, const Fold* fold)
     {
         const Geom& g = p->g;
         const bool co = chunk_base != nullptr;
@@ -1530,34 +1507,21 @@ template <typename T> struct Pass {
         ConvArgs<T> r{};
         TileArgs<T>& a = r.t;
         a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)p->lut_xn;
-        a.G = (int)cdiv(g.n2, C); a.W = (int)g.n2; a.ntiles = p->n1l * a.G;
-        a.ia = Affine{g.n2, C, 1, p->n1l * g.n2}; a.oa = a.ia;
-        const double n2 = p->r2c ? (double)p->n2r : (double)g.n2;
-        a.do_scale = (p->flags & DFFT_SCALE_BACKWARD) ? 1 : 0; a.scale = (T)(1.0 / ((double)g.n0 * (double)g.n1 * n2));
-        if (co) {
-            a.co.ediv = (int)g.xd(); a.co.nchunks = p->P;
-            for (int q = 0; q < p->P; q++) { a.co.cptr[q] = chunk_base[q]; a.co.SAq[q] = g.n2; }
-        }
+        x_tiles(p, a, C, g.n2, true);
+        a.oa = a.ia;
+        a.do_scale = (p->flags & DFFT_SCALE_BACKWARD) ? 1 : 0; a.scale = scale_factor(p);
+        if (co) chunk_table(p, a.co, false, g.n2, chunk_base);
         r.mult = (const cx<T>*)mult;
         apply_fold<T>(p, a, fold);
-        if (p->dry) {
-            record_op<T>(p, co ? "XCONV_CO" : "XCONV", 1, p->ex->N, C, false, co, false, a);
-            char buf[64];
-            snprintf(buf, sizeof(buf), ", \"mult\": %llu}", (unsigned long long)(size_t)mult);
-            p->ops.back().pop_back();
-            p->ops.back() += buf;
-            p->launches++;
-            return 0;
-        }
-        ev_record(p, p->pev[2][0]);
-        cudaError_t err = p->ex->launch[co ? PK_XCONV_CO : PK_XCONV](&r, p->sms, p->stream);
-        ev_record(p, p->pev[2][1]);
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "convolution X pass launch (N=%d) failed: %s", p->ex->N, cudaGetErrorString(err));
-        p->launches++;
-        return 0;
+        const int kind = co ? PK_XCONV_CO : PK_XCONV;
+        auto rec = [&] {
+            char extra[64];
+            snprintf(extra, sizeof(extra), ", \"mult\": %llu", (unsigned long long)(size_t)mult);
+            record_op<T>(p->ops, kPassNames[kind], 1, p->ex->N, C, false, co, false, a, extra);
+        };
+        return issue(p, 2, 2, rec, [&] { return p->ex->launch[kind](&r, p->sms, p->stream); }, "convolution X pass", p->ex->N);
     }
 };
-
 
 // exchange offsets (api.cpp:84-133, 613-627): where chunk (sender s -> receiver r) starts
 static long long send_off(const Geom& g, int s, int r, int dir)
@@ -1613,13 +1577,12 @@ static int flags_wait(dfft_plan p, int which, unsigned long long value, cudaStre
     return 0;
 }
 
-static int nccl_exchange(dfft_plan p, const void* sendbuf, void* recvbuf)
+static int nccl_exchange(dfft_plan p, const void* sendbuf, void* recvbuf, int dir)
 {
     const Geom& g = p->g;
-    const int dir = p->direction;
     if (p->dry) {   // describe the all-to-all: element offsets and counts of every chunk this device sends
         char buf[160];
-        std::string o = "{\"op\": \"alltoall\", \"phase\": " + std::to_string(p->phase_base) + ", ";
+        std::string o = "{\"op\": \"alltoall\", \"phase\": " + std::to_string(p->conv && dir == DFFT_BACKWARD ? 2 : 0) + ", ";
         snprintf(buf, sizeof(buf), "\"send\": %llu, \"recv\": %llu, \"esz\": %zu, \"chunks\": [", (unsigned long long)(size_t)sendbuf,
                  (unsigned long long)(size_t)recvbuf, p->esz);
         o += buf;
@@ -1720,7 +1683,7 @@ template <typename T> static int fwd_pipelined(dfft_plan p)
             if (k == 0) rc = Pass<T>::zy_fused_part0(p, p->buf1, p->mid, zk, base);
             else {
                 // part k-1 must have arrived from every sender before the kernel whose X role consumes it starts: a one-CTA gate
-                // kernel, not a poll inside the full-grid kernel (which would hold every SM slot while it waits, see execute_fused)
+                // kernel, not a poll inside the full-grid kernel (which would hold every SM slot while it waits, see execute_slabs)
                 if ((rc = flags_wait(p, 2 + k - 1, p->epoch, A))) return rc;
                 rc = Pass<T>::yx_fused(p, p->mid, zk, k, base, eoff(p->work, (long long)(k - 1) * g.n0 * p->n1l * zk, p->esz), p->buf2);
             }
@@ -1749,7 +1712,7 @@ template <typename T> static int fwd_pipelined(dfft_plan p)
                           : eoff(p->sendbuf, ((long long)k * P + q) * p->n0l * g.yd() * zk, p->esz);
         if (k == 0 && p->fuse) rc = Pass<T>::zy_fused_part0(p, p->buf1, p->mid, zk, base);
         else {
-            if (k == 0 && (rc = Pass<T>::z_pass(p, p->buf1, p->mid, false))) return rc;
+            if (k == 0 && (rc = Pass<T>::z_pass(p, p->buf1, p->mid, false, DFFT_FORWARD))) return rc;
             rc = Pass<T>::y_part(p, p->mid, zk, k, base, k > 0 ? cap : 0);
         }
         if (rc) return rc;
@@ -1842,7 +1805,7 @@ template <typename T> static int bwd_pipelined(dfft_plan p)
         // inverse Z pass of the whole slab on the receive stream (Pass::z_pass launches on the plan stream: join first)
         CU(ev_record_on(p, p->ev_join, B));
         CU(stream_wait(p, A, p->ev_join));
-        if ((rc = Pass<T>::z_pass(p, p->buf2, p->buf2, scale))) return rc;
+        if ((rc = Pass<T>::z_pass(p, p->buf2, p->buf2, scale, DFFT_BACKWARD))) return rc;
         CU(ev_record(p, p->evb[1]));
         CU(ev_record(p, p->pev[0][0])); CU(ev_record(p, p->pev[0][1]));
         if (p2p && (rc = flags_signal(p, 0, p->epoch, A))) return rc;
@@ -1859,207 +1822,96 @@ template <typename T> static int bwd_pipelined(dfft_plan p)
     return 0;
 }
 
-template <typename T> static int execute_fused(dfft_plan p)
+// ---- the non-pipelined slab schedule: forward half, X step, backward half -------------------------------------------------
+// C2C / R2C forward = forward half + forward X, backward = backward X + backward half, convolve = forward half + fused X pass +
+// backward half.  P2P gates and signals: the completion SIGNALS ride inside the pass kernels where the plan has done_ctr (their
+// last CTA publishes the flags: fewer launches, DFFT_SIGNAL_KERNELS=1 restores the separate launches).  The GATES stay one-CTA
+// kernels on purpose: a full-grid kernel that spins on a peer's flag holds every SM slot, and with two plans in flight per device
+// (bench.py's e2e leg) device A can then wait for a kernel of device B that cannot start because B's SMs are held by a kernel
+// waiting for A.  Flag words: ready[r] = e once receiver r has consumed its receive buffer of epoch e, arrive[s] = e once sender
+// s has finished writing this device's receive buffer of epoch e.
+static bool folds(dfft_plan p) { return p->P > 1 && p->xmode == DFFT_EXCHANGE_P2P && p->done_ctr != nullptr && !p->dry; }
+
+// x-slab (bufferDev1) -> the receive buffer `work` [x][y_l][z'] of every device, epoch e: the Z step (fused with Y, or Z then Y),
+// with the Y pass's store doing the pack (into `stage`, NCCL) or the all-to-all itself (into the peers' `work`, P2P)
+template <typename T> static int fwd_half(dfft_plan p, unsigned long long e, bool fused, bool fused_tma)
 {
     const Geom& g = p->g;
-    const int P = p->P, me = p->me;
+    const int P = p->P;
+    const bool p2p = P > 1 && p->xmode == DFFT_EXCHANGE_P2P;
+    void* zout = p2p ? p->stage : p->work;   // Z output; one device: Y runs in place in `work`
+    void* ydst = P == 1 ? p->work : nullptr;
+    const int ymode = P == 1 ? 0 : 1;
+    void* base[DFFT_MAX_CHUNKS];
+    if (P > 1)
+        for (int q = 0; q < P; q++)
+            base[q] = p2p ? eoff(p->peer_work[q], recv_off(g, p->me, q, DFFT_FORWARD), p->esz) : eoff(p->stage, send_off(g, p->me, q, DFFT_FORWARD), p->esz);
+    Fold fy; fy.sig_which = 1; fy.sig_val = e; fy.ctr = 0;   // "arrived" from the Y pass's last CTA
+    const Fold* fold = folds(p) ? &fy : nullptr;
     int rc;
-    p->launches = 0;
-    CU(ev_record(p, p->ev[0]));
-    if (p->pipe) return p->direction == DFFT_FORWARD ? fwd_pipelined<T>(p) : bwd_pipelined<T>(p);
-    if (p->direction == DFFT_FORWARD) {
-        // t0 (+t1): Z pass out of place (bufferDev1 survives), Y pass with the pack (and, P2P, the
-        // all-to-all) folded into its store
-        if (P == 1) {
-            if (p->fuse_tma) {
-                if ((rc = Pass<T>::zy_fused_tma(p, p->buf1, p->work))) return rc;
-            } else if (p->fuse) {
-                if ((rc = Pass<T>::zy_fused(p, p->buf1, p->work, p->work, 0, nullptr, false))) return rc;
-            } else {
-                if ((rc = Pass<T>::z_pass(p, p->buf1, p->work, false))) return rc;
-                if ((rc = Pass<T>::y_pass(p, p->work, p->work, 0, nullptr))) return rc;
-            }
-            CU(ev_record(p, p->ev[1]));
-            CU(ev_record(p, p->ev[2]));
-            if (p->natural) { if ((rc = Pass<T>::x_natural(p, p->work, p->buf2))) return rc; }
-            else if ((rc = Pass<T>::x_fwd(p, p->work, p->buf2))) return rc;
-        } else if (p->xmode == DFFT_EXCHANGE_P2P) {
-            void* base[DFFT_MAX_CHUNKS];
-            for (int q = 0; q < P; q++) base[q] = eoff(p->peer_work[q], recv_off(g, me, q, DFFT_FORWARD), p->esz);
-            p->epoch++;
-            if (p->overlap) {
-                if ((rc = flags_wait(p, 0, p->epoch - 1))) return rc;   // every receiver has consumed the previous epoch
-                if ((rc = Pass<T>::fwd_overlapped(p, base))) return rc;
-                CU(ev_record(p, p->ev[1]));
-                CU(ev_record(p, p->ev[2]));
-                if ((rc = flags_signal(p, 0, p->epoch))) return rc;
-                CU(ev_record(p, p->ev[3]));
-                p->timed = true;
-                return 0;
-            }
-            // The completion SIGNALS ride inside the pass kernels (their last CTA publishes the flags: 4 launches per transform
-            // instead of 6, DFFT_SIGNAL_KERNELS=1 restores the separate launches).  The GATES stay one-CTA kernels on purpose: a
-            // full-grid kernel that spins on a peer's flag holds every SM slot, and with two plans in flight per device (bench.py's
-            // e2e leg) device A can then wait for a kernel of device B that cannot start because B's SMs are held by a kernel waiting for A.
-            const bool fold = p->done_ctr != nullptr && !p->dry;
-            Fold fy; fy.sig_which = 1; fy.sig_val = p->epoch; fy.ctr = 0;
-            Fold fx; fx.sig_which = 0; fx.sig_val = p->epoch; fx.ctr = 1;
-            const bool foldx = fold && Pass<T>::x_fwd_folds(p);
-            if (p->fuse) {
-                if ((rc = flags_wait(p, 0, p->epoch - 1))) return rc;   // every receiver has consumed the previous epoch
-                if ((rc = Pass<T>::zy_fused(p, p->buf1, p->buf2, nullptr, 1, base, false, fold ? &fy : nullptr))) return rc;
-            } else {
-                if ((rc = Pass<T>::z_pass(p, p->buf1, p->buf2, false))) return rc;
-                if ((rc = flags_wait(p, 0, p->epoch - 1))) return rc;
-                if ((rc = Pass<T>::y_pass(p, p->buf2, nullptr, 1, base, fold ? &fy : nullptr))) return rc;
-            }
-            if (!fold && (rc = flags_signal(p, 1, p->epoch))) return rc;
-            CU(ev_record(p, p->ev[1]));
-            if ((rc = flags_wait(p, 1, p->epoch))) return rc;        // t2: exposed wait for the slowest sender
-            CU(ev_record(p, p->ev[2]));
-            if ((rc = Pass<T>::x_fwd(p, p->work, p->buf2, foldx ? &fx : nullptr))) return rc;
-            if (!foldx && (rc = flags_signal(p, 0, p->epoch))) return rc;
-        } else {
-            void* base[DFFT_MAX_CHUNKS];
-            for (int q = 0; q < P; q++) base[q] = eoff(p->buf2, send_off(g, me, q, DFFT_FORWARD), p->esz);
-            if (p->fuse) {
-                if ((rc = Pass<T>::zy_fused(p, p->buf1, p->work, nullptr, 1, base, false))) return rc;
-            } else {
-                if ((rc = Pass<T>::z_pass(p, p->buf1, p->work, false))) return rc;
-                if ((rc = Pass<T>::y_pass(p, p->work, nullptr, 1, base))) return rc;
-            }
-            CU(ev_record(p, p->ev[1]));
-            if ((rc = nccl_exchange(p, p->buf2, p->work))) return rc;
-            CU(ev_record(p, p->ev[2]));
-            if ((rc = Pass<T>::x_fwd(p, p->work, p->buf2))) return rc;
-        }
-        CU(ev_record(p, p->ev[3]));
-    } else {
-        const bool scale = (p->flags & DFFT_SCALE_BACKWARD) != 0;
-        if (P == 1) {
-            if (p->natural) { if ((rc = Pass<T>::x_natural(p, p->buf1, p->buf2))) return rc; }
-            else if ((rc = Pass<T>::x_bwd(p, p->buf1, p->buf2, nullptr))) return rc;
-            CU(ev_record(p, p->ev[1]));
-            CU(ev_record(p, p->ev[2]));
-            if (p->fuse) { if ((rc = Pass<T>::zy_fused(p, p->buf2, p->buf2, nullptr, 0, nullptr, scale))) return rc; }
-            else if ((rc = Pass<T>::y_pass(p, p->buf2, p->buf2, 0, nullptr))) return rc;
-        } else if (p->xmode == DFFT_EXCHANGE_P2P) {
-            p->epoch++;
-            const bool fold = p->done_ctr != nullptr && !p->dry;
-            Fold fxb; fxb.sig_which = 1; fxb.sig_val = p->epoch; fxb.ctr = 0;      // signals folded, gates separate (see the forward branch)
-            Fold fyz; fyz.ctr = 1;
-            if (p->fuse) { fyz.sig_which = 0; fyz.sig_val = p->epoch; }   // the fused kernel is the last one: it also signals "consumed"
-            if ((rc = flags_wait(p, 0, p->epoch - 1))) return rc;
-            void* base[DFFT_MAX_CHUNKS];
-            for (int q = 0; q < P; q++) base[q] = eoff(p->peer_work[q], recv_off(g, me, q, DFFT_BACKWARD), p->esz);
-            if ((rc = Pass<T>::x_bwd(p, p->buf1, nullptr, base, fold ? &fxb : nullptr))) return rc;
-            if (!fold && (rc = flags_signal(p, 1, p->epoch))) return rc;
-            CU(ev_record(p, p->ev[1]));
-            if ((rc = flags_wait(p, 1, p->epoch))) return rc;
-            CU(ev_record(p, p->ev[2]));
-            void* cb[DFFT_MAX_CHUNKS];
-            for (int q = 0; q < P; q++) cb[q] = eoff(p->work, (long long)q * p->n0l * g.yd() * g.n2, p->esz);
-            if (p->fuse) { if ((rc = Pass<T>::zy_fused(p, nullptr, p->buf2, nullptr, 2, cb, scale, fold ? &fyz : nullptr))) return rc; }
-            else if ((rc = Pass<T>::y_pass(p, nullptr, p->buf2, 2, cb, fold ? &fyz : nullptr))) return rc;
-            if (!(fold && p->fuse) && (rc = flags_signal(p, 0, p->epoch))) return rc;
-        } else {
-            if ((rc = Pass<T>::x_bwd(p, p->buf1, p->buf2, nullptr))) return rc;
-            CU(ev_record(p, p->ev[1]));
-            if ((rc = nccl_exchange(p, p->buf2, p->work))) return rc;
-            CU(ev_record(p, p->ev[2]));
-            void* cb[DFFT_MAX_CHUNKS];
-            for (int q = 0; q < P; q++) cb[q] = eoff(p->work, (long long)q * p->n0l * g.yd() * g.n2, p->esz);
-            if (p->fuse) { if ((rc = Pass<T>::zy_fused(p, nullptr, p->buf2, nullptr, 2, cb, scale))) return rc; }
-            else if ((rc = Pass<T>::y_pass(p, nullptr, p->buf2, 2, cb))) return rc;
-        }
-        if (!p->fuse && (rc = Pass<T>::z_pass(p, p->buf2, p->buf2, scale))) return rc;
-        CU(ev_record(p, p->ev[3]));
+    if (fused_tma) return Pass<T>::zy_fused_tma(p, p->buf1, p->work);
+    if (fused) {
+        if (p2p && (rc = flags_wait(p, 0, e - 1))) return rc;   // every receiver has consumed the previous epoch
+        return Pass<T>::zy_fused(p, p->buf1, zout, ydst, ymode, base, false, fold, DFFT_FORWARD);
     }
-    p->timed = true;
+    if (p->r2c) rc = Pass<T>::z_real(p, p->buf1, zout, false, DFFT_FORWARD);
+    else rc = Pass<T>::z_pass(p, p->buf1, zout, false, DFFT_FORWARD);
+    if (rc) return rc;
+    if (p2p && (rc = flags_wait(p, 0, e - 1))) return rc;
+    return Pass<T>::y_pass(p, zout, ydst, ymode, base, fold, DFFT_FORWARD);
+}
+
+// what follows the pass that sent epoch e: its "arrived" signal unless folded, event `sent`, the arrival wait (P2P) or the NCCL
+// all-to-all of `stage` into `work`, event `arrived` (either event may be null)
+static int deliver(dfft_plan p, unsigned long long e, int dir, cudaEvent_t sent, cudaEvent_t arrived)
+{
+    const bool p2p = p->P > 1 && p->xmode == DFFT_EXCHANGE_P2P;
+    int rc;
+    if (p2p && !folds(p) && (rc = flags_signal(p, 1, e))) return rc;
+    if (sent) CU(ev_record(p, sent));
+    if (p2p && (rc = flags_wait(p, 1, e))) return rc;   // exposed wait for the slowest sender
+    if (p->P > 1 && !p2p && (rc = nccl_exchange(p, p->stage, p->work, dir))) return rc;
+    if (arrived) CU(ev_record(p, arrived));
     return 0;
 }
 
-// R2C / C2R plans: the C2C Y and X passes and exchanges over the nzh half-spectrum columns around the real-data Z pass; never fused
-// or pipelined.  The user's real buffer never holds complex data: where the C2C schedules borrow `out` (the forward Z output of the
-// P2P exchange, the NCCL send buffer, the backward Y output) an R2C plan uses its own `mid`.
-template <typename T> static int execute_real(dfft_plan p)
+// receive buffer -> x-slab (bufferDev2), epoch e: Y from the chunks of `rbuf` (one device: from `src`) into `ybwd`, then Z (fused
+// with Y, in place, or the real-data pass into bufferDev2), with "consumed" signalled once Y has read the receive buffer
+template <typename T> static int bwd_half(dfft_plan p, unsigned long long e, bool fused, const void* src, void* rbuf, bool scale)
 {
     const Geom& g = p->g;
-    const int P = p->P, me = p->me;
+    const int P = p->P;
+    const bool p2p = P > 1 && p->xmode == DFFT_EXCHANGE_P2P;
+    void* cb[DFFT_MAX_CHUNKS];
+    if (P > 1)
+        for (int q = 0; q < P; q++) cb[q] = eoff(rbuf, (long long)q * p->n0l * g.yd() * g.n2, p->esz);
+    const void* ysrc = P == 1 ? src : nullptr;
+    const int ymode = P == 1 ? 0 : 2;
+    Fold fyz; fyz.sig_which = 0; fyz.sig_val = e; fyz.ctr = 1;   // the fused kernel is the last reader: its last CTA signals "consumed"
+    const bool fold = fused && folds(p);
     int rc;
-    p->launches = 0;
-    CU(ev_record(p, p->ev[0]));
-    if (p->direction == DFFT_FORWARD) {
-        if (P == 1) {
-            if ((rc = Pass<T>::z_real(p, p->buf1, p->work, false))) return rc;
-            if ((rc = Pass<T>::y_pass(p, p->work, p->work, 0, nullptr))) return rc;
-            CU(ev_record(p, p->ev[1]));
-            CU(ev_record(p, p->ev[2]));
-            if (p->natural) { if ((rc = Pass<T>::x_natural(p, p->work, p->buf2))) return rc; }
-            else if ((rc = Pass<T>::x_fwd(p, p->work, p->buf2))) return rc;
-        } else if (p->xmode == DFFT_EXCHANGE_P2P) {
-            void* base[DFFT_MAX_CHUNKS];
-            for (int q = 0; q < P; q++) base[q] = eoff(p->peer_work[q], recv_off(g, me, q, DFFT_FORWARD), p->esz);
-            p->epoch++;
-            const bool fold = p->done_ctr != nullptr && !p->dry;   // completion signals inside the pass kernels, as in execute_fused
-            Fold fy; fy.sig_which = 1; fy.sig_val = p->epoch; fy.ctr = 0;
-            Fold fx; fx.sig_which = 0; fx.sig_val = p->epoch; fx.ctr = 1;
-            const bool foldx = fold && Pass<T>::x_fwd_folds(p);
-            if ((rc = Pass<T>::z_real(p, p->buf1, p->mid, false))) return rc;
-            if ((rc = flags_wait(p, 0, p->epoch - 1))) return rc;   // every receiver has consumed the previous epoch
-            if ((rc = Pass<T>::y_pass(p, p->mid, nullptr, 1, base, fold ? &fy : nullptr))) return rc;
-            if (!fold && (rc = flags_signal(p, 1, p->epoch))) return rc;
-            CU(ev_record(p, p->ev[1]));
-            if ((rc = flags_wait(p, 1, p->epoch))) return rc;
-            CU(ev_record(p, p->ev[2]));
-            if ((rc = Pass<T>::x_fwd(p, p->work, p->buf2, foldx ? &fx : nullptr))) return rc;
-            if (!foldx && (rc = flags_signal(p, 0, p->epoch))) return rc;
-        } else {
-            void* base[DFFT_MAX_CHUNKS];
-            for (int q = 0; q < P; q++) base[q] = eoff(p->mid, send_off(g, me, q, DFFT_FORWARD), p->esz);
-            if ((rc = Pass<T>::z_real(p, p->buf1, p->work, false))) return rc;
-            if ((rc = Pass<T>::y_pass(p, p->work, nullptr, 1, base))) return rc;
-            CU(ev_record(p, p->ev[1]));
-            if ((rc = nccl_exchange(p, p->mid, p->work))) return rc;
-            CU(ev_record(p, p->ev[2]));
-            if ((rc = Pass<T>::x_fwd(p, p->work, p->buf2))) return rc;
-        }
-    } else {
-        const bool scale = (p->flags & DFFT_SCALE_BACKWARD) != 0;
-        if (P == 1) {
-            if (p->natural) { if ((rc = Pass<T>::x_natural(p, p->buf1, p->work))) return rc; }
-            else if ((rc = Pass<T>::x_bwd(p, p->buf1, p->work, nullptr))) return rc;
-            CU(ev_record(p, p->ev[1]));
-            CU(ev_record(p, p->ev[2]));
-            if ((rc = Pass<T>::y_pass(p, p->work, p->work, 0, nullptr))) return rc;
-            if ((rc = Pass<T>::z_real(p, p->work, p->buf2, scale))) return rc;
-        } else {
-            void* cb[DFFT_MAX_CHUNKS];
-            for (int q = 0; q < P; q++) cb[q] = eoff(p->work, (long long)q * p->n0l * g.yd() * g.n2, p->esz);
-            if (p->xmode == DFFT_EXCHANGE_P2P) {
-                p->epoch++;
-                const bool fold = p->done_ctr != nullptr && !p->dry;
-                Fold fxb; fxb.sig_which = 1; fxb.sig_val = p->epoch; fxb.ctr = 0;
-                if ((rc = flags_wait(p, 0, p->epoch - 1))) return rc;
-                void* base[DFFT_MAX_CHUNKS];
-                for (int q = 0; q < P; q++) base[q] = eoff(p->peer_work[q], recv_off(g, me, q, DFFT_BACKWARD), p->esz);
-                if ((rc = Pass<T>::x_bwd(p, p->buf1, nullptr, base, fold ? &fxb : nullptr))) return rc;
-                if (!fold && (rc = flags_signal(p, 1, p->epoch))) return rc;
-                CU(ev_record(p, p->ev[1]));
-                if ((rc = flags_wait(p, 1, p->epoch))) return rc;
-                CU(ev_record(p, p->ev[2]));
-                if ((rc = Pass<T>::y_pass(p, nullptr, p->mid, 2, cb))) return rc;
-                if ((rc = flags_signal(p, 0, p->epoch))) return rc;   // the receive buffer is consumed
-            } else {
-                if ((rc = Pass<T>::x_bwd(p, p->buf1, p->mid, nullptr))) return rc;
-                CU(ev_record(p, p->ev[1]));
-                if ((rc = nccl_exchange(p, p->mid, p->work))) return rc;
-                CU(ev_record(p, p->ev[2]));
-                if ((rc = Pass<T>::y_pass(p, nullptr, p->mid, 2, cb))) return rc;
-            }
-            if ((rc = Pass<T>::z_real(p, p->mid, p->buf2, scale))) return rc;
-        }
-    }
+    if (fused) rc = Pass<T>::zy_fused(p, ysrc, p->ybwd, nullptr, ymode, cb, scale, fold ? &fyz : nullptr, DFFT_BACKWARD);
+    else rc = Pass<T>::y_pass(p, ysrc, p->ybwd, ymode, cb, nullptr, DFFT_BACKWARD);
+    if (rc) return rc;
+    if (p2p && !fold && (rc = flags_signal(p, 0, e))) return rc;
+    if (p->r2c) return Pass<T>::z_real(p, p->ybwd, p->buf2, scale, DFFT_BACKWARD);
+    if (!fused) return Pass<T>::z_pass(p, p->buf2, p->buf2, scale, DFFT_BACKWARD);
+    return 0;
+}
+
+// Overlapped forward (P2P): the whole transform in one kernel, t3 behind the per-part arrivals
+template <typename T> static int execute_overlapped(dfft_plan p)
+{
+    const Geom& g = p->g;
+    int rc;
+    void* base[DFFT_MAX_CHUNKS];
+    for (int q = 0; q < p->P; q++) base[q] = eoff(p->peer_work[q], recv_off(g, p->me, q, DFFT_FORWARD), p->esz);
+    p->epoch++;
+    if ((rc = flags_wait(p, 0, p->epoch - 1))) return rc;   // every receiver has consumed the previous epoch
+    if ((rc = Pass<T>::fwd_overlapped(p, base))) return rc;
+    CU(ev_record(p, p->ev[1]));
+    CU(ev_record(p, p->ev[2]));
+    if ((rc = flags_signal(p, 0, p->epoch))) return rc;
     CU(ev_record(p, p->ev[3]));
     p->timed = true;
     return 0;
@@ -2082,109 +1934,54 @@ template <typename T> static int execute_real(dfft_plan p)
 //     the previous execute, the only reader of r's work2, is done;
 //   * the waits are >= tests on monotonic words: the previous execute's e2 (= e1 - 1) never satisfies the wait for e1, and a sender
 //     publishes e2 only from its fused X pass, after every store of its forward Y pass.
-template <typename T> static int execute_convolve(dfft_plan p, const void* mult)
+template <typename T> static int execute_slabs(dfft_plan p, const void* mult)
 {
     const Geom& g = p->g;
     const int P = p->P, me = p->me;
-    const bool p2p = p->xmode == DFFT_EXCHANGE_P2P;
+    const bool p2p = P > 1 && p->xmode == DFFT_EXCHANGE_P2P;
     int rc;
-    struct Half {
-        dfft_plan p;
-        void set(int h) {   // h = 0 forward half, 1 backward half, -1 between executes
-            p->direction = h == 1 ? DFFT_BACKWARD : DFFT_FORWARD;
-            p->fuse = h < 0 ? (p->conv_fuse[0] || p->conv_fuse[1]) : p->conv_fuse[h];
-            p->fuse_tma = h == 0 && p->conv_fuse_tma;
-            p->phase_base = h == 1 ? 2 : 0;
-        }
-        ~Half() { set(-1); }
-    } half{p};
     p->launches = 0;
     CU(ev_record(p, p->ev[0]));
-    half.set(0);
-    const bool fold = p2p && p->done_ctr != nullptr && !p->dry;   // completion signals inside the pass kernels, as in execute_fused
-    unsigned long long e1 = 0, e2 = 0;
-    void* base[DFFT_MAX_CHUNKS];
-    if (P == 1) {
-        if (p->r2c) {
-            if ((rc = Pass<T>::z_real(p, p->buf1, p->work, false))) return rc;
-            if ((rc = Pass<T>::y_pass(p, p->work, p->work, 0, nullptr))) return rc;
-        } else if (p->fuse_tma) {
-            if ((rc = Pass<T>::zy_fused_tma(p, p->buf1, p->work))) return rc;
-        } else if (p->fuse) {
-            if ((rc = Pass<T>::zy_fused(p, p->buf1, p->work, p->work, 0, nullptr, false))) return rc;
-        } else {
-            if ((rc = Pass<T>::z_pass(p, p->buf1, p->work, false))) return rc;
-            if ((rc = Pass<T>::y_pass(p, p->work, p->work, 0, nullptr))) return rc;
-        }
-    } else if (p2p) {
+    if (p->pipe) return p->direction == DFFT_FORWARD ? fwd_pipelined<T>(p) : bwd_pipelined<T>(p);
+    if (p->overlap) return execute_overlapped<T>(p);
+    unsigned long long e1 = 0, e2 = 0;   // epochs of the forward and the backward exchange (one of them for C2C / R2C)
+    if (p2p) {
         e1 = ++p->epoch;
-        e2 = ++p->epoch;
-        for (int q = 0; q < P; q++) base[q] = eoff(p->peer_work[q], recv_off(g, me, q, DFFT_FORWARD), p->esz);
-        Fold fy; fy.sig_which = 1; fy.sig_val = e1; fy.ctr = 0;
-        if (p->r2c) {
-            if ((rc = Pass<T>::z_real(p, p->buf1, p->mid, false))) return rc;
-            if ((rc = flags_wait(p, 0, e1 - 1))) return rc;
-            if ((rc = Pass<T>::y_pass(p, p->mid, nullptr, 1, base, fold ? &fy : nullptr))) return rc;
-        } else if (p->fuse) {
-            if ((rc = flags_wait(p, 0, e1 - 1))) return rc;
-            if ((rc = Pass<T>::zy_fused(p, p->buf1, p->mid, nullptr, 1, base, false, fold ? &fy : nullptr))) return rc;
-        } else {
-            if ((rc = Pass<T>::z_pass(p, p->buf1, p->mid, false))) return rc;
-            if ((rc = flags_wait(p, 0, e1 - 1))) return rc;
-            if ((rc = Pass<T>::y_pass(p, p->mid, nullptr, 1, base, fold ? &fy : nullptr))) return rc;
-        }
-        if (!fold && (rc = flags_signal(p, 1, e1))) return rc;
-        if ((rc = flags_wait(p, 1, e1))) return rc;
-    } else {
-        for (int q = 0; q < P; q++) base[q] = eoff(p->mid, send_off(g, me, q, DFFT_FORWARD), p->esz);
-        if (p->r2c) {
-            if ((rc = Pass<T>::z_real(p, p->buf1, p->work, false))) return rc;
-            if ((rc = Pass<T>::y_pass(p, p->work, nullptr, 1, base))) return rc;
-        } else if (p->fuse) {
-            if ((rc = Pass<T>::zy_fused(p, p->buf1, p->work, nullptr, 1, base, false))) return rc;
-        } else {
-            if ((rc = Pass<T>::z_pass(p, p->buf1, p->work, false))) return rc;
-            if ((rc = Pass<T>::y_pass(p, p->work, nullptr, 1, base))) return rc;
-        }
-        if ((rc = nccl_exchange(p, p->mid, p->work))) return rc;
+        e2 = p->conv ? ++p->epoch : e1;
     }
-    CU(ev_record(p, p->ev[1]));
-    if (P == 1) {
-        if ((rc = Pass<T>::x_conv(p, p->work, p->work, nullptr, mult))) return rc;
-    } else if (p2p) {
-        for (int q = 0; q < P; q++) base[q] = eoff(p->peer_work2[q], recv_off(g, me, q, DFFT_BACKWARD), p->esz);
+    void* base[DFFT_MAX_CHUNKS];
+    if (p->conv) {
+        if ((rc = fwd_half<T>(p, e1, p->conv_fuse[0], p->conv_fuse_tma))) return rc;
+        if ((rc = deliver(p, e1, DFFT_FORWARD, nullptr, p->ev[1]))) return rc;
         Fold fc; fc.sig_which = 1; fc.sig_val = e2; fc.ctr = 1;
-        if ((rc = Pass<T>::x_conv(p, p->work, nullptr, base, mult, fold ? &fc : nullptr))) return rc;
-        if (!fold && (rc = flags_signal(p, 1, e2))) return rc;
+        if (P == 1) rc = Pass<T>::x_conv(p, p->work, p->work, nullptr, mult, nullptr);
+        else if (p2p) {
+            for (int q = 0; q < P; q++) base[q] = eoff(p->peer_work2[q], recv_off(g, me, q, DFFT_BACKWARD), p->esz);
+            rc = Pass<T>::x_conv(p, p->work, nullptr, base, mult, folds(p) ? &fc : nullptr);
+        } else rc = Pass<T>::x_conv(p, p->work, p->stage, nullptr, mult, nullptr);   // [x][y_l][z'] is grouped by destination
+        if (rc) return rc;
+        if ((rc = deliver(p, e2, DFFT_BACKWARD, p->ev[2], nullptr))) return rc;
+        if ((rc = bwd_half<T>(p, e2, p->conv_fuse[1], p->work, p2p ? p->work2 : p->work, false))) return rc;
+    } else if (p->direction == DFFT_FORWARD) {
+        if ((rc = fwd_half<T>(p, e1, p->fuse, p->fuse_tma))) return rc;
+        if ((rc = deliver(p, e1, DFFT_FORWARD, p->ev[1], p->ev[2]))) return rc;
+        Fold fx; fx.sig_which = 0; fx.sig_val = e1; fx.ctr = 1;   // "consumed" from the X pass's last CTA (not on the TMA kernel)
+        const bool foldx = folds(p) && Pass<T>::x_fwd_folds(p);
+        if (p->natural) rc = Pass<T>::x_natural(p, p->work, p->buf2);
+        else rc = Pass<T>::x_fwd(p, p->work, p->buf2, foldx ? &fx : nullptr);
+        if (rc) return rc;
+        if (p2p && !foldx && (rc = flags_signal(p, 0, e1))) return rc;
     } else {
-        if ((rc = Pass<T>::x_conv(p, p->work, p->mid, nullptr, mult))) return rc;   // [x][y_l][z'] is grouped by destination
-    }
-    CU(ev_record(p, p->ev[2]));
-    half.set(1);
-    if (P == 1) {
-        if (p->r2c) {
-            if ((rc = Pass<T>::y_pass(p, p->work, p->work, 0, nullptr))) return rc;
-            if ((rc = Pass<T>::z_real(p, p->work, p->buf2, false))) return rc;
-        } else if (p->fuse) {
-            if ((rc = Pass<T>::zy_fused(p, p->work, p->buf2, nullptr, 0, nullptr, false))) return rc;
-        } else {
-            if ((rc = Pass<T>::y_pass(p, p->work, p->buf2, 0, nullptr))) return rc;
-            if ((rc = Pass<T>::z_pass(p, p->buf2, p->buf2, false))) return rc;
-        }
-    } else {
-        void* rbuf = p2p ? p->work2 : p->work;
-        if (p2p) { if ((rc = flags_wait(p, 1, e2))) return rc; }
-        else if ((rc = nccl_exchange(p, p->mid, p->work))) return rc;
-        void* cb[DFFT_MAX_CHUNKS];
-        for (int q = 0; q < P; q++) cb[q] = eoff(rbuf, (long long)q * p->n0l * g.yd() * g.n2, p->esz);
-        Fold fyz; fyz.sig_which = 0; fyz.sig_val = e2; fyz.ctr = 1;   // the fused kernel's last CTA signals "work2 consumed"
-        const bool fold_yz = fold && p->fuse && !p->r2c;
-        if (p->fuse && !p->r2c) {
-            if ((rc = Pass<T>::zy_fused(p, nullptr, p->buf2, nullptr, 2, cb, false, fold_yz ? &fyz : nullptr))) return rc;
-        } else if ((rc = Pass<T>::y_pass(p, nullptr, p->r2c ? p->mid : p->buf2, 2, cb))) return rc;
-        if (p2p && !fold_yz && (rc = flags_signal(p, 0, e2))) return rc;
-        if (p->r2c) { if ((rc = Pass<T>::z_real(p, p->mid, p->buf2, false))) return rc; }
-        else if (!p->fuse && (rc = Pass<T>::z_pass(p, p->buf2, p->buf2, false))) return rc;
+        Fold fxb; fxb.sig_which = 1; fxb.sig_val = e1; fxb.ctr = 0;
+        if (P == 1) rc = p->natural ? Pass<T>::x_natural(p, p->buf1, p->ybwd) : Pass<T>::x_bwd(p, p->buf1, p->ybwd, nullptr);
+        else if (p2p) {
+            if ((rc = flags_wait(p, 0, e1 - 1))) return rc;
+            for (int q = 0; q < P; q++) base[q] = eoff(p->peer_work[q], recv_off(g, me, q, DFFT_BACKWARD), p->esz);
+            rc = Pass<T>::x_bwd(p, p->buf1, nullptr, base, folds(p) ? &fxb : nullptr);
+        } else rc = Pass<T>::x_bwd(p, p->buf1, p->stage, nullptr);
+        if (rc) return rc;
+        if ((rc = deliver(p, e1, DFFT_BACKWARD, p->ev[1], p->ev[2]))) return rc;
+        if ((rc = bwd_half<T>(p, e1, p->fuse, p->ybwd, p->work, (p->flags & DFFT_SCALE_BACKWARD) != 0))) return rc;
     }
     CU(ev_record(p, p->ev[3]));
     p->timed = true;
@@ -2202,11 +1999,11 @@ template <typename T> static int execute_stage(dfft_plan p, int stage)
     if (sid == 0) {          // fftZY
         void* buf = dir == DFFT_FORWARD ? p->buf1 : p->buf2;
         if (dir == DFFT_FORWARD) {
-            if ((rc = Pass<T>::z_pass(p, buf, buf, false))) return rc;
-            if ((rc = Pass<T>::y_pass(p, buf, buf, 0, nullptr))) return rc;
+            if ((rc = Pass<T>::z_pass(p, buf, buf, false, dir))) return rc;
+            if ((rc = Pass<T>::y_pass(p, buf, buf, 0, nullptr, nullptr, dir))) return rc;
         } else {
-            if ((rc = Pass<T>::y_pass(p, buf, buf, 0, nullptr))) return rc;
-            if ((rc = Pass<T>::z_pass(p, buf, buf, (p->flags & DFFT_SCALE_BACKWARD) != 0))) return rc;
+            if ((rc = Pass<T>::y_pass(p, buf, buf, 0, nullptr, nullptr, dir))) return rc;
+            if ((rc = Pass<T>::z_pass(p, buf, buf, (p->flags & DFFT_SCALE_BACKWARD) != 0, dir))) return rc;
         }
     } else if (sid == 1) {   // localTransposeUneven
         cudaError_t e = launch_pack_rows(p->buf1, p->buf2, (int)p->esz, p->n0l, g.n1, g.n2, P, dir == DFFT_FORWARD, p->sms, p->stream);
@@ -2263,8 +2060,7 @@ extern "C" int dfft_execute(dfft_plan p)
         p->timed = true;
         return 0;
     }
-    if (p->r2c) return p->prec == DFFT_DOUBLE ? execute_real<double>(p) : execute_real<float>(p);
-    return p->prec == DFFT_DOUBLE ? execute_fused<double>(p) : execute_fused<float>(p);
+    return p->prec == DFFT_DOUBLE ? execute_slabs<double>(p, nullptr) : execute_slabs<float>(p, nullptr);
 }
 
 extern "C" int dfft_execute_convolve(dfft_plan p, const void* multiplier)
@@ -2275,7 +2071,7 @@ extern "C" int dfft_execute_convolve(dfft_plan p, const void* multiplier)
     if ((uintptr_t)multiplier % p->esz) return fail(DFFT_EINVAL, "dfft_execute_convolve: the multiplier is not aligned to its complex element size (%zu bytes)", p->esz);
     if (p->dry) p->ops.clear();
     else CU(cudaSetDevice(p->device));
-    return p->prec == DFFT_DOUBLE ? execute_convolve<double>(p, multiplier) : execute_convolve<float>(p, multiplier);
+    return p->prec == DFFT_DOUBLE ? execute_slabs<double>(p, multiplier) : execute_slabs<float>(p, multiplier);
 }
 
 extern "C" int dfft_synchronize(dfft_plan p)
@@ -2380,11 +2176,7 @@ extern "C" int dfft_plan_counts(dfft_plan p, long long* ic, long long* oc, long 
 extern "C" long long dfft_debug_plan_ops(dfft_plan p, char* buf, long long cap)
 {
     if (!p) return -1;
-    std::string o = "[";
-    for (size_t i = 0; i < p->ops.size(); i++) { if (i) o += ", "; o += p->ops[i]; }
-    o += "]";
-    if (buf && cap > (long long)o.size()) memcpy(buf, o.c_str(), o.size() + 1);
-    return (long long)o.size() + 1;
+    return ops_json(p->ops, buf, cap);
 }
 
 extern "C" int dfft_plan_launches(dfft_plan p) { return p ? p->launches : 0; }
@@ -2392,13 +2184,10 @@ extern "C" int dfft_plan_exchange(dfft_plan p) { return p ? p->xmode : 0; }
 /* bit 0 / 1 / 2: the un-chunked Z / Y / X pass of this plan runs on the TMA-pipelined kernel (fft_tma.cuh) */
 extern "C" int dfft_plan_tma_mask(dfft_plan p)
 {
-    if (!p || p->dry) return 0;
+    if (!p) return 0;
     const Geom& g = p->g;
-    int m = 0;
-    if (p->tz && (p->tz->use & (1u << TMA_Z)) && (p->n0l * g.n1) % p->tz->C == 0) m |= 1;
-    if (p->ty && (p->ty->use & (1u << TMA_Y)) && g.n2 % p->ty->C == 0) m |= 2;
-    if (p->tx && (p->tx->use & (1u << (p->direction == DFFT_FORWARD ? TMA_XF : TMA_XB))) && g.n2 % p->tx->C == 0) m |= 4;
-    return m;
+    return (tma_ok(p, TMA_Z, p->n0l * g.n1) ? 1 : 0) | (tma_ok(p, TMA_Y, g.n2) ? 2 : 0) |
+           (tma_ok(p, p->direction == DFFT_FORWARD ? TMA_XF : TMA_XB, g.n2) ? 4 : 0);
 }
 /* developer hook (DFFT_DEBUG_TIMELINE=1, single-kernel forward path): device-side timeline of the last execute, microseconds
  * relative to the kernel's start: [0] end of phase 0, [1] first X tile, [2] kernel end, [3..5] mean us per Z / Y / X tile,
@@ -2650,8 +2439,7 @@ extern "C" long long dfft_debug_lines_ops(int n, long long stride, long long nli
                                           int precision, int direction, int two_d, char* buf, long long cap)
 {
     dfft_lines_plan_s lp;
-    dfft_plan_s rec;   // only its `ops` vector is used
-    rec.dry = true;
+    std::vector<std::string> ops;
     lp.prec = precision;
     int rc = 0;
     if (two_d) {
@@ -2667,7 +2455,6 @@ extern "C" long long dfft_debug_lines_ops(int n, long long stride, long long nli
         lp.npass = 1;
     }
     if (rc) return rc;
-    static const char* names[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW", "Z_R2C", "Z_C2R"};
     for (int k = 0; k < lp.npass; k++) {
         const LinePass& ps = lp.pass[(direction == DFFT_BACKWARD && !lp.ordered) ? lp.npass - 1 - k : k];
         TileArgs<double> a{};
@@ -2675,14 +2462,10 @@ extern "C" long long dfft_debug_lines_ops(int n, long long stride, long long nli
         a.ia = ps.ia; a.oa = ps.oa; a.G = ps.G; a.W = ps.W; a.ntiles = ps.ntiles;
         a.inv = direction == DFFT_BACKWARD; a.tw_n = ps.tw_n;
         const int C = ps.kind == PK_Z ? ps.e->z_C : (ps.kind == PK_Y ? ps.e->s_C : ps.e->x_C);
-        record_op<double>(&rec, names[ps.kind], k, ps.e->N, C, false, false, ps.kind == PK_XF_TW, a);
+        record_op<double>(ops, kPassNames[ps.kind], k, ps.e->N, C, false, false, ps.kind == PK_XF_TW, a);
     }
     lp.temp = nullptr;
-    std::string o = "[";
-    for (size_t i = 0; i < rec.ops.size(); i++) { if (i) o += ", "; o += rec.ops[i]; }
-    o += "]";
-    if (buf && cap > (long long)o.size()) memcpy(buf, o.c_str(), o.size() + 1);
-    return (long long)o.size() + 1;
+    return ops_json(ops, buf, cap);
 }
 
 // ---- real lines: R2C / C2R over densely packed lines (1-D) and the rows of row-major matrices (2-D) --------------------------
@@ -2825,11 +2608,9 @@ extern "C" long long dfft_debug_real_lines_ops(int n, int ny, long long batch, i
 {
     if (direction != DFFT_FORWARD && direction != DFFT_BACKWARD) return fail(DFFT_EINVAL, "bad direction");
     dfft_lines_plan_s lp;
-    dfft_plan_s rec;   // only its `ops` vector is used
-    rec.dry = true;
+    std::vector<std::string> ops;
     const int rc = make_real_lines(&lp, n, ny, batch, precision, two_d != 0, true);
     if (rc) return rc;
-    static const char* names[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW", "Z_R2C", "Z_C2R"};
     const int d = direction == DFFT_FORWARD ? 0 : 1;
     for (int k = 0; k < lp.nreal; k++) {
         const LinePass& ps = lp.rpass[d][k];
@@ -2837,20 +2618,12 @@ extern "C" long long dfft_debug_real_lines_ops(int n, int ny, long long batch, i
         real_line_args<double>(ps, line_buf(ps.src, fake_addr(0, 5), fake_addr(0, 2), lp.temp), line_buf(ps.dst, fake_addr(0, 5), fake_addr(0, 2), lp.temp),
                                direction, r);
         const bool realk = ps.kind == PK_Z_R2C || ps.kind == PK_Z_C2R;
-        record_op<double>(&rec, names[ps.kind], k, ps.e->N, realk ? ps.e->z_C : ps.e->s_C, false, false, false, r.t);
-        if (realk) {
-            char b[128];
-            snprintf(b, sizeof(b), ", \"nzh\": %d, \"pair\": [%lld, %lld]}", ps.e->N / 2 + 1, ps.ld_in, ps.ld_out);
-            rec.ops.back().pop_back();
-            rec.ops.back() += b;
-        }
+        char extra[128] = "";
+        if (realk) snprintf(extra, sizeof(extra), ", \"nzh\": %d, \"pair\": [%lld, %lld]", ps.e->N / 2 + 1, ps.ld_in, ps.ld_out);
+        record_op<double>(ops, kPassNames[ps.kind], k, ps.e->N, realk ? ps.e->z_C : ps.e->s_C, false, false, false, r.t, extra);
     }
     lp.temp = nullptr;
-    std::string o = "[";
-    for (size_t i = 0; i < rec.ops.size(); i++) { if (i) o += ", "; o += rec.ops[i]; }
-    o += "]";
-    if (buf && cap > (long long)o.size()) memcpy(buf, o.c_str(), o.size() + 1);
-    return (long long)o.size() + 1;
+    return ops_json(ops, buf, cap);
 }
 
 extern "C" int dfft_fft_lines(void* data, int n, long long stride, long long nlines, long long inner, long long inner_dist,
