@@ -38,7 +38,7 @@ __all__ = [
     "BootstrapComm", "fft_mpi_init", "fft_mpi_plan_dft_c2c_3d", "fft_mpi_execute_dft_3d_c2c", "fft_mpi_destroy_plan",
     "fft_mpi_alloc_local_memory", "fft_mpi_local_size_3d", "fft_mpi_cleanup", "getMaxDataCount", "supported_lengths",
     "fft_mpi_plan_dft_r2c_3d", "local_size_r2c_3d", "fft_mpi_plan_dft_convolve_3d",
-    "fft_lines", "lines_ops", "LinesPlan", "RealLinesPlan", "real_lines_ops", "length_kind", "length_schedule", "memcpy_htod", "memcpy_dtoh", "exchange_table", "comm_allgather",
+    "fft_lines", "lines_ops", "LinesPlan", "RealLinesPlan", "real_lines_ops", "lines_3d_ops", "length_kind", "length_schedule", "memcpy_htod", "memcpy_dtoh", "exchange_table", "comm_allgather",
 ]
 
 
@@ -105,6 +105,10 @@ def lib():
     L.dfft_lines_plan_create_r2c.argtypes = [i, ll, i, P(vp)]
     L.dfft_lines_plan_create_r2c_2d.argtypes = [i, i, ll, i, P(vp)]
     L.dfft_lines_execute_real.argtypes = [vp, vp, vp, i]
+    L.dfft_lines_plan_create_3d.argtypes = [i, i, i, ll, i, P(vp)]
+    L.dfft_lines_plan_create_r2c_3d.argtypes = [i, i, i, ll, i, P(vp)]
+    L.dfft_debug_lines_3d_ops.argtypes = [i, i, i, ll, i, i, i, ctypes.c_char_p, ll]
+    L.dfft_debug_lines_3d_ops.restype = ll
     L.dfft_debug_real_lines_ops.argtypes = [i, i, ll, i, i, i, ctypes.c_char_p, ll]
     L.dfft_debug_real_lines_ops.restype = ll
     L.dfft_length_kind.argtypes = [i, i]
@@ -397,11 +401,14 @@ def memcpy_dtoh(host_ptr, dev_ptr, nbytes):
 
 class LinesPlan:
     """templateFFT engine surface (templateFFT.h:361-365): initializeFFT -> LinesPlan(...), launchFFTKernel -> execute,
-    deleteFFT -> destroy.  Batched 1-D lines (contiguous or strided) or, with `two_d=(nx, ny, batch)`, batched 2-D."""
+    deleteFFT -> destroy.  Batched 1-D lines (contiguous or strided), with `two_d=(nx, ny, batch)` batched 2-D, or with
+    `three_d=(nx, ny, nz, batch)` batched 3-D (numpy.fft.fftn over the last three axes of a[batch][nz][ny][nx])."""
 
-    def __init__(self, n=None, stride=1, nlines=0, inner=0, inner_dist=0, outer_dist=0, precision=DOUBLE, two_d=None):
+    def __init__(self, n=None, stride=1, nlines=0, inner=0, inner_dist=0, outer_dist=0, precision=DOUBLE, two_d=None, three_d=None):
         h = ctypes.c_void_p()
-        if two_d is not None:
+        if three_d is not None:
+            _check(lib().dfft_lines_plan_create_3d(*three_d, precision, ctypes.byref(h)), "dfft_lines_plan_create_3d")
+        elif two_d is not None:
             _check(lib().dfft_lines_plan_create_2d(two_d[0], two_d[1], two_d[2], precision, ctypes.byref(h)), "dfft_lines_plan_create_2d")
         else:
             _check(lib().dfft_lines_plan_create(n, stride, nlines, inner, inner_dist, outer_dist, precision, ctypes.byref(h)), "dfft_lines_plan_create")
@@ -426,11 +433,14 @@ class LinesPlan:
 class RealLinesPlan:
     """Real-data lines: R2C (FORWARD) / C2R (BACKWARD, unnormalised), out of place.  `nlines` densely packed real lines of `n`
     points <-> as many half spectra of n//2+1 complex points, or, with `two_d=(nx, ny, batch)`, `batch` row-major ny x nx real
-    matrices <-> ny x (nx//2+1) complex matrices (numpy.fft.rfft2 layout)."""
+    matrices <-> ny x (nx//2+1) complex matrices (numpy.fft.rfft2 layout), or, with `three_d=(nx, ny, nz, batch)`, nz x ny x nx
+    real arrays <-> nz x ny x (nx//2+1) complex arrays (numpy.fft.rfftn layout)."""
 
-    def __init__(self, n=None, nlines=0, precision=DOUBLE, two_d=None):
+    def __init__(self, n=None, nlines=0, precision=DOUBLE, two_d=None, three_d=None):
         h = ctypes.c_void_p()
-        if two_d is not None:
+        if three_d is not None:
+            _check(lib().dfft_lines_plan_create_r2c_3d(*three_d, precision, ctypes.byref(h)), "dfft_lines_plan_create_r2c_3d")
+        elif two_d is not None:
             _check(lib().dfft_lines_plan_create_r2c_2d(two_d[0], two_d[1], two_d[2], precision, ctypes.byref(h)), "dfft_lines_plan_create_r2c_2d")
         else:
             _check(lib().dfft_lines_plan_create_r2c(n, nlines, precision, ctypes.byref(h)), "dfft_lines_plan_create_r2c")
@@ -462,6 +472,19 @@ def real_lines_ops(n, nlines, direction, precision=DOUBLE, two_d=None):
         raise DfftError(f"dfft_debug_real_lines_ops failed ({need}): " + lib().dfft_last_error().decode())
     buf = ctypes.create_string_buffer(int(need))
     lib().dfft_debug_real_lines_ops(*args, buf, need)
+    return json.loads(buf.value.decode())
+
+
+def lines_3d_ops(nx, ny, nz, batch, direction, precision=DOUBLE, real=False):
+    """passes LinesPlan(three_d=...) / RealLinesPlan(three_d=...) would launch for `direction` (host-only test hook, see
+    dfft_debug_lines_3d_ops); read DFFT_NO_PLANE / DFFT_FORCE_PLANE / DFFT_GENERIC at the call, as plan creation does"""
+    import json
+    args = (nx, ny, nz, batch, precision, direction, int(bool(real)))
+    need = lib().dfft_debug_lines_3d_ops(*args, None, 0)
+    if need < 0:
+        raise DfftError(f"dfft_debug_lines_3d_ops failed ({need}): " + lib().dfft_last_error().decode())
+    buf = ctypes.create_string_buffer(int(need))
+    lib().dfft_debug_lines_3d_ops(*args, buf, need)
     return json.loads(buf.value.decode())
 
 

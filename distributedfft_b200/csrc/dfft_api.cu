@@ -2226,18 +2226,19 @@ struct LinePass {
     long long tw_n = 0;          // four-step twiddle modulus (PK_XF_TW)
     int src = 0, dst = 0;        // LB_IN (the caller's data / a real plan's `in`), LB_TEMP (the plan's temporary), LB_OUT
     long long ld_in = 0, ld_out = 0;   // PK_Z_R2C / PK_Z_C2R: distance between the two lines of a pair (RealZArgs), each side's elements
+    bool plane = false;          // X + Y of ntiles whole e->N x e->N planes in one launch of e->plane (PlaneArgs); `kind` unused
 };
 enum { LB_IN = 0, LB_TEMP = 1, LB_OUT = 2 };
 struct dfft_lines_plan_s {
     int prec = 0, device = 0, sms = 132, npass = 0;
     bool ordered = false;        // passes run in the same order for both directions (four-step)
     void* temp = nullptr;
-    LinePass pass[2];
-    // real plans (dfft_lines_plan_create_r2c[_2d]): the passes of each direction in execution order, [0] forward, [1] backward;
+    LinePass pass[3];
+    // real plans (dfft_lines_plan_create_r2c[_2d|_3d]): the passes of each direction in execution order, [0] forward, [1] backward;
     // `pass` stays empty.  Read by dfft_lines_execute_real and dfft_debug_real_lines_ops alike
     bool real = false;
     int nreal = 0;
-    LinePass rpass[2][2];
+    LinePass rpass[2][3];
     long long rcount = 0, ccount = 0;   // reals and complex elements of the caller's real / complex buffer
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[2] = {nullptr, nullptr};
@@ -2248,6 +2249,13 @@ template <typename T> static void upload_lut_e(void** dst, const SizeEntry* e, b
 {
     if (contiguous) upload_lut<T>(dst, e->z_nstages, e->z_rad);
     else upload_lut<T>(dst, e->s_nstages, e->s_rad);
+}
+
+// a * b * c < 2^31 (the kernels' 32-bit row counts TileArgs::W / G), without overflow for any non-negative arguments.  Column
+// counts need no check: a strided pass's columns (nx*ny, ny*(nx/2+1)) are below 2^25 for every supported length
+static bool fits_int(long long a, long long b, long long c = 1)
+{
+    return (__int128)a * b * c <= 0x7fffffff;
 }
 
 static int make_line_pass(LinePass& lp, int n, long long stride, long long nlines, long long inner, long long inner_dist, long long outer_dist,
@@ -2293,7 +2301,7 @@ extern "C" int dfft_lines_destroy(dfft_lines_plan p)
     if (!p) return 0;
     cudaSetDevice(p->device);
     if (p->stream) cudaStreamSynchronize(p->stream);
-    for (int i = 0; i < 2; i++) if (p->pass[i].lut) cudaFree(p->pass[i].lut);
+    for (auto& lp : p->pass) if (lp.lut) cudaFree(lp.lut);
     for (auto& dir : p->rpass)
         for (auto& lp : dir) if (lp.lut) cudaFree(lp.lut);
     if (p->temp) cudaFree(p->temp);
@@ -2396,17 +2404,73 @@ extern "C" int dfft_lines_plan_create_2d(int nx, int ny, long long batch, int pr
     return 0;
 }
 
+static bool env_on(const char* name)
+{
+    const char* v = getenv(name);
+    return v && atoi(v) != 0;
+}
+
+// batch nz x ny x nx volumes (nx fastest), in place: X along the batch*nz*ny rows, Y over the nx columns of every plane (stride
+// nx), Z over the nx*ny columns of every volume (stride nx*ny); backward in reverse.  Where nx == ny and the entry has a plane
+// kernel that is the default for its shape (plane_default; DFFT_FORCE_PLANE=1: wherever instantiated), X and Y are one launch
+// of it over the batch*nz planes.  DFFT_NO_PLANE=1 keeps the separate passes.  Read at plan creation
+static int make_lines_3d(dfft_lines_plan p, int nx, int ny, int nz, long long batch, int precision, bool dry)
+{
+    if (nx < 1 || ny < 1 || nz < 1 || batch < 0 || (precision != DFFT_DOUBLE && precision != DFFT_FLOAT)) return fail(DFFT_EINVAL, "bad arguments");
+    if (!fits_int(ny, nz, batch)) return fail(DFFT_EUNSUPPORTED, "%d x %d x %lld rows: at most 2^31 - 1 per plan", ny, nz, batch);
+    const long long planes = (long long)nz * batch, rows = planes * ny, plane = (long long)nx * ny;
+    const SizeEntry* ex = find_size_entry(nx, precision);
+    const bool use_plane = ex && nx == ny && ex->plane && !env_on("DFFT_NO_PLANE") && (plane_default(nx, precision) || env_on("DFFT_FORCE_PLANE"));
+    int rc = 0, k = 0;
+    if (use_plane) {
+        LinePass& lp = p->pass[k++];
+        lp.e = ex; lp.plane = true; lp.ntiles = planes;
+        lp.ia = lp.oa = Affine{plane, 0, nx, 1};   // for the records: plane, row and point strides
+        if (!dry) {
+            if (precision == DFFT_DOUBLE) upload_lut_e<double>(&lp.lut, ex, true);
+            else upload_lut_e<float>(&lp.lut, ex, true);
+            if (cudaGetLastError() != cudaSuccess || !lp.lut) return fail(DFFT_ECUDA, "twiddle table upload failed");
+        }
+    } else {
+        rc = make_line_pass(p->pass[k++], nx, 1, rows, rows, nx, 0, precision, dry);
+        if (!rc) rc = make_line_pass(p->pass[k++], ny, nx, nx * planes, nx, 1, plane, precision, dry);
+    }
+    if (!rc) rc = make_line_pass(p->pass[k++], nz, plane, plane * batch, plane, 1, plane * nz, precision, dry);
+    if (rc) return rc;
+    p->npass = k;
+    return 0;
+}
+
+extern "C" int dfft_lines_plan_create_3d(int nx, int ny, int nz, long long batch, int precision, dfft_lines_plan* out)
+{
+    if (!out) return fail(DFFT_EINVAL, "null plan pointer");
+    *out = nullptr;
+    if (precision != DFFT_DOUBLE && precision != DFFT_FLOAT) return fail(DFFT_EINVAL, "bad arguments");
+    dfft_lines_plan p = new dfft_lines_plan_s;
+    int rc = lines_plan_common(p, precision);
+    if (!rc) rc = make_lines_3d(p, nx, ny, nz, batch, precision, false);
+    if (rc) { dfft_lines_destroy(p); return rc; }
+    *out = p;
+    return 0;
+}
+
 template <typename T> static int lines_execute_impl(dfft_lines_plan p, void* data, int direction)
 {
     CU(cudaEventRecord(p->ev[0], p->stream));
     for (int k = 0; k < p->npass; k++) {
         const LinePass& lp = p->pass[(direction == DFFT_BACKWARD && !p->ordered) ? p->npass - 1 - k : k];
         if (lp.ntiles <= 0) continue;
-        TileArgs<T> a{};
-        a.in = (const cx<T>*)(lp.src ? p->temp : data); a.out = (cx<T>*)(lp.dst ? p->temp : data); a.lut = (const cx<T>*)lp.lut;
-        a.ia = lp.ia; a.oa = lp.oa; a.G = lp.G; a.W = lp.W; a.ntiles = lp.ntiles;
-        a.inv = direction == DFFT_BACKWARD; a.gen = lp.e->gen; a.tw_n = lp.tw_n;
-        cudaError_t err = lp.e->launch[lp.kind](&a, p->sms, p->stream);
+        cudaError_t err;
+        if (lp.plane) {
+            const PlaneArgs<T> pa{(const cx<T>*)data, (cx<T>*)data, (const cx<T>*)lp.lut, lp.ntiles, direction == DFFT_BACKWARD ? 1 : 0};
+            err = lp.e->plane(&pa, p->sms, p->stream);
+        } else {
+            TileArgs<T> a{};
+            a.in = (const cx<T>*)(lp.src ? p->temp : data); a.out = (cx<T>*)(lp.dst ? p->temp : data); a.lut = (const cx<T>*)lp.lut;
+            a.ia = lp.ia; a.oa = lp.oa; a.G = lp.G; a.W = lp.W; a.ntiles = lp.ntiles;
+            a.inv = direction == DFFT_BACKWARD; a.gen = lp.e->gen; a.tw_n = lp.tw_n;
+            err = lp.e->launch[lp.kind](&a, p->sms, p->stream);
+        }
         if (err != cudaSuccess) return fail(DFFT_ECUDA, "line pass launch failed: %s", cudaGetErrorString(err));
     }
     CU(cudaEventRecord(p->ev[1], p->stream));
@@ -2484,15 +2548,18 @@ static void make_real_pass(LinePass& lp, const SizeEntry* e, long long nlines, b
     lp.src = src; lp.dst = dst;
 }
 
-// 1-D: `batch` lines of n points (ny unused).  2-D: `batch` ny x n matrices, rows real <-> rows of n/2+1 complex points
-static int make_real_lines(dfft_lines_plan p, int n, int ny, long long batch, int precision, bool two_d, bool dry)
+// 1-D: `batch` lines of n points (ny, nz unused).  2-D: `batch` ny x n matrices, rows real <-> rows of n/2+1 complex points.
+// 3-D: `batch` nz x ny x n volumes, likewise
+static int make_real_lines(dfft_lines_plan p, int n, int ny, int nz, long long batch, int precision, int dims, bool dry)
 {
-    if (batch < 0 || (two_d && ny < 1) || (precision != DFFT_DOUBLE && precision != DFFT_FLOAT)) return fail(DFFT_EINVAL, "bad arguments");
+    if (batch < 0 || (dims >= 2 && ny < 1) || (dims == 3 && nz < 1) || (precision != DFFT_DOUBLE && precision != DFFT_FLOAT))
+        return fail(DFFT_EINVAL, "bad arguments");
     const SizeEntry* e = n < 2 ? nullptr : find_size_entry(n, precision);
     if (!e) return fail(DFFT_EUNSUPPORTED, "real lines of %d points: the length must be 2..13-smooth and fit one shared-memory line", n);
     if (!e->launch[PK_Z_R2C] || !e->launch[PK_Z_C2R]) return fail(DFFT_EUNSUPPORTED, "the kernel entry of length %d has no real-data kernels", n);
-    const long long rows = two_d ? (long long)ny * batch : batch;
-    if (rows > 0x7fffffffLL) return fail(DFFT_EUNSUPPORTED, "%lld real lines: at most 2^31 - 1 per plan", rows);
+    const long long my = dims >= 2 ? ny : 1, mz = dims == 3 ? nz : 1;
+    if (!fits_int(my, mz, batch)) return fail(DFFT_EUNSUPPORTED, "%lld x %lld x %lld real lines: at most 2^31 - 1 per plan", my, mz, batch);
+    const long long rows = my * mz * batch;
     const long long H = n / 2 + 1;
     p->real = true;
     p->prec = precision;
@@ -2501,19 +2568,25 @@ static int make_real_lines(dfft_lines_plan p, int n, int ny, long long batch, in
     LinePass* f = p->rpass[0];
     LinePass* b = p->rpass[1];
     make_real_pass(f[0], e, rows, true, LB_IN, LB_OUT);
-    if (!two_d) {
+    if (dims == 1) {
         make_real_pass(b[0], e, rows, false, LB_IN, LB_OUT);
         p->nreal = 1;
     } else {
-        // along ny: the H columns of every half-spectrum matrix, matrices ny*H apart.  Forward in place in `out`; backward from
-        // `in` into the temporary, so that `in` is never written
-        int rc = make_line_pass(f[1], ny, H, H * batch, H, 1, H * ny, precision, dry);
-        if (!rc) rc = make_line_pass(b[0], ny, H, H * batch, H, 1, H * ny, precision, dry);
+        // along ny: the H columns of every half-spectrum matrix, matrices ny*H apart; along nz (3-D): the ny*H columns of every
+        // volume, volumes nz*ny*H apart.  Forward in place in `out` after the real pass; backward the strided passes in reverse,
+        // the first from `in` into the temporary, so that `in` is never written, the rest in place there
+        const int ns = dims - 1;   // strided passes: f[1..ns] forward, b[0..ns-1] backward (the same passes in reverse)
+        auto along_y = [&](LinePass& lp) { return make_line_pass(lp, ny, H, H * mz * batch, H, 1, H * ny, precision, dry); };
+        auto along_z = [&](LinePass& lp) { return make_line_pass(lp, nz, H * ny, H * ny * batch, H * ny, 1, H * ny * nz, precision, dry); };
+        int rc = along_y(f[1]);
+        if (!rc) rc = along_y(b[ns - 1]);
+        if (!rc && dims == 3) rc = along_z(f[2]);
+        if (!rc && dims == 3) rc = along_z(b[0]);
         if (rc) return rc;
-        f[1].src = f[1].dst = LB_OUT;
-        b[0].src = LB_IN; b[0].dst = LB_TEMP;
-        make_real_pass(b[1], e, rows, false, LB_TEMP, LB_OUT);
-        p->nreal = 2;
+        for (int k = 0; k < ns; k++) { b[k].src = k == 0 ? LB_IN : LB_TEMP; b[k].dst = LB_TEMP; }
+        for (int k = 1; k <= ns; k++) f[k].src = f[k].dst = LB_OUT;
+        make_real_pass(b[ns], e, rows, false, LB_TEMP, LB_OUT);
+        p->nreal = dims;
         const size_t esz = precision == DFFT_FLOAT ? 8 : 16;
         if (dry) p->temp = fake_addr(0, 4);
         else if (p->ccount > 0) CU(cudaMalloc(&p->temp, (size_t)p->ccount * esz));
@@ -2547,13 +2620,13 @@ template <typename T> static void real_line_args(const LinePass& lp, const void*
     r.ld_in = lp.ld_in; r.ld_out = lp.ld_out;
 }
 
-static int real_plan_create(int n, int ny, long long batch, int precision, bool two_d, dfft_lines_plan* out)
+static int real_plan_create(int n, int ny, int nz, long long batch, int precision, int dims, dfft_lines_plan* out)
 {
     if (!out) return fail(DFFT_EINVAL, "null plan pointer");
     *out = nullptr;
     dfft_lines_plan p = new dfft_lines_plan_s;
     int rc = lines_plan_common(p, precision);
-    if (!rc) rc = make_real_lines(p, n, ny, batch, precision, two_d, false);
+    if (!rc) rc = make_real_lines(p, n, ny, nz, batch, precision, dims, false);
     if (rc) { dfft_lines_destroy(p); return rc; }
     *out = p;
     return 0;
@@ -2561,12 +2634,17 @@ static int real_plan_create(int n, int ny, long long batch, int precision, bool 
 
 extern "C" int dfft_lines_plan_create_r2c(int n, long long nlines, int precision, dfft_lines_plan* plan)
 {
-    return real_plan_create(n, 1, nlines, precision, false, plan);
+    return real_plan_create(n, 1, 1, nlines, precision, 1, plan);
 }
 
 extern "C" int dfft_lines_plan_create_r2c_2d(int nx, int ny, long long batch, int precision, dfft_lines_plan* plan)
 {
-    return real_plan_create(nx, ny, batch, precision, true, plan);
+    return real_plan_create(nx, ny, 1, batch, precision, 2, plan);
+}
+
+extern "C" int dfft_lines_plan_create_r2c_3d(int nx, int ny, int nz, long long batch, int precision, dfft_lines_plan* plan)
+{
+    return real_plan_create(nx, ny, nz, batch, precision, 3, plan);
 }
 
 template <typename T> static int lines_execute_real_impl(dfft_lines_plan p, const void* in, void* out, int direction)
@@ -2609,7 +2687,7 @@ extern "C" long long dfft_debug_real_lines_ops(int n, int ny, long long batch, i
     if (direction != DFFT_FORWARD && direction != DFFT_BACKWARD) return fail(DFFT_EINVAL, "bad direction");
     dfft_lines_plan_s lp;
     std::vector<std::string> ops;
-    const int rc = make_real_lines(&lp, n, ny, batch, precision, two_d != 0, true);
+    const int rc = make_real_lines(&lp, n, ny, 1, batch, precision, two_d ? 2 : 1, true);
     if (rc) return rc;
     const int d = direction == DFFT_FORWARD ? 0 : 1;
     for (int k = 0; k < lp.nreal; k++) {
@@ -2621,6 +2699,46 @@ extern "C" long long dfft_debug_real_lines_ops(int n, int ny, long long batch, i
         char extra[128] = "";
         if (realk) snprintf(extra, sizeof(extra), ", \"nzh\": %d, \"pair\": [%lld, %lld]", ps.e->N / 2 + 1, ps.ld_in, ps.ld_out);
         record_op<double>(ops, kPassNames[ps.kind], k, ps.e->N, realk ? ps.e->z_C : ps.e->s_C, false, false, false, r.t, extra);
+    }
+    lp.temp = nullptr;
+    return ops_json(ops, buf, cap);
+}
+
+/* test hook (host only): the passes of a 3-D lines plan for `direction`, JSON as dfft_debug_lines_ops (complex: the caller's data
+ * is buffer 1) or dfft_debug_real_lines_ops (real != 0: in = buffer 5, out = 2, temporary = 4).  The plane kernel's record is
+ * "XY_PLANE" with ntiles = planes and ia = oa = [plane, 0, row, point] strides */
+extern "C" long long dfft_debug_lines_3d_ops(int nx, int ny, int nz, long long batch, int precision, int direction, int real, char* buf, long long cap)
+{
+    if (direction != DFFT_FORWARD && direction != DFFT_BACKWARD) return fail(DFFT_EINVAL, "bad direction");
+    dfft_lines_plan_s lp;
+    std::vector<std::string> ops;
+    if (real) {
+        const int rc = make_real_lines(&lp, nx, ny, nz, batch, precision, 3, true);
+        if (rc) return rc;
+        const int d = direction == DFFT_FORWARD ? 0 : 1;
+        for (int k = 0; k < lp.nreal; k++) {
+            const LinePass& ps = lp.rpass[d][k];
+            RealZArgs<double> r{};
+            real_line_args<double>(ps, line_buf(ps.src, fake_addr(0, 5), fake_addr(0, 2), lp.temp), line_buf(ps.dst, fake_addr(0, 5), fake_addr(0, 2), lp.temp),
+                                   direction, r);
+            const bool realk = ps.kind == PK_Z_R2C || ps.kind == PK_Z_C2R;
+            char extra[128] = "";
+            if (realk) snprintf(extra, sizeof(extra), ", \"nzh\": %d, \"pair\": [%lld, %lld]", ps.e->N / 2 + 1, ps.ld_in, ps.ld_out);
+            record_op<double>(ops, kPassNames[ps.kind], k, ps.e->N, realk ? ps.e->z_C : ps.e->s_C, false, false, false, r.t, extra);
+        }
+    } else {
+        lp.prec = precision;
+        const int rc = make_lines_3d(&lp, nx, ny, nz, batch, precision, true);
+        if (rc) return rc;
+        for (int k = 0; k < lp.npass; k++) {
+            const LinePass& ps = lp.pass[direction == DFFT_BACKWARD ? lp.npass - 1 - k : k];
+            TileArgs<double> a{};
+            a.in = (const double2*)fake_addr(0, 1); a.out = (double2*)fake_addr(0, 1);
+            a.ia = ps.ia; a.oa = ps.oa; a.G = ps.G; a.W = ps.W; a.ntiles = ps.ntiles;
+            a.inv = direction == DFFT_BACKWARD;
+            const int C = ps.plane ? ps.e->N : (ps.kind == PK_Z ? ps.e->z_C : ps.e->s_C);
+            record_op<double>(ops, ps.plane ? "XY_PLANE" : kPassNames[ps.kind], k, ps.e->N, C, false, false, false, a);
+        }
     }
     lp.temp = nullptr;
     return ops_json(ops, buf, cap);

@@ -7,6 +7,7 @@
 #include <vector>
 #include "fft_passes.cuh"
 #include "fft_real.cuh"
+#include "fft_plane.cuh"
 
 namespace dfft {
 
@@ -42,6 +43,8 @@ typedef cudaError_t (*FusedLaunchFn)(const void* args_a, const void* args_b, con
 // send side (Y pass of part k, peer stores) and receive side (X pass of part k-1) of the exchange in one kernel (fft_fused_yx_kernel)
 typedef cudaError_t (*FusedYxLaunchFn)(const void* args_y, const void* args_x, const YxCtl* ctl, int sm_count, cudaStream_t stream);
 typedef cudaError_t (*Fused3LaunchFn)(const void* args_z, const void* args_y, const void* args_x, const Fused3Ctl* ctl, int sm_count, cudaStream_t stream);
+// X and Y passes of square planes in one sweep (fft_plane_kernel): args = PlaneArgs<T>
+typedef cudaError_t (*PlaneLaunchFn)(const void* plane_args, int sm_count, cudaStream_t stream);
 
 struct SizeEntry {
     int N;
@@ -57,7 +60,12 @@ struct SizeEntry {
     FusedYxLaunchFn fused_yx;        // Y (peer-store configuration) + X roles of this entry in one kernel; nullptr unless both fill the same CTA
     Fused3LaunchFn fused3;           // same restriction, and the X configuration must fill the same CTA as the peer-store Y role (else nullptr)
     const void* gen;      // run-time schedule (GenSched) of a generic-length entry, nullptr for tuned lengths
+    PlaneLaunchFn plane;  // valid for square planes: the contiguous (X) and strided (Y) passes of whole N x N planes in one kernel;
+                          // default entries of N = 16, 32, 64 only (both roles share one schedule there), else nullptr
 };
+
+// whether fft_plane_kernel is the default for (N, prec) (measured against the two separate passes, dfft_kernels_common.cu)
+bool plane_default(int N, int prec);
 
 // TMA-pipelined pass kernels (fft_tma.cuh), instantiated for the lengths whose C-line tile fills a 64 KB ring slot
 typedef cudaError_t (*TmaLaunchFn)(int mode, const void* tma_args, const void* map_in, const void* map_out, int sm_count, cudaStream_t stream);

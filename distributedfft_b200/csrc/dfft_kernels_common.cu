@@ -33,6 +33,19 @@ const SizeEntry* find_size_entry(int N, int prec)
     return def;
 }
 
+// fft_plane_kernel against the separate X and Y passes, per (N, precision), from csrc/tools/lines3d_bench.py on H100
+// (DESIGN.md section 7): true = the plane kernel is the default of the 3-D lines plans for that shape
+static const struct { int N, prec; bool use; } kPlaneUse[] = {
+    {16, 0, true}, {32, 0, true}, {64, 0, true}, {16, 1, true}, {32, 1, true}, {64, 1, true},
+};
+
+bool plane_default(int N, int prec)
+{
+    for (const auto& u : kPlaneUse)
+        if (u.N == N && u.prec == prec) return u.use;
+    return false;
+}
+
 void list_sizes(int prec, std::vector<int>& out)
 {
     out.clear();

@@ -91,6 +91,34 @@ cudaError_t launch_conv(const void* vargs, int sm_count, cudaStream_t st)
     return cudaGetLastError();
 }
 
+// X + Y passes of square planes (fft_plane_kernel): vargs is a PlaneArgs<T>; P planes per CTA
+template <class S, typename T, int P, int MINB>
+cudaError_t launch_plane(const void* vargs, int sm_count, cudaStream_t st)
+{
+    const PlaneArgs<T>& a = *reinterpret_cast<const PlaneArgs<T>*>(vargs);
+    auto kern = fft_plane_kernel<S, T, P, MINB>;
+    constexpr size_t smem = PlaneSmem<S, T, P>::bytes;
+    static std::atomic<int> occ_cache[64];
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    int occ = occ_cache[dev & 63].load();
+    if (occ == 0) {
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, S::T * S::N * P, smem);
+        if (e != cudaSuccess) return e;
+        if (occ < 1) return cudaErrorLaunchOutOfResources;
+        occ_cache[dev & 63].store(occ);
+    }
+    const long long groups = (a.planes + P - 1) / P;
+    if (groups <= 0) return cudaSuccess;
+    long long grid = (long long)sm_count * occ;
+    if (grid > groups) grid = groups;
+    kern<<<(unsigned)grid, S::T * S::N * P, smem, st>>>(a);
+    return cudaGetLastError();
+}
+
 template <class OpA, class OpB, typename T, int MINB>
 cudaError_t launch_fused(const void* va, const void* vb, const FusedCtl* ctl, int sm_count, cudaStream_t st)
 {
@@ -259,6 +287,14 @@ SizeEntry make_entry(int variant = 0)
         // spectral convolution along x (the X axis of a convolve plan uses this entry's strided schedule and twiddle table)
         e.launch[PK_XCONV] = launch_conv<SS, T, Y::C, Y::TW, false, Y::MB, Y::PP>;
         e.launch[PK_XCONV_CO] = launch_conv<SS, T, PEER::C, PEER::TW, true, PEER::MB, PEER::PP>;
+        // X and Y passes of whole square planes in one kernel, where both roles share one schedule (and so one twiddle table).
+        // Register budget: 64 per thread (2 CTAs of 512 / 4 of 256 threads), except 32-point fp64, which spills at 64 and is
+        // given 85 (3 CTAs of 256); 64-point fp64 keeps 2 CTAs of 512 with a small spill (DESIGN.md section 3.8)
+        if constexpr (std::is_same<ZS, SS>::value && (ZS::N == 16 || ZS::N == 32 || ZS::N == 64)) {
+            constexpr int P = plane_group<ZS>();
+            constexpr int MBP = (sizeof(T) == 8 && ZS::N == 32) ? 3 : 1024 / (ZS::T * ZS::N * P);
+            e.plane = launch_plane<ZS, T, P, MBP>;
+        }
     }
     // fused two-pass kernels: the contiguous role is re-tiled so that both roles fill the same CTA
     constexpr int NT = SS::T * Y::C, NTP = SS::T * PEER::C;

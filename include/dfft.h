@@ -269,6 +269,12 @@ typedef struct dfft_lines_plan_s* dfft_lines_plan;
 int dfft_lines_plan_create(int n, long long stride, long long nlines, long long inner, long long inner_dist,
                            long long outer_dist, int precision, dfft_lines_plan* plan);
 int dfft_lines_plan_create_2d(int nx, int ny, long long batch, int precision, dfft_lines_plan* plan);
+/* batch row-major nz x ny x nx complex arrays (nx fastest), in place through dfft_lines_execute:
+ * numpy.fft.fftn(a, axes=(1, 2, 3)) on a[batch][nz][ny][nx]; backward unnormalised (ifftn * nx*ny*nz).
+ * nx takes any length a contiguous lines pass takes, ny and nz any length a strided one takes.  Where nx == ny is 16, 32 or 64
+ * the X and Y passes run as one kernel over whole planes held in shared memory (DFFT_NO_PLANE=1 at plan creation: separate
+ * passes; the results are bitwise the same).  2^31 or more rows (ny*nz*batch) are DFFT_EUNSUPPORTED. */
+int dfft_lines_plan_create_3d(int nx, int ny, int nz, long long batch, int precision, dfft_lines_plan* plan);
 int dfft_lines_execute(dfft_lines_plan plan, void* data, int direction);
 int dfft_lines_synchronize(dfft_lines_plan plan);
 void* dfft_lines_stream(dfft_lines_plan plan);
@@ -283,6 +289,11 @@ int dfft_lines_destroy(dfft_lines_plan plan);
  * plan-owned temporary of batch*ny*(nx/2+1) complex elements. */
 int dfft_lines_plan_create_r2c(int n, long long nlines, int precision, dfft_lines_plan* plan);
 int dfft_lines_plan_create_r2c_2d(int nx, int ny, long long batch, int precision, dfft_lines_plan* plan);
+/* batch real nz x ny x nx arrays <-> batch nz x ny x (nx/2+1) complex arrays (numpy.fft.rfftn layout), out of place through
+ * dfft_lines_execute_real; C2R = irfftn(., s=(nz, ny, nx)) * nx*ny*nz, with the same ignored imaginary parts as the 2-D C2R.
+ * nx as the 1-D real plan, ny and nz as a strided C2C lines pass; the backward transform uses a plan-owned temporary of
+ * batch*nz*ny*(nx/2+1) complex elements and never writes `in`.  2^31 or more real rows are DFFT_EUNSUPPORTED. */
+int dfft_lines_plan_create_r2c_3d(int nx, int ny, int nz, long long batch, int precision, dfft_lines_plan* plan);
 /* FORWARD: in = reals -> out = half spectra.  BACKWARD: in = half spectra -> out = reals, unnormalised (numpy.fft.irfft / irfft2
  * times n / nx*ny; the imaginary parts at bin 0 and, for even n, bin n/2 are ignored, as in the 3-D C2R).  `in` is never
  * written.  Null or overlapping buffers, a buffer not aligned to its element size, and a complex plan are DFFT_EINVAL (and a
@@ -291,6 +302,10 @@ int dfft_lines_execute_real(dfft_lines_plan plan, const void* in, void* out, int
 /* test hook (host only): the passes of a real lines plan (1-D: n, nlines = batch, ny unused; 2-D when two_d != 0), same JSON
  * as dfft_debug_lines_ops, with "nzh" and "pair" on the real passes; in = buffer 5, out = buffer 2, temporary = buffer 4 */
 long long dfft_debug_real_lines_ops(int n, int ny, long long batch, int precision, int direction, int two_d, char* buf, long long cap);
+/* test hook (host only): the passes of either 3-D lines plan for `direction`, JSON like dfft_debug_lines_ops (complex, data =
+ * buffer 1) / dfft_debug_real_lines_ops (real != 0); the plane kernel is one "XY_PLANE" record over ntiles planes */
+long long dfft_debug_lines_3d_ops(int nx, int ny, int nz, long long batch, int precision, int direction, int real,
+                                  char* buf, long long cap);
 /* one-shot convenience (plan + execute + synchronize + destroy), used by the per-axis parity tests */
 int dfft_fft_lines(void* data, int n, long long stride, long long nlines, long long inner, long long inner_dist,
                    long long outer_dist, int direction, int precision);
