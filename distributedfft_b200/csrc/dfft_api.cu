@@ -2227,6 +2227,7 @@ struct LinePass {
     int src = 0, dst = 0;        // LB_IN (the caller's data / a real plan's `in`), LB_TEMP (the plan's temporary), LB_OUT
     long long ld_in = 0, ld_out = 0;   // PK_Z_R2C / PK_Z_C2R: distance between the two lines of a pair (RealZArgs), each side's elements
     bool plane = false;          // X + Y of ntiles whole e->N x e->N planes in one launch of e->plane (PlaneArgs); `kind` unused
+    bool inv = false;            // convolve plans: this pass runs the inverse transform
 };
 enum { LB_IN = 0, LB_TEMP = 1, LB_OUT = 2 };
 struct dfft_lines_plan_s {
@@ -2240,6 +2241,14 @@ struct dfft_lines_plan_s {
     int nreal = 0;
     LinePass rpass[2][3];
     long long rcount = 0, ccount = 0;   // reals and complex elements of the caller's real / complex buffer
+    // convolve plans (dfft_lines_plan_create_convolve_[r2c_]3d): the passes of one execute in order, the multiply folded into the
+    // PK_XCONV pass; `pass` and `rpass` stay empty.  Read by dfft_lines_execute_convolve and dfft_debug_lines_conv_3d_ops alike.
+    // Inverse passes share their forward pass's twiddle table
+    bool conv = false;
+    int nconv = 0;
+    LinePass cpass[5];
+    long long batch = 0, mvol = 0;   // volumes; complex elements of one volume's multiplier
+    double scale = 0;                // DFFT_SCALE_BACKWARD: 1 / (nx*ny*nz), folded into the multiply; 0 = unnormalised
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[2] = {nullptr, nullptr};
     bool timed = false;
@@ -2304,6 +2313,11 @@ extern "C" int dfft_lines_destroy(dfft_lines_plan p)
     for (auto& lp : p->pass) if (lp.lut) cudaFree(lp.lut);
     for (auto& dir : p->rpass)
         for (auto& lp : dir) if (lp.lut) cudaFree(lp.lut);
+    for (int k = 0; k < p->nconv; k++) {
+        bool shared = false;
+        for (int j = 0; j < k; j++) shared |= p->cpass[j].lut == p->cpass[k].lut;
+        if (p->cpass[k].lut && !shared) cudaFree(p->cpass[k].lut);
+    }
     if (p->temp) cudaFree(p->temp);
     for (auto& e : p->ev) if (e) cudaEventDestroy(e);
     if (p->stream) cudaStreamDestroy(p->stream);
@@ -2481,6 +2495,7 @@ template <typename T> static int lines_execute_impl(dfft_lines_plan p, void* dat
 extern "C" int dfft_lines_execute(dfft_lines_plan p, void* data, int direction)
 {
     if (!p || !data || (direction != DFFT_FORWARD && direction != DFFT_BACKWARD)) return fail(DFFT_EINVAL, "bad arguments");
+    if (p->conv) return fail(DFFT_EINVAL, "a convolve lines plan runs with dfft_lines_execute_convolve");
     if (p->real) return fail(DFFT_EINVAL, "a real lines plan runs with dfft_lines_execute_real");
     CU(cudaSetDevice(p->device));
     return p->prec == DFFT_DOUBLE ? lines_execute_impl<double>(p, data, direction) : lines_execute_impl<float>(p, data, direction);
@@ -2668,6 +2683,7 @@ template <typename T> static int lines_execute_real_impl(dfft_lines_plan p, cons
 extern "C" int dfft_lines_execute_real(dfft_lines_plan p, const void* in, void* out, int direction)
 {
     if (!p || !in || !out || (direction != DFFT_FORWARD && direction != DFFT_BACKWARD)) return fail(DFFT_EINVAL, "bad arguments");
+    if (p->conv) return fail(DFFT_EINVAL, "a convolve lines plan runs with dfft_lines_execute_convolve");
     if (!p->real) return fail(DFFT_EINVAL, "a complex lines plan runs with dfft_lines_execute");
     const size_t rsz = p->prec == DFFT_FLOAT ? 4 : 8, csz = 2 * rsz;
     const bool fwd = direction == DFFT_FORWARD;
@@ -2740,6 +2756,155 @@ extern "C" long long dfft_debug_lines_3d_ops(int nx, int ny, int nz, long long b
             record_op<double>(ops, ps.plane ? "XY_PLANE" : kPassNames[ps.kind], k, ps.e->N, C, false, false, false, a);
         }
     }
+    lp.temp = nullptr;
+    return ops_json(ops, buf, cap);
+}
+
+// ---- batched 3-D spectral convolution on the lines engine: out = ifftn(fftn(in) * m) per volume --------------------------------
+// The forward passes of the 3-D lines plan (make_lines_3d / make_real_lines), the Z pass replaced by PK_XCONV (forward Z, multiply,
+// inverse Z in one column pass, as the slab convolve plan's X pass; fft_conv_shared_kernel when one multiplier serves every
+// volume), then the forward passes before Z again, inverse and in reverse order:
+//   C2C, plane kernel: XY_PLANE in -> out, XCONV, inverse XY_PLANE (6 volume sweeps + the multiplier)
+//   C2C, other shapes: X in -> out, Y, XCONV, inverse Y, inverse X (10 sweeps)
+//   R2C:               Z_R2C in -> temp, Y, XCONV, inverse Y, Z_C2R temp -> out
+// Everything after the first pass is in place in `out` (C2C) or the plan's temporary (R2C), so `in` is only read and in == out
+// works.  The Z length needs the convolve kernel: a tuned default entry (launch[PK_XCONV], as dfft_plan_convolve_* asks of x)
+static int make_lines_conv_3d(dfft_lines_plan p, int nx, int ny, int nz, long long batch, int precision, bool real, unsigned flags, bool dry)
+{
+    if (flags & ~DFFT_SCALE_BACKWARD) return fail(DFFT_EINVAL, "convolve lines plans take no flag but DFFT_SCALE_BACKWARD");
+    int rc = real ? make_real_lines(p, nx, ny, nz, batch, precision, 3, dry) : make_lines_3d(p, nx, ny, nz, batch, precision, dry);
+    if (rc) return rc;
+    LinePass* f = real ? p->rpass[0] : p->pass;   // forward passes in execution order, Z last
+    const int nf = real ? p->nreal : p->npass;
+    const LinePass& z = f[nf - 1];
+    if (z.kind != PK_Y || z.e->gen || !z.e->launch[PK_XCONV])
+        return fail(DFFT_EUNSUPPORTED, "the z length %d has no convolution kernel (it needs a tuned length, dfft_length_kind == 2, of the default kernel table)", nz);
+    const int buf = real ? LB_TEMP : LB_OUT;
+    int k = 0;
+    for (int j = 0; j < nf; j++) {
+        LinePass& lp = p->cpass[k++] = f[j];
+        lp.src = j == 0 ? LB_IN : buf; lp.dst = buf;
+    }
+    p->cpass[nf - 1].kind = PK_XCONV;
+    for (int j = nf - 2; j >= (real ? 1 : 0); j--) {
+        LinePass& lp = p->cpass[k++] = f[j];
+        lp.src = lp.dst = buf; lp.inv = true;
+    }
+    if (real) p->cpass[k++] = p->rpass[1][nf - 1];   // Z_C2R temp -> out
+    p->nconv = k;
+    // the builders' passes the schedule does not use give back their twiddle tables
+    auto used = [&](void* t) { for (int j = 0; j < k; j++) if (p->cpass[j].lut == t) return true; return false; };
+    for (auto& lp : p->pass) { if (lp.lut && !used(lp.lut)) cudaFree(lp.lut); lp = LinePass{}; }
+    for (auto& dir : p->rpass)
+        for (auto& lp : dir) { if (lp.lut && !used(lp.lut)) cudaFree(lp.lut); lp = LinePass{}; }
+    p->npass = p->nreal = 0;
+    p->conv = true;
+    p->real = real;
+    p->batch = batch;
+    const long long vol = (long long)nx * ny * nz;
+    p->mvol = real ? (long long)nz * ny * (nx / 2 + 1) : vol;
+    if (real) p->rcount = vol * batch;
+    else p->ccount = vol * batch;
+    p->scale = (flags & DFFT_SCALE_BACKWARD) ? 1.0 / (double)vol : 0.0;
+    return 0;
+}
+
+static int conv_plan_create(int nx, int ny, int nz, long long batch, int precision, bool real, unsigned flags, dfft_lines_plan* out)
+{
+    if (!out) return fail(DFFT_EINVAL, "null plan pointer");
+    *out = nullptr;
+    if (precision != DFFT_DOUBLE && precision != DFFT_FLOAT) return fail(DFFT_EINVAL, "bad arguments");
+    dfft_lines_plan p = new dfft_lines_plan_s;
+    int rc = lines_plan_common(p, precision);
+    if (!rc) rc = make_lines_conv_3d(p, nx, ny, nz, batch, precision, real, flags, false);
+    if (rc) { dfft_lines_destroy(p); return rc; }
+    *out = p;
+    return 0;
+}
+
+extern "C" int dfft_lines_plan_create_convolve_3d(int nx, int ny, int nz, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
+{
+    return conv_plan_create(nx, ny, nz, batch, precision, false, flags, plan);
+}
+
+extern "C" int dfft_lines_plan_create_convolve_r2c_3d(int nx, int ny, int nz, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
+{
+    return conv_plan_create(nx, ny, nz, batch, precision, true, flags, plan);
+}
+
+// pass k of a convolve lines plan: launched on the plan's stream, or (ops) only recorded, phase = k
+template <typename T>
+static cudaError_t conv_line_pass(const dfft_lines_plan_s* p, int k, const void* in, void* out, const void* mult, bool shared,
+                                  std::vector<std::string>* ops = nullptr)
+{
+    const LinePass& lp = p->cpass[k];
+    ConvArgs<T> c{};
+    RealZArgs<T> r{};
+    real_line_args<T>(lp, line_buf(lp.src, in, out, p->temp), line_buf(lp.dst, in, out, p->temp), lp.inv ? DFFT_BACKWARD : DFFT_FORWARD, r);
+    const bool realk = lp.kind == PK_Z_R2C || lp.kind == PK_Z_C2R;
+    if (lp.plane) {
+        const PlaneArgs<T> pa{r.t.in, r.t.out, r.t.lut, lp.ntiles, r.t.inv};
+        if (ops) record_op<T>(*ops, "XY_PLANE", k, lp.e->N, lp.e->N, false, false, false, r.t);
+        return ops ? cudaSuccess : lp.e->plane(&pa, p->sms, p->stream);
+    }
+    if (lp.kind == PK_XCONV) {
+        c.t = r.t;
+        c.t.do_scale = p->scale != 0; c.t.scale = (T)p->scale;
+        c.mult = (const cx<T>*)mult; c.mult_shared = shared ? 1 : 0;
+    }
+    if (ops) {
+        char extra[128] = "";
+        if (realk) snprintf(extra, sizeof(extra), ", \"nzh\": %d, \"pair\": [%lld, %lld]", lp.e->N / 2 + 1, lp.ld_in, lp.ld_out);
+        if (lp.kind == PK_XCONV) snprintf(extra, sizeof(extra), ", \"mult\": %llu, \"shared\": %d", (unsigned long long)(size_t)mult, shared ? 1 : 0);
+        const int C = realk || lp.kind == PK_Z ? lp.e->z_C : lp.e->s_C;
+        record_op<T>(*ops, kPassNames[lp.kind], k, lp.e->N, C, false, false, false, lp.kind == PK_XCONV ? c.t : r.t, extra);
+        return cudaSuccess;
+    }
+    const void* args = realk ? (const void*)&r : lp.kind == PK_XCONV ? (const void*)&c : (const void*)&r.t;
+    return lp.e->launch[lp.kind](args, p->sms, p->stream);
+}
+
+template <typename T> static int lines_execute_conv_impl(dfft_lines_plan p, const void* in, void* out, const void* mult, bool shared)
+{
+    CU(cudaEventRecord(p->ev[0], p->stream));
+    for (int k = 0; k < p->nconv; k++) {
+        if (p->cpass[k].ntiles <= 0) continue;
+        const cudaError_t err = conv_line_pass<T>(p, k, in, out, mult, shared);
+        if (err != cudaSuccess) return fail(DFFT_ECUDA, "convolve line pass launch failed: %s", cudaGetErrorString(err));
+    }
+    CU(cudaEventRecord(p->ev[1], p->stream));
+    p->timed = true;
+    return 0;
+}
+
+extern "C" int dfft_lines_execute_convolve(dfft_lines_plan p, const void* in, void* out, const void* mult, long long mult_count)
+{
+    if (!p || !in || !out || !mult) return fail(DFFT_EINVAL, "bad arguments");
+    if (!p->conv) return fail(DFFT_EINVAL, "dfft_lines_execute_convolve needs a plan from dfft_lines_plan_create_convolve_3d / _r2c_3d");
+    if (mult_count != 1 && mult_count != p->batch) return fail(DFFT_EINVAL, "mult_count must be 1 or the plan's batch (%lld), not %lld", p->batch, mult_count);
+    const size_t rsz = p->prec == DFFT_FLOAT ? 4 : 8, csz = 2 * rsz, esz = p->real ? rsz : csz;
+    const uintptr_t a = (uintptr_t)in, b = (uintptr_t)out, m = (uintptr_t)mult;
+    if (a % esz || b % esz || m % csz) return fail(DFFT_EINVAL, "a buffer is not aligned to its element size");
+    const uintptr_t io = (uintptr_t)((p->real ? p->rcount : p->ccount) * esz), mb = (uintptr_t)(mult_count * p->mvol * csz);
+    if (a != b && a < b + io && b < a + io) return fail(DFFT_EINVAL, "`in` and `out` overlap without being the same buffer");
+    if (m < b + io && b < m + mb) return fail(DFFT_EINVAL, "the multiplier overlaps `out`");
+    CU(cudaSetDevice(p->device));
+    const bool shared = mult_count == 1;
+    return p->prec == DFFT_DOUBLE ? lines_execute_conv_impl<double>(p, in, out, mult, shared) : lines_execute_conv_impl<float>(p, in, out, mult, shared);
+}
+
+/* test hook (host only): the passes of a convolve lines plan, JSON as dfft_debug_lines_3d_ops; in = buffer 5, out = 2,
+ * temporary = 4, multiplier = 8 of device 0.  XCONV carries "mult" and "shared" (1: mult_count == 1) */
+extern "C" long long dfft_debug_lines_conv_3d_ops(int nx, int ny, int nz, long long batch, int precision, int real, unsigned flags,
+                                                  long long mult_count, char* buf, long long cap)
+{
+    dfft_lines_plan_s lp;
+    lp.prec = precision;
+    const int rc = make_lines_conv_3d(&lp, nx, ny, nz, batch, precision, real != 0, flags, true);
+    if (rc) return rc;
+    if (mult_count != 1 && mult_count != batch) return fail(DFFT_EINVAL, "mult_count must be 1 or the plan's batch");
+    std::vector<std::string> ops;
+    for (int k = 0; k < lp.nconv; k++) conv_line_pass<double>(&lp, k, fake_addr(0, 5), fake_addr(0, 2), fake_addr(0, 8), mult_count == 1, &ops);
     lp.temp = nullptr;
     return ops_json(ops, buf, cap);
 }

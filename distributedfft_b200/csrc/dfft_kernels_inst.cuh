@@ -64,12 +64,14 @@ cudaError_t launch_real(const void* vargs, int sm_count, cudaStream_t st)
     return cudaGetLastError();
 }
 
-// spectral convolution column pass (fft_conv_kernel): vargs is a ConvArgs<T>
-template <class S, typename T, int C, bool TW, bool CO, int MINB, bool PP>
-cudaError_t launch_conv(const void* vargs, int sm_count, cudaStream_t st)
+// spectral convolution column pass (fft_conv_kernel, or fft_conv_shared_kernel when ConvArgs::mult_shared): vargs is a ConvArgs<T>
+template <class S, typename T, int C, bool TW, bool CO, int MINB, bool PP, bool SH>
+cudaError_t launch_conv_k(const ConvArgs<T>& a, int sm_count, cudaStream_t st)
 {
-    const ConvArgs<T>& a = *reinterpret_cast<const ConvArgs<T>*>(vargs);
-    auto kern = fft_conv_kernel<S, T, C, TW, CO, MINB, PP>;
+    auto kern = [] {   // only the kernel of this mode is instantiated
+        if constexpr (SH) return fft_conv_shared_kernel<S, T, C, TW, MINB, PP>;
+        else return fft_conv_kernel<S, T, C, TW, CO, MINB, PP>;
+    }();
     constexpr size_t smem = TileSmem<S, T, C, PP>::bytes(CO);
     static std::atomic<int> occ_cache[64];
     int dev = 0;
@@ -89,6 +91,18 @@ cudaError_t launch_conv(const void* vargs, int sm_count, cudaStream_t st)
     if (grid > a.t.ntiles) grid = a.t.ntiles;
     kern<<<(unsigned)grid, S::T * C, smem, st>>>(a);
     return cudaGetLastError();
+}
+
+template <class S, typename T, int C, bool TW, bool CO, int MINB, bool PP>
+cudaError_t launch_conv(const void* vargs, int sm_count, cudaStream_t st)
+{
+    const ConvArgs<T>& a = *reinterpret_cast<const ConvArgs<T>*>(vargs);
+    if constexpr (!CO) {   // the shared multiplier exists for the local-store kind only
+        if (a.mult_shared) return launch_conv_k<S, T, C, TW, CO, MINB, PP, true>(a, sm_count, st);
+    } else {
+        if (a.mult_shared) return cudaErrorInvalidValue;
+    }
+    return launch_conv_k<S, T, C, TW, CO, MINB, PP, false>(a, sm_count, st);
 }
 
 // X + Y passes of square planes (fft_plane_kernel): vargs is a PlaneArgs<T>; P planes per CTA

@@ -427,14 +427,18 @@ __global__ void __launch_bounds__(S::T* C, MINB) fft_tile_kernel(const TileArgs<
 // input map with the multiplier's own base (its layout is the receive buffer's [x][y_l][z']) and the inverse run starts from the
 // same register layout.  Unnormalised (x N per axis); TileArgs::do_scale folds 1/scale into the multiply.  TileArgs::inv is unused.
 // CHUNK_OUT: the store is split by x (ChunkTab co, the PK_XB_CO addressing) into the peers' receive buffers.
+// SHARED (fft_conv_shared_kernel, local store only): the multiplier's offset leaves out a * ia.SA, so one multiplier serves every
+// `a` (every volume of a batched lines plan).  A kernel of its own rather than a run-time branch: the per-volume kernel every
+// slab plan runs compiles to the same code as before (the extra address arithmetic moved registers and spills of some kinds).
 // ------------------------------------------------------------------------------------------
 template <typename T> struct ConvArgs {
     TileArgs<T> t;
     const cx<T>* mult;
+    int mult_shared;       // launcher only: 1 runs fft_conv_shared_kernel; 0 (the slab plans zero-initialise ConvArgs) the per-volume kernel
 };
 
-template <class S, typename T, int C, bool TWREG, bool CHUNK_OUT, int MINB, bool PINGPONG>
-__global__ void __launch_bounds__(S::T* C, MINB) fft_conv_kernel(const ConvArgs<T> R)
+template <class S, typename T, int C, bool TWREG, bool CHUNK_OUT, bool PINGPONG, bool SHARED>
+__device__ __forceinline__ void conv_tiles(const ConvArgs<T>& R)
 {
     static_assert(S::valid(), "bad schedule");
     using Op = TileOp<S, T, C, MAP_C, MAP_C, TWREG, false, CHUNK_OUT, PINGPONG>;
@@ -453,6 +457,7 @@ __global__ void __launch_bounds__(S::T* C, MINB) fft_conv_kernel(const ConvArgs<
         const int b = (int)(tile - a * A.G);
         const bool ok = b * C + c < A.W;
         const long long off = a * A.ia.SA + b * A.ia.SB + c * A.ia.cs + (long long)t * A.ia.es;
+        const long long moff = SHARED ? off - a * A.ia.SA : off;
         cx<T> v[RR];
 #pragma unroll
         for (int u = 0; u < RR; u++) v[u] = ok ? ld_stream(A.in + off + (long long)u * TT * A.ia.es) : mk<T>(0, 0);
@@ -460,7 +465,7 @@ __global__ void __launch_bounds__(S::T* C, MINB) fft_conv_kernel(const ConvArgs<
         // multiply, then the inverse as swap -> forward -> swap (the swap-in is folded into the multiply's result)
 #pragma unroll
         for (int u = 0; u < RR; u++) {
-            cx<T> m = ok ? ld_stream(R.mult + off + (long long)u * TT * A.ia.es) : mk<T>(0, 0);
+            cx<T> m = ok ? ld_stream(R.mult + moff + (long long)u * TT * A.ia.es) : mk<T>(0, 0);
             if (do_scale) { m.x *= A.scale; m.y *= A.scale; }
             v[u] = cswap(cmul(v[u], m));
         }
@@ -484,6 +489,18 @@ __global__ void __launch_bounds__(S::T* C, MINB) fft_conv_kernel(const ConvArgs<
         }
     }
     signal_when_grid_done<T>(A);
+}
+
+template <class S, typename T, int C, bool TWREG, bool CHUNK_OUT, int MINB, bool PINGPONG>
+__global__ void __launch_bounds__(S::T* C, MINB) fft_conv_kernel(const ConvArgs<T> R)
+{
+    conv_tiles<S, T, C, TWREG, CHUNK_OUT, PINGPONG, false>(R);
+}
+
+template <class S, typename T, int C, bool TWREG, int MINB, bool PINGPONG>
+__global__ void __launch_bounds__(S::T* C, MINB) fft_conv_shared_kernel(const ConvArgs<T> R)
+{
+    conv_tiles<S, T, C, TWREG, false, PINGPONG, true>(R);
 }
 
 // ------------------------------------------------------------------------------------------

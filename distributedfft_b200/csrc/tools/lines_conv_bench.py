@@ -1,0 +1,195 @@
+#!/usr/bin/env python
+"""Batched 3-D spectral convolution: the convolve lines plan against the three calls it replaces, one GPU (developer tool).
+
+    python distributedfft_b200/csrc/tools/lines_conv_bench.py [--steps 30] [--rounds 3] [--warmup 5] [--case NAME]
+
+Every case convolves `batch` volumes with one multiplier of unit modulus / N (so repeated in-place steps keep their magnitude).
+Four arms get the same seeded data:
+  shared   LinesConvolvePlan, one multiplier for every volume (mult_count = 1), out of place
+  pervol   the same plan with `batch` identical copies of the multiplier (mult_count = batch)
+  3call    LinesPlan(three_d=...) forward in place, torch multiply by the shared multiplier, LinesPlan backward
+           (real: RealLinesPlan forward into a spectrum buffer, multiply, backward into the output)
+  torch    torch.fft.fftn * m -> ifftn (rfftn / irfftn for real cases; cuFFT, for context)
+Before timing, the outputs of all four are compared: shared and pervol with np.array_equal, 3call and torch by rel_l2 against
+shared.  Each round times `steps` executes of each arm with CUDA events on the arm's own stream (the plans' streams; torch's
+current stream for torch), arms alternating, after `warmup` untimed executes.
+
+Prints one JSON object per case and a summary table: ms per step (median of the rounds), conv / 3call, and the HBM sweep model
+of each arm in bytes with its GB/s at the measured time (V = one sweep of the batch, M = the multiplier as read):
+  C2C plane shape  conv 6V + M      3call 10V + M
+  C2C other        conv 10V + M     3call 14V + M
+  real             conv 2Vr + 8Vc + M   3call 2Vr + 12Vc + M   (Vr: real data, Vc: the half spectra)
+Card name, power limit and SM clock (nvidia-smi, read-only query) are printed before and after."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+sys.path.insert(0, ROOT)
+
+# name, precision ("d" / "f"), (nx, ny, nz, batch), real.  128^3 has no plane kernel; 48^3 is a non-power-of-two plane
+CASES = [
+    ("16^3x16384", "d", (16, 16, 16, 16384), False), ("32^3x2048", "d", (32, 32, 32, 2048), False),
+    ("64^3x256", "d", (64, 64, 64, 256), False), ("128^3x32", "d", (128, 128, 128, 32), False),
+    ("48^3x512", "d", (48, 48, 48, 512), False),
+    ("16^3x16384-f32", "f", (16, 16, 16, 16384), False), ("32^3x2048-f32", "f", (32, 32, 32, 2048), False),
+    ("64^3x256-f32", "f", (64, 64, 64, 256), False),
+    ("real-64^3x256", "d", (64, 64, 64, 256), True),
+]
+
+
+def gpu_state():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm", "--format=csv,noheader", "-i", "0"],
+                             capture_output=True, text=True, timeout=20).stdout.strip()
+        name, plim, clk = [s.strip() for s in out.split(",")]
+        return {"name": name, "power_limit": plim, "sm_clock": clk}
+    except Exception as exc:   # the numbers still stand; the record says why the card state is missing
+        return {"error": str(exc)}
+
+
+def time_steps(torch, stream, fn, steps):
+    st = torch.cuda.ExternalStream(stream) if stream is not None else torch.cuda.current_stream()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record(st)
+    with torch.cuda.stream(st):
+        for _ in range(steps):
+            fn()
+    b.record(st)
+    b.synchronize()
+    return a.elapsed_time(b) / steps
+
+
+def run_case(torch, np, dfft, case, args):
+    name, p, shape, real = case
+    nx, ny, nz, batch = shape
+    prec = dfft.FLOAT if p == "f" else dfft.DOUBLE
+    rdt, cdt = (torch.float32, torch.complex64) if p == "f" else (torch.float64, torch.complex128)
+    er = 4 if p == "f" else 8
+    ec = 2 * er
+    H = nx // 2 + 1
+    N = nx * ny * nz
+    mx = H if real else nx
+    dims = (-3, -2, -1)
+    gen = torch.Generator(device="cuda").manual_seed(7)
+    x = torch.randn((batch, nz, ny, nx), dtype=rdt if real else cdt, device="cuda", generator=gen)
+    phase = torch.rand((nz, ny, mx), dtype=rdt, device="cuda", generator=gen) * (2 * np.pi)
+    m1 = (torch.polar(torch.ones_like(phase), phase) / N).to(cdt).contiguous()
+    mb = m1.expand(batch, nz, ny, mx).contiguous()
+    conv = dfft.LinesConvolvePlan(shape, precision=prec, real=real)
+    fwd = dfft.RealLinesPlan(three_d=shape, precision=prec) if real else dfft.LinesPlan(three_d=shape, precision=prec)
+    try:
+        y = {k: torch.empty_like(x) for k in ("shared", "pervol")}
+        z = x.clone()                                                                 # the three-call arm's buffer
+        spec = torch.empty((batch, nz, ny, H), dtype=cdt, device="cuda") if real else None
+        zout = torch.empty_like(x) if real else z
+
+        def three_calls():
+            if real:
+                fwd.execute(x.data_ptr(), spec.data_ptr(), dfft.FORWARD)
+                spec.mul_(m1)
+                fwd.execute(spec.data_ptr(), zout.data_ptr(), dfft.BACKWARD)
+            else:
+                fwd.execute(z.data_ptr(), dfft.FORWARD)
+                z.mul_(m1)
+                fwd.execute(z.data_ptr(), dfft.BACKWARD)
+
+        def torch_arm():
+            if real:
+                return torch.fft.irfftn(torch.fft.rfftn(x, dim=dims) * m1, s=(nz, ny, nx), dim=dims)
+            return torch.fft.ifftn(torch.fft.fftn(x, dim=dims) * m1, dim=dims)
+
+        jobs = {
+            "shared": (conv.stream, lambda: conv.execute(x.data_ptr(), y["shared"].data_ptr(), m1.data_ptr(), 1)),
+            "pervol": (conv.stream, lambda: conv.execute(x.data_ptr(), y["pervol"].data_ptr(), mb.data_ptr(), batch)),
+            "3call": (fwd.stream, three_calls),
+            "torch": (None, torch_arm),
+        }
+        # cross-check before timing: one step of every arm from the same input
+        torch.cuda.synchronize()
+        for k in ("shared", "pervol"):
+            jobs[k][1]()
+        conv.synchronize()
+        with torch.cuda.stream(torch.cuda.ExternalStream(fwd.stream)):
+            three_calls()
+        fwd.synchronize()
+        t_out = torch_arm() * N                                                       # torch's ifftn is normalised
+        torch.cuda.synchronize()
+        ref = y["shared"]
+
+        def rel(a):
+            return float(torch.linalg.vector_norm(a - ref) / torch.linalg.vector_norm(ref))
+        check = {"shared_eq_pervol": bool(torch.equal(y["shared"], y["pervol"])), "rel_l2_3call": rel(zout), "rel_l2_torch": rel(t_out)}
+        del t_out
+        for st, fn in jobs.values():
+            with torch.cuda.stream(torch.cuda.ExternalStream(st) if st is not None else torch.cuda.current_stream()):
+                for _ in range(args.warmup):
+                    fn()
+        torch.cuda.synchronize()
+        rounds = []
+        for _ in range(args.rounds):
+            rounds.append({k: time_steps(torch, st, fn, args.steps) for k, (st, fn) in jobs.items()})
+        torch.cuda.synchronize()
+    finally:
+        conv.destroy()
+        fwd.destroy()
+    med = {k: float(np.median([r[k] for r in rounds])) for k in rounds[0]}
+    plane = dfft.lines_conv_3d_ops(nx, ny, nz, batch, prec, real)[0]["op"] == "XY_PLANE"
+    Msh, Mpv = ec * nz * ny * mx, ec * nz * ny * mx * batch
+    if real:
+        Vr, Vc = er * N * batch, ec * nz * ny * H * batch
+        conv_b, call_b = 2 * Vr + 8 * Vc, 2 * Vr + 12 * Vc
+        model = "conv 2Vr+8Vc+M, 3call 2Vr+12Vc+M"
+    else:
+        V = ec * N * batch
+        conv_b, call_b = (6 * V, 10 * V) if plane else (10 * V, 14 * V)
+        model = "conv 6V+M, 3call 10V+M" if plane else "conv 10V+M, 3call 14V+M"
+    model_bytes = {"shared": conv_b + Msh, "pervol": conv_b + Mpv, "3call": call_b + Msh}
+    res = {
+        "case": name, "precision": "float" if p == "f" else "double", "shape": list(shape), "real": real, "plane_kernel": plane,
+        "steps": args.steps, "rounds": rounds, "median_ms": med,
+        "ratio_shared_vs_3call": med["shared"] / med["3call"], "ratio_pervol_vs_3call": med["pervol"] / med["3call"],
+        "sweep_model": model, "model_bytes": model_bytes,
+        "model_gbps": {k: b / med[k] / 1e6 for k, b in model_bytes.items()}, "cross_check": check,
+    }
+    torch.cuda.empty_cache()
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=30)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--case", action="append", help="run only these cases (default: all)")
+    args = ap.parse_args()
+    import numpy as np
+    import torch
+    import distributedfft_b200 as dfft
+
+    torch.cuda.set_device(0)
+    for var in ("DFFT_NO_PLANE", "DFFT_FORCE_PLANE", "DFFT_GENERIC", "DFFT_VARIANT"):
+        os.environ.pop(var, None)
+    print(json.dumps({"gpu_before": gpu_state()}), flush=True)
+    results = []
+    for case in CASES:
+        if args.case and case[0] not in args.case:
+            continue
+        r = run_case(torch, np, dfft, case, args)
+        results.append(r)
+        print(json.dumps(r), flush=True)
+    print(json.dumps({"gpu_after": gpu_state()}), flush=True)
+    print("%-16s %5s %9s %9s %9s %9s %6s %6s %7s %7s %7s  %s" % (
+        "case", "plane", "shared", "pervol", "3call", "torch", "sh/3c", "pv/3c", "GB/s_sh", "GB/s_pv", "GB/s_3c", "cross-check"))
+    for r in results:
+        m, g, c = r["median_ms"], r["model_gbps"], r["cross_check"]
+        print("%-16s %5s %9.3f %9.3f %9.3f %9.3f %6.3f %6.3f %7.0f %7.0f %7.0f  eq=%s 3call=%.1e torch=%.1e" % (
+            r["case"], "on" if r["plane_kernel"] else "off", m["shared"], m["pervol"], m["3call"], m["torch"],
+            r["ratio_shared_vs_3call"], r["ratio_pervol_vs_3call"], g["shared"], g["pervol"], g["3call"],
+            c["shared_eq_pervol"], c["rel_l2_3call"], c["rel_l2_torch"]))
+
+
+if __name__ == "__main__":
+    main()

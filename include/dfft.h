@@ -306,6 +306,31 @@ long long dfft_debug_real_lines_ops(int n, int ny, long long batch, int precisio
  * buffer 1) / dfft_debug_real_lines_ops (real != 0); the plane kernel is one "XY_PLANE" record over ntiles planes */
 long long dfft_debug_lines_3d_ops(int nx, int ny, int nz, long long batch, int precision, int direction, int real,
                                   char* buf, long long cap);
+/* Batched 3-D spectral convolution on the lines engine: batch row-major nz x ny x nx volumes (nx fastest),
+ *   C2C: out = ifftn(fftn(in) * m) over axes (1, 2, 3), unnormalised (x nx*ny*nz) unless DFFT_SCALE_BACKWARD;
+ *   R2C: out = irfftn(rfftn(in) * m, s=(nz, ny, nx)) * nx*ny*nz, real in / real out (numpy's C2R convention, as
+ *        dfft_plan_convolve_r2c_3d: the imaginary parts the C2R ignores are ignored here too).
+ * m is complex in the plan's precision, natural order: [z][y][x] (C2C) or [z][y][nx/2+1] (R2C) per volume.  One execute runs
+ * the forward passes of the 3-D lines plan with the Z pass replaced by one column pass that transforms along z, multiplies and
+ * transforms back (the slab convolve plan's fused X pass), then the passes before it inverted: 3 launches where nx == ny has the
+ * plane kernel of dfft_lines_plan_create_3d (read at creation, DFFT_NO_PLANE / DFFT_FORCE_PLANE as there), 5 otherwise.  The
+ * R2C plan owns a temporary of batch*nz*ny*(nx/2+1) complex elements.
+ * Lengths: nz needs a tuned kernel of the default table (dfft_length_kind(nz, precision) == 2; DFFT_GENERIC and DFFT_VARIANT
+ * entries are DFFT_EUNSUPPORTED).  C2C: nx and ny as dfft_lines_plan_create_3d; R2C: nx as dfft_lines_plan_create_r2c_3d, ny as
+ * a strided C2C lines pass.  2^31 or more rows are DFFT_EUNSUPPORTED, as in the 3-D lines plans.
+ * Flags: DFFT_SCALE_BACKWARD folds 1/(nx*ny*nz) into the multiply; any other bit is DFFT_EINVAL. */
+int dfft_lines_plan_create_convolve_3d(int nx, int ny, int nz, long long batch, int precision, unsigned flags, dfft_lines_plan* plan);
+int dfft_lines_plan_create_convolve_r2c_3d(int nx, int ny, int nz, long long batch, int precision, unsigned flags, dfft_lines_plan* plan);
+/* mult_count = 1: one multiplier shared by every volume; = batch: one per volume, densely packed.  in == out (in place) or
+ * disjoint buffers; `in` is never written when they are distinct, `mult` never.  DFFT_EINVAL: a null pointer, a buffer not
+ * aligned to its element size (fp32 complex at an 8-byte offset is fine), a partial overlap of in and out, a multiplier that
+ * overlaps out, another mult_count, and a plan that is not a convolve lines plan (dfft_lines_execute / dfft_lines_execute_real
+ * on a convolve plan are DFFT_EINVAL too).  Asynchronous on the plan's stream (dfft_lines_synchronize waits). */
+int dfft_lines_execute_convolve(dfft_lines_plan plan, const void* in, void* out, const void* mult, long long mult_count);
+/* test hook (host only): the passes of either convolve lines plan, JSON as dfft_debug_lines_3d_ops with in = buffer 5, out = 2,
+ * temporary = 4, multiplier = 8; the column pass is "XCONV" with "mult" and "shared" (1 when mult_count == 1) */
+long long dfft_debug_lines_conv_3d_ops(int nx, int ny, int nz, long long batch, int precision, int real, unsigned flags,
+                                       long long mult_count, char* buf, long long cap);
 /* one-shot convenience (plan + execute + synchronize + destroy), used by the per-axis parity tests */
 int dfft_fft_lines(void* data, int n, long long stride, long long nlines, long long inner, long long inner_dist,
                    long long outer_dist, int direction, int precision);
