@@ -38,7 +38,7 @@ __all__ = [
     "BootstrapComm", "fft_mpi_init", "fft_mpi_plan_dft_c2c_3d", "fft_mpi_execute_dft_3d_c2c", "fft_mpi_destroy_plan",
     "fft_mpi_alloc_local_memory", "fft_mpi_local_size_3d", "fft_mpi_cleanup", "getMaxDataCount", "supported_lengths",
     "fft_mpi_plan_dft_r2c_3d", "local_size_r2c_3d", "fft_mpi_plan_dft_convolve_3d",
-    "fft_lines", "lines_ops", "LinesPlan", "RealLinesPlan", "real_lines_ops", "lines_3d_ops", "LinesConvolvePlan", "lines_conv_3d_ops", "length_kind", "length_schedule", "memcpy_htod", "memcpy_dtoh", "exchange_table", "comm_allgather",
+    "fft_lines", "lines_ops", "LinesPlan", "RealLinesPlan", "real_lines_ops", "lines_3d_ops", "LinesConvolvePlan", "lines_conv_3d_ops", "lines_conv_2d_ops", "length_kind", "length_schedule", "memcpy_htod", "memcpy_dtoh", "exchange_table", "comm_allgather",
 ]
 
 
@@ -114,6 +114,10 @@ def lib():
     L.dfft_lines_execute_convolve.argtypes = [vp, vp, vp, vp, ll]
     L.dfft_debug_lines_conv_3d_ops.argtypes = [i, i, i, ll, i, i, ctypes.c_uint, ll, ctypes.c_char_p, ll]
     L.dfft_debug_lines_conv_3d_ops.restype = ll
+    L.dfft_lines_plan_create_convolve_2d.argtypes = [i, i, ll, i, ctypes.c_uint, P(vp)]
+    L.dfft_lines_plan_create_convolve_r2c_2d.argtypes = [i, i, ll, i, ctypes.c_uint, P(vp)]
+    L.dfft_debug_lines_conv_2d_ops.argtypes = [i, i, ll, i, i, ctypes.c_uint, ll, ctypes.c_char_p, ll]
+    L.dfft_debug_lines_conv_2d_ops.restype = ll
     L.dfft_debug_real_lines_ops.argtypes = [i, i, ll, i, i, i, ctypes.c_char_p, ll]
     L.dfft_debug_real_lines_ops.restype = ll
     L.dfft_length_kind.argtypes = [i, i]
@@ -472,12 +476,17 @@ class LinesConvolvePlan:
     a[batch][nz][ny][nx], unnormalised (x nx*ny*nz) unless flags=SCALE_BACKWARD; with real=True, real in / real out,
     out = irfftn(rfftn(in) * m, s=(nz, ny, nx)) * nx*ny*nz.  m is complex in the plan's precision, [nz][ny][nx] (real:
     [nz][ny][nx//2+1]) per volume; execute with mult_count=1 shares one multiplier among all volumes, mult_count=batch gives
-    each its own.  in_ptr == out_ptr runs in place; `in` and the multiplier are never written otherwise."""
+    each its own.  in_ptr == out_ptr runs in place; `in` and the multiplier are never written otherwise.
+    `two_d=(nx, ny, batch)` instead: the same over the last two axes of a[batch][ny][nx] (m: [ny][nx], real: [ny][nx//2+1]
+    per image).  Exactly one of three_d and two_d is given."""
 
-    def __init__(self, three_d, precision=DOUBLE, real=False, flags=0):
+    def __init__(self, three_d=None, precision=DOUBLE, real=False, flags=0, two_d=None):
+        if (three_d is None) == (two_d is None):
+            raise ValueError("give exactly one of three_d and two_d")
         h = ctypes.c_void_p()
-        name = "dfft_lines_plan_create_convolve_r2c_3d" if real else "dfft_lines_plan_create_convolve_3d"
-        _check(getattr(lib(), name)(*three_d, precision, flags, ctypes.byref(h)), name)
+        dims = "3d" if two_d is None else "2d"
+        name = ("dfft_lines_plan_create_convolve_r2c_" if real else "dfft_lines_plan_create_convolve_") + dims
+        _check(getattr(lib(), name)(*(three_d if two_d is None else two_d), precision, flags, ctypes.byref(h)), name)
         self.handle = h
 
     def execute(self, in_ptr, out_ptr, mult_ptr, mult_count=1):
@@ -507,6 +516,20 @@ def lines_conv_3d_ops(nx, ny, nz, batch, precision=DOUBLE, real=False, flags=0, 
         raise DfftError(f"dfft_debug_lines_conv_3d_ops failed ({need}): " + lib().dfft_last_error().decode())
     buf = ctypes.create_string_buffer(int(need))
     lib().dfft_debug_lines_conv_3d_ops(*args, buf, need)
+    return json.loads(buf.value.decode())
+
+
+def lines_conv_2d_ops(nx, ny, batch, precision=DOUBLE, real=False, flags=0, mult_count=1):
+    """passes LinesConvolvePlan(two_d=(nx, ny, batch), ...) would launch per execute (host-only test hook, see
+    dfft_debug_lines_conv_2d_ops; buffers as lines_conv_3d_ops); read DFFT_NO_PLANE / DFFT_FORCE_PLANE / DFFT_GENERIC at the
+    call, as plan creation does"""
+    import json
+    args = (nx, ny, batch, precision, int(bool(real)), flags, mult_count)
+    need = lib().dfft_debug_lines_conv_2d_ops(*args, None, 0)
+    if need < 0:
+        raise DfftError(f"dfft_debug_lines_conv_2d_ops failed ({need}): " + lib().dfft_last_error().decode())
+    buf = ctypes.create_string_buffer(int(need))
+    lib().dfft_debug_lines_conv_2d_ops(*args, buf, need)
     return json.loads(buf.value.decode())
 
 

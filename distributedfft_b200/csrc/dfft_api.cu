@@ -2226,7 +2226,9 @@ struct LinePass {
     long long tw_n = 0;          // four-step twiddle modulus (PK_XF_TW)
     int src = 0, dst = 0;        // LB_IN (the caller's data / a real plan's `in`), LB_TEMP (the plan's temporary), LB_OUT
     long long ld_in = 0, ld_out = 0;   // PK_Z_R2C / PK_Z_C2R: distance between the two lines of a pair (RealZArgs), each side's elements
-    bool plane = false;          // X + Y of ntiles whole e->N x e->N planes in one launch of e->plane (PlaneArgs); `kind` unused
+    bool plane = false;          // X + Y of ntiles whole e->N x e->N planes in one launch of e->plane (PlaneArgs); `kind` unused,
+                                 // except that kind == PK_XCONV is the whole 2-D convolution of ntiles images in one launch of
+                                 // e->plane_conv (PlaneConvArgs)
     bool inv = false;            // convolve plans: this pass runs the inverse transform
 };
 enum { LB_IN = 0, LB_TEMP = 1, LB_OUT = 2 };
@@ -2241,14 +2243,14 @@ struct dfft_lines_plan_s {
     int nreal = 0;
     LinePass rpass[2][3];
     long long rcount = 0, ccount = 0;   // reals and complex elements of the caller's real / complex buffer
-    // convolve plans (dfft_lines_plan_create_convolve_[r2c_]3d): the passes of one execute in order, the multiply folded into the
-    // PK_XCONV pass; `pass` and `rpass` stay empty.  Read by dfft_lines_execute_convolve and dfft_debug_lines_conv_3d_ops alike.
-    // Inverse passes share their forward pass's twiddle table
+    // convolve plans (dfft_lines_plan_create_convolve_[r2c_]{2d,3d}): the passes of one execute in order, the multiply folded
+    // into the PK_XCONV pass; `pass` and `rpass` stay empty.  Read by dfft_lines_execute_convolve and the
+    // dfft_debug_lines_conv_{2d,3d}_ops hooks alike.  Inverse passes share their forward pass's twiddle table
     bool conv = false;
     int nconv = 0;
     LinePass cpass[5];
-    long long batch = 0, mvol = 0;   // volumes; complex elements of one volume's multiplier
-    double scale = 0;                // DFFT_SCALE_BACKWARD: 1 / (nx*ny*nz), folded into the multiply; 0 = unnormalised
+    long long batch = 0, mvol = 0;   // volumes (images); complex elements of one volume's (image's) multiplier
+    double scale = 0;                // DFFT_SCALE_BACKWARD: 1 / (elements of a volume or image), folded into the multiply; 0 = unnormalised
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[2] = {nullptr, nullptr};
     bool timed = false;
@@ -2402,6 +2404,16 @@ extern "C" int dfft_lines_plan_create(int n, long long stride, long long nlines,
     return 0;
 }
 
+// batch ny x nx matrices (nx fastest), in place: X along the batch*ny rows, Y over the nx columns of every matrix (stride nx);
+// backward in reverse
+static int make_lines_2d(dfft_lines_plan p, int nx, int ny, long long batch, int precision, bool dry)
+{
+    int rc = make_line_pass(p->pass[0], nx, 1, (long long)ny * batch, (long long)ny * batch, nx, 0, precision, dry);
+    if (!rc) rc = make_line_pass(p->pass[1], ny, nx, (long long)nx * batch, nx, 1, (long long)nx * ny, precision, dry);
+    p->npass = 2;
+    return rc;
+}
+
 /* batch of 2-D transforms, nx fastest: the reference's FFTdim = 2 application (Test_2D.cpp: size = {X, Y, Z}) */
 extern "C" int dfft_lines_plan_create_2d(int nx, int ny, long long batch, int precision, dfft_lines_plan* out)
 {
@@ -2410,10 +2422,8 @@ extern "C" int dfft_lines_plan_create_2d(int nx, int ny, long long batch, int pr
     if (nx < 1 || ny < 1 || batch < 0 || (precision != DFFT_DOUBLE && precision != DFFT_FLOAT)) return fail(DFFT_EINVAL, "bad arguments");
     dfft_lines_plan p = new dfft_lines_plan_s;
     int rc = lines_plan_common(p, precision);
-    if (!rc) rc = make_line_pass(p->pass[0], nx, 1, (long long)ny * batch, (long long)ny * batch, nx, 0, precision);
-    if (!rc) rc = make_line_pass(p->pass[1], ny, nx, (long long)nx * batch, nx, 1, (long long)nx * ny, precision);
+    if (!rc) rc = make_lines_2d(p, nx, ny, batch, precision, false);
     if (rc) { dfft_lines_destroy(p); return rc; }
-    p->npass = 2;
     *out = p;
     return 0;
 }
@@ -2522,11 +2532,7 @@ extern "C" long long dfft_debug_lines_ops(int n, long long stride, long long nli
     lp.prec = precision;
     int rc = 0;
     if (two_d) {
-        const int nx = n, ny = (int)stride;
-        const long long batch = nlines;
-        rc = make_line_pass(lp.pass[0], nx, 1, (long long)ny * batch, (long long)ny * batch, nx, 0, precision, true);
-        if (!rc) rc = make_line_pass(lp.pass[1], ny, nx, (long long)nx * batch, nx, 1, (long long)nx * ny, precision, true);
-        lp.npass = 2;
+        rc = make_lines_2d(&lp, n, (int)stride, nlines, precision, true);
     } else if (!find_size_entry(n, precision) && stride == 1 && inner_dist == n) {
         rc = make_four_step(&lp, n, nlines, precision, true);
     } else {
@@ -2760,25 +2766,42 @@ extern "C" long long dfft_debug_lines_3d_ops(int nx, int ny, int nz, long long b
     return ops_json(ops, buf, cap);
 }
 
-// ---- batched 3-D spectral convolution on the lines engine: out = ifftn(fftn(in) * m) per volume --------------------------------
-// The forward passes of the 3-D lines plan (make_lines_3d / make_real_lines), the Z pass replaced by PK_XCONV (forward Z, multiply,
-// inverse Z in one column pass, as the slab convolve plan's X pass; fft_conv_shared_kernel when one multiplier serves every
-// volume), then the forward passes before Z again, inverse and in reverse order:
-//   C2C, plane kernel: XY_PLANE in -> out, XCONV, inverse XY_PLANE (6 volume sweeps + the multiplier)
-//   C2C, other shapes: X in -> out, Y, XCONV, inverse Y, inverse X (10 sweeps)
-//   R2C:               Z_R2C in -> temp, Y, XCONV, inverse Y, Z_C2R temp -> out
+// ---- batched 2-D and 3-D spectral convolution on the lines engine: out = ifftn(fftn(in) * m) per image / volume ---------------
+// The forward passes of the 2-D or 3-D lines plan (make_lines_2d / make_lines_3d / make_real_lines), the last one (Y in 2-D, Z in
+// 3-D) replaced by PK_XCONV (forward, multiply, inverse in one column pass, as the slab convolve plan's X pass;
+// fft_conv_shared_kernel when one multiplier serves every image / volume), then the forward passes before it again, inverse and
+// in reverse order:
+//   3-D C2C, plane kernel: XY_PLANE in -> out, XCONV, inverse XY_PLANE (6 volume sweeps + the multiplier)
+//   3-D C2C, other shapes: X in -> out, Y, XCONV, inverse Y, inverse X (10 sweeps)
+//   3-D R2C:               Z_R2C in -> temp, Y, XCONV, inverse Y, Z_C2R temp -> out
+//   2-D C2C, plane conv:   XY_PLANE_CONV in -> out: the whole convolution of nx == ny images in one launch of e->plane_conv
+//                          (plane_conv_default; DFFT_FORCE_PLANE=1: wherever instantiated; DFFT_NO_PLANE=1: never) (2 sweeps)
+//   2-D C2C, other shapes: X in -> out, XCONV, inverse X (6 sweeps)
+//   2-D R2C:               Z_R2C in -> temp, XCONV, Z_C2R temp -> out
 // Everything after the first pass is in place in `out` (C2C) or the plan's temporary (R2C), so `in` is only read and in == out
-// works.  The Z length needs the convolve kernel: a tuned default entry (launch[PK_XCONV], as dfft_plan_convolve_* asks of x)
-static int make_lines_conv_3d(dfft_lines_plan p, int nx, int ny, int nz, long long batch, int precision, bool real, unsigned flags, bool dry)
+// works.  The convolved length (ny in 2-D, nz in 3-D) needs the convolve kernel: a tuned default entry (launch[PK_XCONV], as
+// dfft_plan_convolve_* asks of x)
+static int make_lines_conv(dfft_lines_plan p, int dims, int nx, int ny, int nz, long long batch, int precision, bool real, unsigned flags, bool dry)
 {
     if (flags & ~DFFT_SCALE_BACKWARD) return fail(DFFT_EINVAL, "convolve lines plans take no flag but DFFT_SCALE_BACKWARD");
-    int rc = real ? make_real_lines(p, nx, ny, nz, batch, precision, 3, dry) : make_lines_3d(p, nx, ny, nz, batch, precision, dry);
+    const int nc = dims == 3 ? nz : ny;   // the convolved axis
+    int rc;
+    if (real) {
+        rc = make_real_lines(p, nx, ny, nz, batch, precision, dims, dry);
+    } else if (dims == 3) {
+        rc = make_lines_3d(p, nx, ny, nz, batch, precision, dry);
+    } else {
+        if (nx < 1 || ny < 1 || batch < 0 || (precision != DFFT_DOUBLE && precision != DFFT_FLOAT)) return fail(DFFT_EINVAL, "bad arguments");
+        if (!fits_int(ny, batch)) return fail(DFFT_EUNSUPPORTED, "%d x %lld rows: at most 2^31 - 1 per plan", ny, batch);
+        rc = make_lines_2d(p, nx, ny, batch, precision, dry);
+    }
     if (rc) return rc;
-    LinePass* f = real ? p->rpass[0] : p->pass;   // forward passes in execution order, Z last
+    LinePass* f = real ? p->rpass[0] : p->pass;   // forward passes in execution order, the convolved axis last
     const int nf = real ? p->nreal : p->npass;
     const LinePass& z = f[nf - 1];
     if (z.kind != PK_Y || z.e->gen || !z.e->launch[PK_XCONV])
-        return fail(DFFT_EUNSUPPORTED, "the z length %d has no convolution kernel (it needs a tuned length, dfft_length_kind == 2, of the default kernel table)", nz);
+        return fail(DFFT_EUNSUPPORTED, "the %c length %d has no convolution kernel (it needs a tuned length, dfft_length_kind == 2, of the default kernel table)",
+                    dims == 3 ? 'z' : 'y', nc);
     const int buf = real ? LB_TEMP : LB_OUT;
     int k = 0;
     for (int j = 0; j < nf; j++) {
@@ -2791,6 +2814,15 @@ static int make_lines_conv_3d(dfft_lines_plan p, int nx, int ny, int nz, long lo
         lp.src = lp.dst = buf; lp.inv = true;
     }
     if (real) p->cpass[k++] = p->rpass[1][nf - 1];   // Z_C2R temp -> out
+    const SizeEntry* ex = f[0].e;
+    if (dims == 2 && !real && nx == ny && ex->plane_conv && !env_on("DFFT_NO_PLANE") && (plane_conv_default(nx, precision) || env_on("DFFT_FORCE_PLANE"))) {
+        // the three passes become one: the X pass's contiguous twiddle table serves both roles (one Sched at these lengths)
+        LinePass& lp = p->cpass[0];
+        lp.plane = true; lp.kind = PK_XCONV; lp.ntiles = batch;
+        lp.ia = lp.oa = Affine{(long long)nx * ny, 0, nx, 1};   // for the records: image, row and point strides
+        for (int j = 1; j < k; j++) p->cpass[j] = LinePass{};
+        k = 1;
+    }
     p->nconv = k;
     // the builders' passes the schedule does not use give back their twiddle tables
     auto used = [&](void* t) { for (int j = 0; j < k; j++) if (p->cpass[j].lut == t) return true; return false; };
@@ -2801,22 +2833,22 @@ static int make_lines_conv_3d(dfft_lines_plan p, int nx, int ny, int nz, long lo
     p->conv = true;
     p->real = real;
     p->batch = batch;
-    const long long vol = (long long)nx * ny * nz;
-    p->mvol = real ? (long long)nz * ny * (nx / 2 + 1) : vol;
+    const long long vol = (long long)nx * ny * (dims == 3 ? nz : 1);
+    p->mvol = real ? vol / nx * (nx / 2 + 1) : vol;
     if (real) p->rcount = vol * batch;
     else p->ccount = vol * batch;
     p->scale = (flags & DFFT_SCALE_BACKWARD) ? 1.0 / (double)vol : 0.0;
     return 0;
 }
 
-static int conv_plan_create(int nx, int ny, int nz, long long batch, int precision, bool real, unsigned flags, dfft_lines_plan* out)
+static int conv_plan_create(int dims, int nx, int ny, int nz, long long batch, int precision, bool real, unsigned flags, dfft_lines_plan* out)
 {
     if (!out) return fail(DFFT_EINVAL, "null plan pointer");
     *out = nullptr;
     if (precision != DFFT_DOUBLE && precision != DFFT_FLOAT) return fail(DFFT_EINVAL, "bad arguments");
     dfft_lines_plan p = new dfft_lines_plan_s;
     int rc = lines_plan_common(p, precision);
-    if (!rc) rc = make_lines_conv_3d(p, nx, ny, nz, batch, precision, real, flags, false);
+    if (!rc) rc = make_lines_conv(p, dims, nx, ny, nz, batch, precision, real, flags, false);
     if (rc) { dfft_lines_destroy(p); return rc; }
     *out = p;
     return 0;
@@ -2824,12 +2856,22 @@ static int conv_plan_create(int nx, int ny, int nz, long long batch, int precisi
 
 extern "C" int dfft_lines_plan_create_convolve_3d(int nx, int ny, int nz, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
 {
-    return conv_plan_create(nx, ny, nz, batch, precision, false, flags, plan);
+    return conv_plan_create(3, nx, ny, nz, batch, precision, false, flags, plan);
 }
 
 extern "C" int dfft_lines_plan_create_convolve_r2c_3d(int nx, int ny, int nz, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
 {
-    return conv_plan_create(nx, ny, nz, batch, precision, true, flags, plan);
+    return conv_plan_create(3, nx, ny, nz, batch, precision, true, flags, plan);
+}
+
+extern "C" int dfft_lines_plan_create_convolve_2d(int nx, int ny, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
+{
+    return conv_plan_create(2, nx, ny, 1, batch, precision, false, flags, plan);
+}
+
+extern "C" int dfft_lines_plan_create_convolve_r2c_2d(int nx, int ny, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
+{
+    return conv_plan_create(2, nx, ny, 1, batch, precision, true, flags, plan);
 }
 
 // pass k of a convolve lines plan: launched on the plan's stream, or (ops) only recorded, phase = k
@@ -2842,6 +2884,18 @@ static cudaError_t conv_line_pass(const dfft_lines_plan_s* p, int k, const void*
     RealZArgs<T> r{};
     real_line_args<T>(lp, line_buf(lp.src, in, out, p->temp), line_buf(lp.dst, in, out, p->temp), lp.inv ? DFFT_BACKWARD : DFFT_FORWARD, r);
     const bool realk = lp.kind == PK_Z_R2C || lp.kind == PK_Z_C2R;
+    if (lp.plane && lp.kind == PK_XCONV) {
+        const long long n = lp.e->N;
+        const PlaneConvArgs<T> pc{{r.t.in, r.t.out, r.t.lut, lp.ntiles, 0}, (const cx<T>*)mult, shared ? 0 : n * n, (T)p->scale, p->scale != 0 ? 1 : 0};
+        if (ops) {
+            r.t.do_scale = pc.do_scale; r.t.scale = pc.scale;
+            char extra[128];
+            snprintf(extra, sizeof(extra), ", \"mult\": %llu, \"shared\": %d", (unsigned long long)(size_t)mult, shared ? 1 : 0);
+            record_op<T>(*ops, "XY_PLANE_CONV", k, lp.e->N, lp.e->N, false, false, false, r.t, extra);
+            return cudaSuccess;
+        }
+        return lp.e->plane_conv(&pc, p->sms, p->stream);
+    }
     if (lp.plane) {
         const PlaneArgs<T> pa{r.t.in, r.t.out, r.t.lut, lp.ntiles, r.t.inv};
         if (ops) record_op<T>(*ops, "XY_PLANE", k, lp.e->N, lp.e->N, false, false, false, r.t);
@@ -2880,7 +2934,7 @@ template <typename T> static int lines_execute_conv_impl(dfft_lines_plan p, cons
 extern "C" int dfft_lines_execute_convolve(dfft_lines_plan p, const void* in, void* out, const void* mult, long long mult_count)
 {
     if (!p || !in || !out || !mult) return fail(DFFT_EINVAL, "bad arguments");
-    if (!p->conv) return fail(DFFT_EINVAL, "dfft_lines_execute_convolve needs a plan from dfft_lines_plan_create_convolve_3d / _r2c_3d");
+    if (!p->conv) return fail(DFFT_EINVAL, "dfft_lines_execute_convolve needs a plan from dfft_lines_plan_create_convolve_[r2c_]2d / _3d");
     if (mult_count != 1 && mult_count != p->batch) return fail(DFFT_EINVAL, "mult_count must be 1 or the plan's batch (%lld), not %lld", p->batch, mult_count);
     const size_t rsz = p->prec == DFFT_FLOAT ? 4 : 8, csz = 2 * rsz, esz = p->real ? rsz : csz;
     const uintptr_t a = (uintptr_t)in, b = (uintptr_t)out, m = (uintptr_t)mult;
@@ -2893,6 +2947,16 @@ extern "C" int dfft_lines_execute_convolve(dfft_lines_plan p, const void* in, vo
     return p->prec == DFFT_DOUBLE ? lines_execute_conv_impl<double>(p, in, out, mult, shared) : lines_execute_conv_impl<float>(p, in, out, mult, shared);
 }
 
+// the records of a dry convolve lines plan's passes (in = buffer 5, out = 2, temporary = 4, multiplier = 8), through conv_line_pass
+static long long conv_ops_json(dfft_lines_plan_s& lp, long long batch, long long mult_count, char* buf, long long cap)
+{
+    if (mult_count != 1 && mult_count != batch) return fail(DFFT_EINVAL, "mult_count must be 1 or the plan's batch");
+    std::vector<std::string> ops;
+    for (int k = 0; k < lp.nconv; k++) conv_line_pass<double>(&lp, k, fake_addr(0, 5), fake_addr(0, 2), fake_addr(0, 8), mult_count == 1, &ops);
+    lp.temp = nullptr;
+    return ops_json(ops, buf, cap);
+}
+
 /* test hook (host only): the passes of a convolve lines plan, JSON as dfft_debug_lines_3d_ops; in = buffer 5, out = 2,
  * temporary = 4, multiplier = 8 of device 0.  XCONV carries "mult" and "shared" (1: mult_count == 1) */
 extern "C" long long dfft_debug_lines_conv_3d_ops(int nx, int ny, int nz, long long batch, int precision, int real, unsigned flags,
@@ -2900,13 +2964,21 @@ extern "C" long long dfft_debug_lines_conv_3d_ops(int nx, int ny, int nz, long l
 {
     dfft_lines_plan_s lp;
     lp.prec = precision;
-    const int rc = make_lines_conv_3d(&lp, nx, ny, nz, batch, precision, real != 0, flags, true);
+    const int rc = make_lines_conv(&lp, 3, nx, ny, nz, batch, precision, real != 0, flags, true);
     if (rc) return rc;
-    if (mult_count != 1 && mult_count != batch) return fail(DFFT_EINVAL, "mult_count must be 1 or the plan's batch");
-    std::vector<std::string> ops;
-    for (int k = 0; k < lp.nconv; k++) conv_line_pass<double>(&lp, k, fake_addr(0, 5), fake_addr(0, 2), fake_addr(0, 8), mult_count == 1, &ops);
-    lp.temp = nullptr;
-    return ops_json(ops, buf, cap);
+    return conv_ops_json(lp, batch, mult_count, buf, cap);
+}
+
+/* test hook (host only): the passes of a 2-D convolve lines plan, JSON as dfft_debug_lines_conv_3d_ops.  The plane-convolve
+ * kernel's record is "XY_PLANE_CONV" with ntiles = images, ia = oa = [image, 0, row, point] strides, "mult" and "shared" */
+extern "C" long long dfft_debug_lines_conv_2d_ops(int nx, int ny, long long batch, int precision, int real, unsigned flags,
+                                                  long long mult_count, char* buf, long long cap)
+{
+    dfft_lines_plan_s lp;
+    lp.prec = precision;
+    const int rc = make_lines_conv(&lp, 2, nx, ny, 1, batch, precision, real != 0, flags, true);
+    if (rc) return rc;
+    return conv_ops_json(lp, batch, mult_count, buf, cap);
 }
 
 extern "C" int dfft_fft_lines(void* data, int n, long long stride, long long nlines, long long inner, long long inner_dist,

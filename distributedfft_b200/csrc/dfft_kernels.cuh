@@ -62,10 +62,14 @@ struct SizeEntry {
     const void* gen;      // run-time schedule (GenSched) of a generic-length entry, nullptr for tuned lengths
     PlaneLaunchFn plane;  // valid for square planes: the contiguous (X) and strided (Y) passes of whole N x N planes in one kernel;
                           // default entries of N = 16, 32, 64 only (both roles share one schedule there), else nullptr
+    PlaneLaunchFn plane_conv;   // set where `plane` is: the 2-D convolution of whole N x N images in one kernel
+                                // (fft_plane_conv_kernel, args = PlaneConvArgs<T>), else nullptr
 };
 
 // whether fft_plane_kernel is the default for (N, prec) (measured against the two separate passes, dfft_kernels_common.cu)
 bool plane_default(int N, int prec);
+// whether fft_plane_conv_kernel is the default of the 2-D convolve lines plans for (N, prec) (measured against the three passes)
+bool plane_conv_default(int N, int prec);
 
 // TMA-pipelined pass kernels (fft_tma.cuh), instantiated for the lengths whose C-line tile fills a 64 KB ring slot
 typedef cudaError_t (*TmaLaunchFn)(int mode, const void* tma_args, const void* map_in, const void* map_out, int sm_count, cudaStream_t stream);

@@ -46,6 +46,19 @@ bool plane_default(int N, int prec)
     return false;
 }
 
+// fft_plane_conv_kernel against the three passes X, XCONV, inverse X, per (N, precision), from
+// csrc/tools/lines_conv_bench.py --dims 2 on H100 (DESIGN.md section 7): true = the default of the 2-D convolve lines plans
+static const struct { int N, prec; bool use; } kPlaneConvUse[] = {
+    {16, 0, true}, {32, 0, true}, {64, 0, true}, {16, 1, true}, {32, 1, true}, {64, 1, true},
+};
+
+bool plane_conv_default(int N, int prec)
+{
+    for (const auto& u : kPlaneConvUse)
+        if (u.N == N && u.prec == prec) return u.use;
+    return false;
+}
+
 void list_sizes(int prec, std::vector<int>& out)
 {
     out.clear();

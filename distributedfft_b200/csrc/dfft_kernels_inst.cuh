@@ -133,6 +133,34 @@ cudaError_t launch_plane(const void* vargs, int sm_count, cudaStream_t st)
     return cudaGetLastError();
 }
 
+// 2-D convolution of whole square images (fft_plane_conv_kernel): vargs is a PlaneConvArgs<T>; P images per CTA
+template <class S, typename T, int P, int MINB>
+cudaError_t launch_plane_conv(const void* vargs, int sm_count, cudaStream_t st)
+{
+    const PlaneConvArgs<T>& a = *reinterpret_cast<const PlaneConvArgs<T>*>(vargs);
+    auto kern = fft_plane_conv_kernel<S, T, P, MINB>;
+    constexpr size_t smem = PlaneSmem<S, T, P>::bytes;
+    static std::atomic<int> occ_cache[64];
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    int occ = occ_cache[dev & 63].load();
+    if (occ == 0) {
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, S::T * S::N * P, smem);
+        if (e != cudaSuccess) return e;
+        if (occ < 1) return cudaErrorLaunchOutOfResources;
+        occ_cache[dev & 63].store(occ);
+    }
+    const long long groups = (a.p.planes + P - 1) / P;
+    if (groups <= 0) return cudaSuccess;
+    long long grid = (long long)sm_count * occ;
+    if (grid > groups) grid = groups;
+    kern<<<(unsigned)grid, S::T * S::N * P, smem, st>>>(a);
+    return cudaGetLastError();
+}
+
 template <class OpA, class OpB, typename T, int MINB>
 cudaError_t launch_fused(const void* va, const void* vb, const FusedCtl* ctl, int sm_count, cudaStream_t st)
 {
@@ -308,6 +336,8 @@ SizeEntry make_entry(int variant = 0)
             constexpr int P = plane_group<ZS>();
             constexpr int MBP = (sizeof(T) == 8 && ZS::N == 32) ? 3 : 1024 / (ZS::T * ZS::N * P);
             e.plane = launch_plane<ZS, T, P, MBP>;
+            // the 2-D convolution of whole images: the plane kernel's CTA shape and register budget
+            e.plane_conv = launch_plane_conv<ZS, T, P, MBP>;
         }
     }
     // fused two-pass kernels: the contiguous role is re-tiled so that both roles fill the same CTA

@@ -107,4 +107,89 @@ __global__ void __launch_bounds__(S::T* S::N* P, MINB) fft_plane_kernel(const Pl
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// fft_plane_conv_kernel -- a whole 2-D spectral convolution of small square images in ONE sweep: out = ifft2(fft2(in) * m)
+// per image, unnormalised (x N*N) unless do_scale.  The CTA shape, thread maps and shared memory are fft_plane_kernel's; per
+// group of P images:
+//   X role forward  : rows (MAP_T) from global memory, contiguous schedule, column-line copy in shared memory
+//   Y role forward  : columns (MAP_C) from the copy, strided schedule; thread (tc, cc) now holds y = tc + u*TT of column xc,
+//                     its own load and store positions
+//   multiply        : conv_tiles' expression, v = cswap(cmul(v, m)) (the inverse's swap-in folded into the product)
+//   Y role inverse  : MAP_C, strided schedule (StageRunner's barrier before its first scatter frees the buffer)
+//   X role inverse  : row-line copy, MAP_T, contiguous schedule, cswap on the store to the rows.  The XCONV pass's store swap
+//                     and the inverse X pass's load swap of the separate passes cancel and are left out
+// Bit-identical to the three passes X, XCONV along y, inverse X (DFFT_NO_PLANE=1): the same schedules and twiddle values (one
+// Sched for both roles at the instantiated lengths), the same butterflies per line, the same multiply.  Every element of a
+// group is in registers before any of it is stored (in place is safe); images past the batch load, read and store nothing.
+// ------------------------------------------------------------------------------------------
+template <typename T> struct PlaneConvArgs {
+    PlaneArgs<T> p;        // p.planes = images; p.inv unused
+    const cx<T>* mult;     // [images or 1][N][N], natural order
+    long long mult_plane;  // multiplier elements between images: 0 (one multiplier for every image) or N*N
+    T scale;               // folded into the multiplier when do_scale
+    int do_scale;
+};
+
+template <class S, typename T, int P, int MINB>
+__global__ void __launch_bounds__(S::T* S::N* P, MINB) fft_plane_conv_kernel(const PlaneConvArgs<T> R)
+{
+    static_assert(S::valid() && S::NSTAGES > 1, "bad schedule");
+    using SM = PlaneSmem<S, T, P>;
+    constexpr int N = S::N, RR = S::R, TT = S::T, C = SM::C, LS = SM::LS;
+    constexpr long long NN = (long long)N * N;
+    const PlaneArgs<T>& A = R.p;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    cx<T>* buf = reinterpret_cast<cx<T>*>(smem_raw);
+    cx<T>* lut_s = reinterpret_cast<cx<T>*>(smem_raw + SM::buf_bytes);
+    uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw + SM::buf_bytes + SM::lut_bytes);
+    stage_twiddles_tma<T>(lut_s, A.lut, S::lut_size(), bar);
+
+    const int tid = threadIdx.x;
+    int tr, cr, tc, cc;   // row role: thread tr of line cr (MAP_T); column role: thread tc of column cc (MAP_C)
+    thread_map<MAP_T, C, TT>(tid, tr, cr);
+    thread_map<MAP_C, C, TT>(tid, tc, cc);
+    const int pr = cr / N, yr = cr % N;   // row role: image of the group and row y
+    const int pc = cc / N, xc = cc % N;   // column role: image of the group and column x
+    const bool do_scale = R.do_scale != 0;
+    const long long groups = (A.planes + P - 1) / P;
+    cx<T> twr[1];
+    int pp = 0;
+    for (long long g = blockIdx.x; g < groups; g += gridDim.x) {
+        const long long p0 = g * P;
+        const bool okr = p0 + pr < A.planes, okc = p0 + pc < A.planes;
+        cx<T> v[RR];
+        const cx<T>* src = A.in + (p0 + pr) * NN + (long long)yr * N + tr;
+#pragma unroll
+        for (int u = 0; u < RR; u++) v[u] = okr ? ld_stream(src + u * TT) : mk<T>(0, 0);
+        StageRunner<S, 0, T, C, MAP_T, MAP_T, false, false>::run(v, tr, cr, tr, cr, buf, pp, lut_s, twr, [] {});
+        __syncthreads();   // every thread's last gather is done: the exchange buffer becomes the image copy
+        // point x = tr + u*TT of row yr -> column line (pr, x), position yr
+#pragma unroll
+        for (int u = 0; u < RR; u++) buf[(pr * N + tr + u * TT) * LS + SmemGeom<T>::pad(yr)] = v[u];
+        __syncthreads();
+        stage_gather<S, T>(v, tc, buf + cc * LS);
+        StageRunner<S, 0, T, C, MAP_C, MAP_C, false, false>::run(v, tc, cc, tc, cc, buf, pp, lut_s, twr, [] {});
+        const cx<T>* mp = R.mult + (p0 + pc) * R.mult_plane + (long long)tc * N + xc;
+#pragma unroll
+        for (int u = 0; u < RR; u++) {
+            cx<T> m = okc ? ld_stream(mp + (long long)u * TT * N) : mk<T>(0, 0);
+            if (do_scale) { m.x *= R.scale; m.y *= R.scale; }
+            v[u] = cswap(cmul(v[u], m));
+        }
+        StageRunner<S, 0, T, C, MAP_C, MAP_C, false, false>::run(v, tc, cc, tc, cc, buf, pp, lut_s, twr, [] {});
+        __syncthreads();
+        // point y = tc + u*TT of column xc -> row line (pc, y), position xc
+#pragma unroll
+        for (int u = 0; u < RR; u++) buf[(pc * N + tc + u * TT) * LS + SmemGeom<T>::pad(xc)] = v[u];
+        __syncthreads();
+        stage_gather<S, T>(v, tr, buf + cr * LS);
+        StageRunner<S, 0, T, C, MAP_T, MAP_T, false, false>::run(v, tr, cr, tr, cr, buf, pp, lut_s, twr, [] {});
+        if (okr) {
+            cx<T>* dst = A.out + (p0 + pr) * NN + (long long)yr * N + tr;
+#pragma unroll
+            for (int u = 0; u < RR; u++) st_stream(dst + u * TT, cswap(v[u]));
+        }
+    }
+}
+
 }  // namespace dfft

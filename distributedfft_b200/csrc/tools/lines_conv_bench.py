@@ -1,24 +1,31 @@
 #!/usr/bin/env python
-"""Batched 3-D spectral convolution: the convolve lines plan against the three calls it replaces, one GPU (developer tool).
+"""Batched 3-D (or, with --dims 2, 2-D) spectral convolution: the convolve lines plan against the three calls it replaces, one
+GPU (developer tool).
 
-    python distributedfft_b200/csrc/tools/lines_conv_bench.py [--steps 30] [--rounds 3] [--warmup 5] [--case NAME]
+    python distributedfft_b200/csrc/tools/lines_conv_bench.py [--dims 3|2] [--steps 30] [--rounds 3] [--warmup 5] [--case NAME]
 
-Every case convolves `batch` volumes with one multiplier of unit modulus / N (so repeated in-place steps keep their magnitude).
-Four arms get the same seeded data:
+Every case convolves `batch` volumes (images) with one multiplier of unit modulus / N (so repeated in-place steps keep their
+magnitude).  The arms get the same seeded data:
   shared   LinesConvolvePlan, one multiplier for every volume (mult_count = 1), out of place
   pervol   the same plan with `batch` identical copies of the multiplier (mult_count = batch)
-  3call    LinesPlan(three_d=...) forward in place, torch multiply by the shared multiplier, LinesPlan backward
+  noplane  (--dims 2, square 16 / 32 / 64 images) the plan created under DFFT_NO_PLANE=1 (X, XCONV, inverse X), shared
+           multiplier; the shared and pervol plans are then created under DFFT_FORCE_PLANE=1, so that the one-kernel
+           convolution is timed whatever kPlaneConvUse says
+  3call    LinesPlan(three_d=... / two_d=...) forward in place, torch multiply by the shared multiplier, LinesPlan backward
            (real: RealLinesPlan forward into a spectrum buffer, multiply, backward into the output)
   torch    torch.fft.fftn * m -> ifftn (rfftn / irfftn for real cases; cuFFT, for context)
-Before timing, the outputs of all four are compared: shared and pervol with np.array_equal, 3call and torch by rel_l2 against
-shared.  Each round times `steps` executes of each arm with CUDA events on the arm's own stream (the plans' streams; torch's
-current stream for torch), arms alternating, after `warmup` untimed executes.
+Before timing, the outputs of all arms are compared: shared against pervol and noplane with torch.equal (bit-identical by
+construction), 3call and torch by rel_l2 against shared.  Each round times `steps` executes of each arm with CUDA events on the
+arm's own stream (the plans' streams; torch's current stream for torch), arms alternating, after `warmup` untimed executes.
 
 Prints one JSON object per case and a summary table: ms per step (median of the rounds), conv / 3call, and the HBM sweep model
 of each arm in bytes with its GB/s at the measured time (V = one sweep of the batch, M = the multiplier as read):
-  C2C plane shape  conv 6V + M      3call 10V + M
-  C2C other        conv 10V + M     3call 14V + M
-  real             conv 2Vr + 8Vc + M   3call 2Vr + 12Vc + M   (Vr: real data, Vc: the half spectra)
+  3-D C2C plane shape  conv 6V + M      3call 10V + M
+  3-D C2C other        conv 10V + M     3call 14V + M
+  3-D real             conv 2Vr + 8Vc + M   3call 2Vr + 12Vc + M   (Vr: real data, Vc: the half spectra)
+  2-D C2C plane shape  conv 2V + M      noplane 6V + M    3call 10V + M
+  2-D C2C other        conv 6V + M      3call 10V + M
+  2-D real             conv 2Vr + 4Vc + M   3call 2Vr + 8Vc + M
 Card name, power limit and SM clock (nvidia-smi, read-only query) are printed before and after."""
 import argparse
 import json
@@ -37,6 +44,16 @@ CASES = [
     ("16^3x16384-f32", "f", (16, 16, 16, 16384), False), ("32^3x2048-f32", "f", (32, 32, 32, 2048), False),
     ("64^3x256-f32", "f", (64, 64, 64, 256), False),
     ("real-64^3x256", "d", (64, 64, 64, 256), True),
+]
+# --dims 2: (nx, ny, batch), about 2^26 complex elements per batch.  48^2 has no plane kernel
+CASES_2D = [
+    ("16^2x262144", "d", (16, 16, 262144), False), ("32^2x65536", "d", (32, 32, 65536), False),
+    ("64^2x16384", "d", (64, 64, 16384), False),
+    ("16^2x262144-f32", "f", (16, 16, 262144), False), ("32^2x65536-f32", "f", (32, 32, 65536), False),
+    ("64^2x16384-f32", "f", (64, 64, 16384), False),
+    ("48^2x16384", "d", (48, 48, 16384), False), ("256^2x1024", "d", (256, 256, 1024), False),
+    ("1024^2x64", "d", (1024, 1024, 64), False),
+    ("real-64^2x16384", "d", (64, 64, 16384), True), ("real-512^2x256", "d", (512, 512, 256), True),
 ]
 
 
@@ -62,28 +79,45 @@ def time_steps(torch, stream, fn, steps):
     return a.elapsed_time(b) / steps
 
 
+def make_conv(dfft, key, shape, prec, real, env):
+    """LinesConvolvePlan with `env` (DFFT_NO_PLANE / DFFT_FORCE_PLANE) set at creation only"""
+    if env:
+        os.environ[env] = "1"
+    try:
+        return dfft.LinesConvolvePlan(**{key: shape}, precision=prec, real=real)
+    finally:
+        if env:
+            os.environ.pop(env)
+
+
 def run_case(torch, np, dfft, case, args):
     name, p, shape, real = case
-    nx, ny, nz, batch = shape
+    two = len(shape) == 3
+    nx, batch = shape[0], shape[-1]
+    spatial = tuple(reversed(shape[:-1]))                                             # (nz, ny, nx) or (ny, nx)
+    key = "two_d" if two else "three_d"
     prec = dfft.FLOAT if p == "f" else dfft.DOUBLE
     rdt, cdt = (torch.float32, torch.complex64) if p == "f" else (torch.float64, torch.complex128)
     er = 4 if p == "f" else 8
     ec = 2 * er
     H = nx // 2 + 1
-    N = nx * ny * nz
+    N = int(np.prod(spatial))
     mx = H if real else nx
-    dims = (-3, -2, -1)
+    mshape = spatial[:-1] + (mx,)
+    dims = tuple(range(-len(spatial), 0))
     gen = torch.Generator(device="cuda").manual_seed(7)
-    x = torch.randn((batch, nz, ny, nx), dtype=rdt if real else cdt, device="cuda", generator=gen)
-    phase = torch.rand((nz, ny, mx), dtype=rdt, device="cuda", generator=gen) * (2 * np.pi)
+    x = torch.randn((batch,) + spatial, dtype=rdt if real else cdt, device="cuda", generator=gen)
+    phase = torch.rand(mshape, dtype=rdt, device="cuda", generator=gen) * (2 * np.pi)
     m1 = (torch.polar(torch.ones_like(phase), phase) / N).to(cdt).contiguous()
-    mb = m1.expand(batch, nz, ny, mx).contiguous()
-    conv = dfft.LinesConvolvePlan(shape, precision=prec, real=real)
-    fwd = dfft.RealLinesPlan(three_d=shape, precision=prec) if real else dfft.LinesPlan(three_d=shape, precision=prec)
+    mb = m1.expand((batch,) + mshape).contiguous()
+    plane_shape = two and not real and shape[0] == shape[1] and shape[0] in (16, 32, 64)
+    conv = make_conv(dfft, key, shape, prec, real, "DFFT_FORCE_PLANE" if plane_shape else None)
+    noplane = make_conv(dfft, key, shape, prec, real, "DFFT_NO_PLANE") if plane_shape else None
+    fwd = dfft.RealLinesPlan(**{key: shape}, precision=prec) if real else dfft.LinesPlan(**{key: shape}, precision=prec)
     try:
-        y = {k: torch.empty_like(x) for k in ("shared", "pervol")}
+        y = {k: torch.empty_like(x) for k in ("shared", "pervol") + (("noplane",) if noplane else ())}
         z = x.clone()                                                                 # the three-call arm's buffer
-        spec = torch.empty((batch, nz, ny, H), dtype=cdt, device="cuda") if real else None
+        spec = torch.empty((batch,) + spatial[:-1] + (H,), dtype=cdt, device="cuda") if real else None
         zout = torch.empty_like(x) if real else z
 
         def three_calls():
@@ -98,20 +132,24 @@ def run_case(torch, np, dfft, case, args):
 
         def torch_arm():
             if real:
-                return torch.fft.irfftn(torch.fft.rfftn(x, dim=dims) * m1, s=(nz, ny, nx), dim=dims)
+                return torch.fft.irfftn(torch.fft.rfftn(x, dim=dims) * m1, s=spatial, dim=dims)
             return torch.fft.ifftn(torch.fft.fftn(x, dim=dims) * m1, dim=dims)
 
         jobs = {
             "shared": (conv.stream, lambda: conv.execute(x.data_ptr(), y["shared"].data_ptr(), m1.data_ptr(), 1)),
             "pervol": (conv.stream, lambda: conv.execute(x.data_ptr(), y["pervol"].data_ptr(), mb.data_ptr(), batch)),
-            "3call": (fwd.stream, three_calls),
-            "torch": (None, torch_arm),
         }
+        if noplane:
+            jobs["noplane"] = (noplane.stream, lambda: noplane.execute(x.data_ptr(), y["noplane"].data_ptr(), m1.data_ptr(), 1))
+        jobs["3call"] = (fwd.stream, three_calls)
+        jobs["torch"] = (None, torch_arm)
         # cross-check before timing: one step of every arm from the same input
         torch.cuda.synchronize()
-        for k in ("shared", "pervol"):
+        for k in y:
             jobs[k][1]()
         conv.synchronize()
+        if noplane:
+            noplane.synchronize()
         with torch.cuda.stream(torch.cuda.ExternalStream(fwd.stream)):
             three_calls()
         fwd.synchronize()
@@ -122,6 +160,8 @@ def run_case(torch, np, dfft, case, args):
         def rel(a):
             return float(torch.linalg.vector_norm(a - ref) / torch.linalg.vector_norm(ref))
         check = {"shared_eq_pervol": bool(torch.equal(y["shared"], y["pervol"])), "rel_l2_3call": rel(zout), "rel_l2_torch": rel(t_out)}
+        if noplane:
+            check["shared_eq_noplane"] = bool(torch.equal(y["shared"], y["noplane"]))
         del t_out
         for st, fn in jobs.values():
             with torch.cuda.stream(torch.cuda.ExternalStream(st) if st is not None else torch.cuda.current_stream()):
@@ -135,22 +175,35 @@ def run_case(torch, np, dfft, case, args):
     finally:
         conv.destroy()
         fwd.destroy()
+        if noplane:
+            noplane.destroy()
     med = {k: float(np.median([r[k] for r in rounds])) for k in rounds[0]}
-    plane = dfft.lines_conv_3d_ops(nx, ny, nz, batch, prec, real)[0]["op"] == "XY_PLANE"
-    Msh, Mpv = ec * nz * ny * mx, ec * nz * ny * mx * batch
+    if two:
+        plane = plane_shape
+    else:
+        plane = dfft.lines_conv_3d_ops(*shape, prec, real)[0]["op"] == "XY_PLANE"
+    Mimg = ec * N // nx * mx
+    Msh, Mpv = Mimg, Mimg * batch
     if real:
-        Vr, Vc = er * N * batch, ec * nz * ny * H * batch
-        conv_b, call_b = 2 * Vr + 8 * Vc, 2 * Vr + 12 * Vc
-        model = "conv 2Vr+8Vc+M, 3call 2Vr+12Vc+M"
+        Vr, Vc = er * N * batch, ec * N // nx * H * batch
+        conv_b, call_b = (2 * Vr + 4 * Vc, 2 * Vr + 8 * Vc) if two else (2 * Vr + 8 * Vc, 2 * Vr + 12 * Vc)
+        model = "conv 2Vr+4Vc+M, 3call 2Vr+8Vc+M" if two else "conv 2Vr+8Vc+M, 3call 2Vr+12Vc+M"
     else:
         V = ec * N * batch
-        conv_b, call_b = (6 * V, 10 * V) if plane else (10 * V, 14 * V)
-        model = "conv 6V+M, 3call 10V+M" if plane else "conv 10V+M, 3call 14V+M"
+        if two:
+            conv_b, call_b = (2 * V if plane else 6 * V), 10 * V
+            model = "conv 2V+M, noplane 6V+M, 3call 10V+M" if plane else "conv 6V+M, 3call 10V+M"
+        else:
+            conv_b, call_b = (6 * V, 10 * V) if plane else (10 * V, 14 * V)
+            model = "conv 6V+M, 3call 10V+M" if plane else "conv 10V+M, 3call 14V+M"
     model_bytes = {"shared": conv_b + Msh, "pervol": conv_b + Mpv, "3call": call_b + Msh}
+    if noplane:
+        model_bytes["noplane"] = 6 * V + Msh
     res = {
         "case": name, "precision": "float" if p == "f" else "double", "shape": list(shape), "real": real, "plane_kernel": plane,
         "steps": args.steps, "rounds": rounds, "median_ms": med,
         "ratio_shared_vs_3call": med["shared"] / med["3call"], "ratio_pervol_vs_3call": med["pervol"] / med["3call"],
+        "ratio_shared_vs_noplane": med["shared"] / med["noplane"] if noplane else None,
         "sweep_model": model, "model_bytes": model_bytes,
         "model_gbps": {k: b / med[k] / 1e6 for k, b in model_bytes.items()}, "cross_check": check,
     }
@@ -164,6 +217,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--case", action="append", help="run only these cases (default: all)")
+    ap.add_argument("--dims", type=int, choices=(2, 3), default=3, help="3-D volumes (default) or 2-D images")
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -174,7 +228,7 @@ def main():
         os.environ.pop(var, None)
     print(json.dumps({"gpu_before": gpu_state()}), flush=True)
     results = []
-    for case in CASES:
+    for case in (CASES_2D if args.dims == 2 else CASES):
         if args.case and case[0] not in args.case:
             continue
         r = run_case(torch, np, dfft, case, args)
@@ -189,6 +243,9 @@ def main():
             r["case"], "on" if r["plane_kernel"] else "off", m["shared"], m["pervol"], m["3call"], m["torch"],
             r["ratio_shared_vs_3call"], r["ratio_pervol_vs_3call"], g["shared"], g["pervol"], g["3call"],
             c["shared_eq_pervol"], c["rel_l2_3call"], c["rel_l2_torch"]))
+        if "noplane" in m:
+            print("%-16s noplane %9.3f ms  GB/s %7.0f  shared/noplane %6.3f  eq=%s" % (
+                r["case"], m["noplane"], g["noplane"], r["ratio_shared_vs_noplane"], c["shared_eq_noplane"]))
 
 
 if __name__ == "__main__":

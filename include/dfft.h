@@ -321,7 +321,24 @@ long long dfft_debug_lines_3d_ops(int nx, int ny, int nz, long long batch, int p
  * Flags: DFFT_SCALE_BACKWARD folds 1/(nx*ny*nz) into the multiply; any other bit is DFFT_EINVAL. */
 int dfft_lines_plan_create_convolve_3d(int nx, int ny, int nz, long long batch, int precision, unsigned flags, dfft_lines_plan* plan);
 int dfft_lines_plan_create_convolve_r2c_3d(int nx, int ny, int nz, long long batch, int precision, unsigned flags, dfft_lines_plan* plan);
-/* mult_count = 1: one multiplier shared by every volume; = batch: one per volume, densely packed.  in == out (in place) or
+/* Batched 2-D spectral convolution on the lines engine: batch row-major ny x nx images (nx fastest),
+ *   C2C: out = ifft2(fft2(in) * m), unnormalised (x nx*ny) unless DFFT_SCALE_BACKWARD;
+ *   R2C: out = irfft2(rfft2(in) * m, s=(ny, nx)) * nx*ny, real in / real out (the imaginary parts the C2R ignores are ignored
+ *        here too, as in the 3-D R2C convolve plan).
+ * m is complex in the plan's precision, natural order: [y][x] (C2C) or [y][nx/2+1] (R2C) per image.  C2C with nx == ny of 16,
+ * 32 or 64 runs the whole convolution in one kernel (X, Y, multiply, inverse Y, inverse X on images held in shared memory: 2
+ * sweeps over the batch + the multiplier) where that kernel is the default for the shape (read at creation; DFFT_NO_PLANE=1
+ * never uses it, DFFT_FORCE_PLANE=1 wherever it is instantiated).  Otherwise 3 launches: X, one column pass that transforms
+ * along y, multiplies and transforms back, inverse X (R2C: the real row pass, the column pass over the nx/2+1 columns, the
+ * inverse real row pass).  The R2C plan owns a temporary of batch*ny*(nx/2+1) complex elements.
+ * Lengths: ny needs a tuned kernel of the default table (dfft_length_kind(ny, precision) == 2; DFFT_GENERIC and DFFT_VARIANT
+ * entries are DFFT_EUNSUPPORTED).  nx: C2C as dfft_lines_plan_create_2d, R2C as dfft_lines_plan_create_r2c_2d.  2^31 or more
+ * rows (ny*batch) are DFFT_EUNSUPPORTED.
+ * Flags: DFFT_SCALE_BACKWARD folds 1/(nx*ny) into the multiply; any other bit is DFFT_EINVAL.  Executed with
+ * dfft_lines_execute_convolve, under the same rules as the 3-D plans. */
+int dfft_lines_plan_create_convolve_2d(int nx, int ny, long long batch, int precision, unsigned flags, dfft_lines_plan* plan);
+int dfft_lines_plan_create_convolve_r2c_2d(int nx, int ny, long long batch, int precision, unsigned flags, dfft_lines_plan* plan);
+/* mult_count = 1: one multiplier shared by every image / volume; = batch: one each, densely packed.  in == out (in place) or
  * disjoint buffers; `in` is never written when they are distinct, `mult` never.  DFFT_EINVAL: a null pointer, a buffer not
  * aligned to its element size (fp32 complex at an 8-byte offset is fine), a partial overlap of in and out, a multiplier that
  * overlaps out, another mult_count, and a plan that is not a convolve lines plan (dfft_lines_execute / dfft_lines_execute_real
@@ -330,6 +347,10 @@ int dfft_lines_execute_convolve(dfft_lines_plan plan, const void* in, void* out,
 /* test hook (host only): the passes of either convolve lines plan, JSON as dfft_debug_lines_3d_ops with in = buffer 5, out = 2,
  * temporary = 4, multiplier = 8; the column pass is "XCONV" with "mult" and "shared" (1 when mult_count == 1) */
 long long dfft_debug_lines_conv_3d_ops(int nx, int ny, int nz, long long batch, int precision, int real, unsigned flags,
+                                       long long mult_count, char* buf, long long cap);
+/* the same for the 2-D convolve lines plans; the one-kernel convolution is one "XY_PLANE_CONV" record with ntiles = images,
+ * ia = oa = [image, 0, row, point] strides, "mult" and "shared" */
+long long dfft_debug_lines_conv_2d_ops(int nx, int ny, long long batch, int precision, int real, unsigned flags,
                                        long long mult_count, char* buf, long long cap);
 /* one-shot convenience (plan + execute + synchronize + destroy), used by the per-axis parity tests */
 int dfft_fft_lines(void* data, int n, long long stride, long long nlines, long long inner, long long inner_dist,
