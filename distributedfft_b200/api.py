@@ -38,7 +38,7 @@ __all__ = [
     "BootstrapComm", "fft_mpi_init", "fft_mpi_plan_dft_c2c_3d", "fft_mpi_execute_dft_3d_c2c", "fft_mpi_destroy_plan",
     "fft_mpi_alloc_local_memory", "fft_mpi_local_size_3d", "fft_mpi_cleanup", "getMaxDataCount", "supported_lengths",
     "fft_mpi_plan_dft_r2c_3d", "local_size_r2c_3d", "fft_mpi_plan_dft_convolve_3d",
-    "fft_lines", "lines_ops", "LinesPlan", "RealLinesPlan", "real_lines_ops", "lines_3d_ops", "LinesConvolvePlan", "lines_conv_3d_ops", "lines_conv_2d_ops", "length_kind", "length_schedule", "memcpy_htod", "memcpy_dtoh", "exchange_table", "comm_allgather",
+    "fft_lines", "lines_ops", "LinesPlan", "RealLinesPlan", "real_lines_ops", "lines_3d_ops", "LinesConvolvePlan", "lines_conv_3d_ops", "lines_conv_2d_ops", "length_kind", "length_schedule", "memcpy_htod", "memcpy_dtoh", "memcpy_dtod", "debug_launch_op", "exchange_table", "comm_allgather",
 ]
 
 
@@ -48,6 +48,18 @@ class DfftError(RuntimeError):
 
 _ALLGATHER = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t)
 _lib = None
+
+
+class _DebugChunks(ctypes.Structure):
+    _fields_ = [("ediv", ctypes.c_int), ("nchunks", ctypes.c_int), ("cptr", ctypes.c_void_p * 32), ("SAq", ctypes.c_longlong * 32)]
+
+
+class _DebugOp(ctypes.Structure):
+    """dfft_debug_op (dfft.h)"""
+    _fields_ = [("N", ctypes.c_int), ("C", ctypes.c_int), ("G", ctypes.c_int), ("W", ctypes.c_int), ("ntiles", ctypes.c_longlong),
+                ("inv", ctypes.c_int), ("do_scale", ctypes.c_int), ("scale", ctypes.c_double), ("tw_n", ctypes.c_longlong),
+                ("in_", ctypes.c_void_p), ("out", ctypes.c_void_p), ("mult", ctypes.c_void_p),
+                ("ia", ctypes.c_longlong * 4), ("oa", ctypes.c_longlong * 4), ("ci", _DebugChunks), ("co", _DebugChunks)]
 
 
 def lib():
@@ -123,6 +135,7 @@ def lib():
     L.dfft_length_kind.argtypes = [i, i]
     L.dfft_debug_plan_ops.argtypes = [vp, ctypes.c_char_p, ll]
     L.dfft_debug_plan_ops.restype = ll
+    L.dfft_debug_launch_op.argtypes = [ctypes.c_char_p, P(_DebugOp), ctypes.c_char_p, P(_DebugOp), i]
     L.dfft_debug_lines_ops.argtypes = [i, ll, ll, ll, ll, ll, i, i, i, ctypes.c_char_p, ll]
     L.dfft_debug_lines_ops.restype = ll
     L.dfft_length_schedule.argtypes = [i, i, P(ctypes.c_int), i]
@@ -408,6 +421,10 @@ def memcpy_dtoh(host_ptr, dev_ptr, nbytes):
     _check(lib().dfft_memcpy(host_ptr, dev_ptr, nbytes, 2), "dfft_memcpy")
 
 
+def memcpy_dtod(dst_ptr, src_ptr, nbytes):
+    _check(lib().dfft_memcpy(dst_ptr, src_ptr, nbytes, 0), "dfft_memcpy")
+
+
 class LinesPlan:
     """templateFFT engine surface (templateFFT.h:361-365): initializeFFT -> LinesPlan(...), launchFFTKernel -> execute,
     deleteFFT -> destroy.  Batched 1-D lines (contiguous or strided), with `two_d=(nx, ny, batch)` batched 2-D, or with
@@ -568,6 +585,31 @@ def lines_ops(n, stride, nlines, inner, inner_dist, outer_dist, direction, preci
     buf = ctypes.create_string_buffer(int(need))
     lib().dfft_debug_lines_ops(n, stride, nlines, inner, inner_dist, outer_dist, precision, direction, int(two_d), buf, need)
     return json.loads(buf.value.decode())
+
+
+def _debug_op(rec):
+    d = _DebugOp()
+    for k in ("N", "C", "G", "W", "ntiles", "inv", "do_scale", "scale", "tw_n"):
+        setattr(d, k, rec[k])
+    d.in_, d.out, d.mult = rec.get("in") or None, rec.get("out") or None, rec.get("mult") or None
+    d.ia[:], d.oa[:] = rec["ia"], rec["oa"]
+    for side in ("ci", "co"):
+        if side in rec:
+            ch, dst = rec[side], getattr(d, side)
+            dst.ediv, dst.nchunks = ch["ediv"], ch["nchunks"]
+            for q in range(min(ch["nchunks"], 32)):
+                dst.cptr[q], dst.SAq[q] = ch["cptr"][q] or None, ch["SAq"][q]
+    return d
+
+
+def debug_launch_op(rec, precision, second=None):
+    """launch the kernel of one recorded pass (a dict of Plan.recorded_ops() with device pointers in place of its symbolic
+    addresses) once on the current device and wait for it; a fused pair passes its second record as `second` (test hook
+    dfft_debug_launch_op).  Returns the library's code: 0, or DFFT_EINVAL (-1) / DFFT_EUNSUPPORTED (-3) for a record it refuses."""
+    a = _debug_op(rec)
+    b = _debug_op(second) if second is not None else None
+    return lib().dfft_debug_launch_op(rec["op"].encode(), ctypes.byref(a), second["op"].encode() if b is not None else None,
+                                      ctypes.byref(b) if b is not None else None, precision)
 
 
 def fft_lines(ptr, n, stride, nlines, inner, inner_dist, outer_dist, direction, precision=DOUBLE):

@@ -543,6 +543,34 @@ template <typename T> static cudaError_t upload_lut(void** dst, int nstages, con
     return cudaMemcpy(*dst, lut.data(), lut.size() * sizeof(cx<T>), cudaMemcpyHostToDevice);
 }
 
+// lines per tile of a pass kind's kernel in entry e: contiguous (Z), strided local (Y, unpack load, convolution X pass), peer /
+// packed store (Y with the chunked store, chunked convolution X pass), X passes
+static int kind_C(const SizeEntry* e, int kind)
+{
+    switch (kind) {
+    case PK_Z: return e->z_C;
+    case PK_Y: case PK_XCONV: return e->s_C;
+    case PK_Y_CI: return e->ci_C;
+    case PK_Y_CO: case PK_XCONV_CO: return e->p_C;
+    case PK_XB_CO: return e->xo_C;
+    default: return e->x_C;
+    }
+}
+
+// twiddle table of the radix schedule a pass kind's kernel runs: the contiguous one (Z), the X one (forward / backward X passes),
+// the strided one otherwise (Y kinds; the convolution X pass, as the natural-order X pass)
+template <typename T> static cudaError_t upload_lut_kind(void** dst, const SizeEntry* e, int kind)
+{
+    if (kind == PK_Z) return upload_lut<T>(dst, e->z_nstages, e->z_rad);
+    if (kind == PK_XF || kind == PK_XB || kind == PK_XB_CO || kind == PK_XF_TW) return upload_lut<T>(dst, e->x_nstages, e->x_rad);
+    return upload_lut<T>(dst, e->s_nstages, e->s_rad);
+}
+
+template <typename T> static void upload_lut_e(void** dst, const SizeEntry* e, bool contiguous)
+{
+    upload_lut_kind<T>(dst, e, contiguous ? PK_Z : PK_Y);
+}
+
 static int share_pointer(dfft_plan p, void* mine, std::vector<void*>& peers)
 {
     // make `mine` (a cudaMalloc allocation of this device) addressable by every rank
@@ -715,17 +743,17 @@ static int plan_create(long long n0, long long n1, long long n2, void* in, void*
     if (dry) {
         // no twiddle tables: the interpreter of the recorded passes does its own transforms
     } else if (precision == DFFT_DOUBLE) {
-        CUP(upload_lut<double>(&p->lut_z, ez->z_nstages, ez->z_rad));
-        CUP(upload_lut<double>(&p->lut_y, ey->s_nstages, ey->s_rad));
-        CUP(upload_lut<double>(&p->lut_x, ex->x_nstages, ex->x_rad));
+        CUP(upload_lut_kind<double>(&p->lut_z, ez, PK_Z));
+        CUP(upload_lut_kind<double>(&p->lut_y, ey, PK_Y));
+        CUP(upload_lut_kind<double>(&p->lut_x, ex, PK_XF));
     } else {
-        CUP(upload_lut<float>(&p->lut_z, ez->z_nstages, ez->z_rad));
-        CUP(upload_lut<float>(&p->lut_y, ey->s_nstages, ey->s_rad));
-        CUP(upload_lut<float>(&p->lut_x, ex->x_nstages, ex->x_rad));
+        CUP(upload_lut_kind<float>(&p->lut_z, ez, PK_Z));
+        CUP(upload_lut_kind<float>(&p->lut_y, ey, PK_Y));
+        CUP(upload_lut_kind<float>(&p->lut_x, ex, PK_XF));
     }
     if (conv && !dry) {   // the fused X pass runs the x entry's strided schedule (as the natural-order X pass does)
-        if (precision == DFFT_DOUBLE) CUP(upload_lut<double>(&p->lut_xn, ex->s_nstages, ex->s_rad));
-        else CUP(upload_lut<float>(&p->lut_xn, ex->s_nstages, ex->s_rad));
+        if (precision == DFFT_DOUBLE) CUP(upload_lut_kind<double>(&p->lut_xn, ex, PK_XCONV));
+        else CUP(upload_lut_kind<float>(&p->lut_xn, ex, PK_XCONV));
     }
     if (!dry) CUP(cudaGetLastError());
     if (!dry && !(flags & DFFT_NO_TMA) && buf2_aligned) {
@@ -1136,7 +1164,7 @@ template <typename T> struct Pass {
         a.inv = dir == DFFT_BACKWARD ? 1 : 0;
         a.gen = e->gen;
         const int axis = axis_override >= 0 ? axis_override : (kind == PK_Z ? 0 : (kind == PK_Y || kind == PK_Y_CO || kind == PK_Y_CI ? 1 : 2));
-        const int C = kind == PK_Z ? e->z_C : (kind == PK_Y || kind == PK_Y_CI ? e->s_C : (kind == PK_Y_CO ? e->p_C : e->x_C));
+        const int C = kind_C(e, kind);
         auto rec = [&] {
             record_op<T>(p->ops, kPassNames[kind], phase(p, dir, dir == DFFT_FORWARD ? axis == 2 : axis != 2), e->N, C, kind == PK_Y_CI,
                          kind == PK_Y_CO || kind == PK_XB_CO, kind == PK_XF || kind == PK_XF_TW, a);
@@ -1227,10 +1255,11 @@ template <typename T> struct Pass {
         }
         TileArgs<T> a{};
         a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)p->lut_y;
-        a.ia = a.oa = y_cols(p, a, mode == 1 ? p->ey->p_C : p->ey->s_C, g.n2);
+        const int kind = mode == 0 ? PK_Y : (mode == 1 ? PK_Y_CO : PK_Y_CI);
+        a.ia = a.oa = y_cols(p, a, kind_C(p->ey, kind), g.n2);
         if (mode != 0) chunk_table(p, mode == 1 ? a.co : a.ci, true, g.n2, chunk_base);
         apply_fold<T>(p, a, fold);
-        return launch(p, p->ey, mode == 0 ? PK_Y : (mode == 1 ? PK_Y_CO : PK_Y_CI), a, dir);
+        return launch(p, p->ey, kind, a, dir);
     }
     // t0 in one persistent kernel (square planes): forward Z (zsrc -> mid) then Y (mid -> ydst, or chunked);
     // backward Y (ysrc or chunked -> mid) then Z (mid -> mid).  ymode as in y_pass.
@@ -1428,7 +1457,7 @@ template <typename T> struct Pass {
     static int xb_part(dfft_plan p, const void* src, long long zk, int k, void* const* chunk_base, int cap)
     {
         TileArgs<T> a{};
-        x_tiles(p, a, p->ex->x_C, zk, false);
+        x_tiles(p, a, p->ex->xo_C, zk, false);
         a.oa.SA = 0;   // the chunk table's SAq places the planes
         a.in = (const cx<T>*)src + k * zk * p->g.n0; a.out = nullptr; a.lut = (const cx<T>*)p->lut_x;
         chunk_table(p, a.co, false, zk, chunk_base);
@@ -1453,7 +1482,7 @@ template <typename T> struct Pass {
     static int yinv_part(dfft_plan p, const void* rpart, void* dst, long long zk, int k, int cap, cudaStream_t st)
     {
         TileArgs<T> a{};
-        yinv_part_args(p, a, rpart, dst, zk, k, p->ey->s_C);
+        yinv_part_args(p, a, rpart, dst, zk, k, p->ey->ci_C);
         a.max_ctas_per_sm = cap;
         return launch(p, p->ey, PK_Y_CI, a, DFFT_BACKWARD, -1, st);
     }
@@ -1488,7 +1517,7 @@ template <typename T> struct Pass {
             return launch_tma(p, p->tx, TMA_XB, t, nullptr, &to, 2, DFFT_BACKWARD);
         }
         TileArgs<T> a{};
-        x_tiles(p, a, p->ex->x_C, g.n2, false);
+        x_tiles(p, a, chunk_base ? p->ex->xo_C : p->ex->x_C, g.n2, false);
         a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)p->lut_x;
         if (chunk_base) {
             chunk_table(p, a.co, false, g.n2, chunk_base);
@@ -1503,7 +1532,8 @@ template <typename T> struct Pass {
     {
         const Geom& g = p->g;
         const bool co = chunk_base != nullptr;
-        const int C = co ? p->ex->p_C : p->ex->s_C;
+        const int kind = co ? PK_XCONV_CO : PK_XCONV;
+        const int C = kind_C(p->ex, kind);
         ConvArgs<T> r{};
         TileArgs<T>& a = r.t;
         a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)p->lut_xn;
@@ -1513,7 +1543,6 @@ template <typename T> struct Pass {
         if (co) chunk_table(p, a.co, false, g.n2, chunk_base);
         r.mult = (const cx<T>*)mult;
         apply_fold<T>(p, a, fold);
-        const int kind = co ? PK_XCONV_CO : PK_XCONV;
         auto rec = [&] {
             char extra[64];
             snprintf(extra, sizeof(extra), ", \"mult\": %llu", (unsigned long long)(size_t)mult);
@@ -2179,6 +2208,140 @@ extern "C" long long dfft_debug_plan_ops(dfft_plan p, char* buf, long long cap)
     return ops_json(p->ops, buf, cap);
 }
 
+static_assert(sizeof(((dfft_debug_chunks*)nullptr)->cptr) / sizeof(void*) == DFFT_MAX_CHUNKS, "dfft_debug_chunks mirrors ChunkTab");
+
+// one record of dfft_debug_launch_op as the kernel's TileArgs; the checks every kind shares.  want_ci / want_co: the kind loads /
+// stores through a chunk table (which must then be given, and must not be otherwise)
+template <typename T>
+static int replay_args(const char* name, const dfft_debug_op* r, const SizeEntry* e, int C, bool want_ci, bool want_co, TileArgs<T>& a)
+{
+    if (r->C != C) return fail(DFFT_EINVAL, "dfft_debug_launch_op: %s record of N=%d has C=%d, the entry's configuration has %d", name, r->N, r->C, C);
+    if (r->G < 1 || r->ntiles < 0 || r->ntiles % r->G || r->W <= (long long)(r->G - 1) * C || r->W > (long long)r->G * C)
+        return fail(DFFT_EINVAL, "dfft_debug_launch_op: %s record with inconsistent G=%d, W=%d, ntiles=%lld (C=%d)", name, r->G, r->W, r->ntiles, C);
+    const dfft_debug_chunks* side[2] = {&r->ci, &r->co};
+    const bool want[2] = {want_ci, want_co};
+    ChunkTab* tab[2] = {&a.ci, &a.co};
+    for (int s = 0; s < 2; s++) {
+        const dfft_debug_chunks& ch = *side[s];
+        if (!want[s]) {
+            if (ch.nchunks != 0) return fail(DFFT_EINVAL, "dfft_debug_launch_op: %s takes no chunk table on its %s side", name, s ? "store" : "load");
+            continue;
+        }
+        if (ch.nchunks < 1 || ch.nchunks > DFFT_MAX_CHUNKS || ch.ediv < 1)
+            return fail(DFFT_EINVAL, "dfft_debug_launch_op: %s needs a chunk table on its %s side", name, s ? "store" : "load");
+        for (int q = 0; q < ch.nchunks; q++) {
+            if (!ch.cptr[q]) return fail(DFFT_EINVAL, "dfft_debug_launch_op: %s chunk %d has a null pointer", name, q);
+            tab[s]->cptr[q] = ch.cptr[q];
+            tab[s]->SAq[q] = ch.SAq[q];
+        }
+        tab[s]->ediv = ch.ediv;
+        tab[s]->nchunks = ch.nchunks;
+    }
+    if ((!want_ci && !r->in) || (!want_co && !r->out)) return fail(DFFT_EINVAL, "dfft_debug_launch_op: %s record with a null buffer", name);
+    a.in = (const cx<T>*)r->in; a.out = (cx<T>*)r->out;
+    a.ia = Affine{r->ia[0], r->ia[1], r->ia[2], r->ia[3]};
+    a.oa = Affine{r->oa[0], r->oa[1], r->oa[2], r->oa[3]};
+    a.ntiles = r->ntiles; a.G = r->G; a.W = r->W;
+    a.inv = r->inv ? 1 : 0; a.do_scale = r->do_scale ? 1 : 0; a.scale = (T)r->scale;
+    a.tw_n = r->tw_n;
+    a.gen = e->gen;
+    return 0;
+}
+
+template <typename T>
+static int replay_op(const char* op, const dfft_debug_op* r, const char* op2, const dfft_debug_op* r2, int precision)
+{
+    int sms = 132, dev = 0;
+    CU(cudaGetDevice(&dev));
+    CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const SizeEntry* e = find_size_entry(r->N, precision);
+    if (!e) return fail(DFFT_EINVAL, "dfft_debug_launch_op: no kernel entry of length %d", r->N);
+    const bool fz = !strcmp(op, "fusedZ"), fy = !strcmp(op, "fusedY");
+    std::vector<void*> owned;   // twiddle tables and fused controls of this launch
+    auto release = [&](int rc) {
+        for (void* q : owned) cudaFree(q);
+        return rc;
+    };
+#define CUR(x)                                                                                        \
+    do {                                                                                              \
+        cudaError_t e_ = (x);                                                                         \
+        if (e_ != cudaSuccess) return release(fail(DFFT_ECUDA, "%s:%d CUDA call '%s' failed: %s", __FILE__, __LINE__, #x, cudaGetErrorString(e_))); \
+    } while (0)
+    auto lut = [&](int kind, const cx<T>** out) {
+        void* d = nullptr;
+        const cudaError_t err = upload_lut_kind<T>(&d, e, kind);
+        if (d) owned.push_back(d);
+        *out = (const cx<T>*)d;
+        return err;
+    };
+    cudaError_t err;
+    if (fz || fy) {
+        // the two roles of a t0 kernel, records in their recorded order: forward fusedZ + fusedY (FK_ZY_CO with the chunked
+        // store), backward fusedY + fusedZ (FK_YZ_CI with the chunked load)
+        const char* other = fz ? "fusedY" : "fusedZ";
+        if (!r2 || !op2 || strcmp(op2, other)) return fail(DFFT_EINVAL, "dfft_debug_launch_op: %s needs its %s record", op, other);
+        if (r2->N != r->N) return fail(DFFT_EINVAL, "dfft_debug_launch_op: the fused roles have lengths %d and %d", r->N, r2->N);
+        const dfft_debug_op& zr = fz ? *r : *r2;
+        const dfft_debug_op& yr = fz ? *r2 : *r;
+        const bool chunked = fz ? yr.co.nchunks != 0 : yr.ci.nchunks != 0;
+        const int kind = fz ? (chunked ? FK_ZY_CO : FK_ZY) : (chunked ? FK_YZ_CI : FK_YZ);
+        const int CZ = kind == FK_ZY_CO ? e->f_zCp : e->f_zC, CY = kind == FK_ZY_CO ? e->p_C : e->s_C;
+        if (!e->fused[kind]) return fail(DFFT_EUNSUPPORTED, "dfft_debug_launch_op: length %d has no fused kernel of kind %d", r->N, kind);
+        TileArgs<T> z{}, y{};
+        int rc = replay_args<T>("fusedZ", &zr, e, CZ, false, false, z);
+        if (!rc) rc = replay_args<T>("fusedY", &yr, e, CY, !fz && chunked, fz && chunked, y);
+        if (rc) return rc;
+        if (z.ntiles / z.G != y.ntiles / y.G) return fail(DFFT_EINVAL, "dfft_debug_launch_op: the fused roles cover different planes");
+        CUR(lut(PK_Z, &z.lut));
+        CUR(lut(PK_Y, &y.lut));
+        // as fused_ctl does for the first execute of a plan: zeroed plane counters and ticket words, role A done at GA
+        FusedCtl c{};
+        c.planes = z.ntiles / z.G;
+        c.GA = fz ? z.G : y.G; c.GB = fz ? y.G : z.G;
+        c.target = (unsigned long long)c.GA;
+        c.lag = 0;
+        CUR(cudaMalloc((void**)&c.plane_done, (size_t)std::max<long long>(c.planes, 1) * sizeof(unsigned long long)));
+        owned.push_back(c.plane_done);
+        CUR(cudaMemset(c.plane_done, 0, (size_t)std::max<long long>(c.planes, 1) * sizeof(unsigned long long)));
+        CUR(cudaMalloc((void**)&c.ticket, 4 * sizeof(unsigned int)));
+        owned.push_back(c.ticket);
+        CUR(cudaMemset(c.ticket, 0, 4 * sizeof(unsigned int)));
+        err = fz ? e->fused[kind](&z, &y, &c, sms, nullptr) : e->fused[kind](&y, &z, &c, sms, nullptr);
+    } else {
+        int kind = -1;
+        for (int k = 0; k < PK_COUNT; k++)
+            if (!strcmp(op, kPassNames[k])) kind = k;
+        if (kind < 0 || kind == PK_Z_R2C || kind == PK_Z_C2R)
+            return fail(DFFT_EINVAL, "dfft_debug_launch_op: '%s' is not a record this hook launches", op);
+        if (!e->launch[kind]) return fail(DFFT_EUNSUPPORTED, "dfft_debug_launch_op: length %d has no %s kernel", r->N, op);
+        if (r2 || op2) return fail(DFFT_EINVAL, "dfft_debug_launch_op: %s is one record", op);
+        const bool conv = kind == PK_XCONV || kind == PK_XCONV_CO;
+        if (conv && !r->mult) return fail(DFFT_EINVAL, "dfft_debug_launch_op: %s record with a null multiplier", op);
+        ConvArgs<T> cv{};
+        TileArgs<T>& a = cv.t;
+        const int rc = replay_args<T>(op, r, e, kind_C(e, kind), kind == PK_Y_CI, kind == PK_Y_CO || kind == PK_XB_CO || kind == PK_XCONV_CO, a);
+        if (rc) return rc;
+        CUR(lut(kind, &a.lut));
+        cv.mult = (const cx<T>*)r->mult;
+        err = e->launch[kind](conv ? (const void*)&cv : (const void*)&a, sms, nullptr);
+    }
+    if (err != cudaSuccess) cudaGetLastError();   // a refused launch must not be reported again by the next one
+    CUR(err);
+    CUR(cudaStreamSynchronize(nullptr));
+#undef CUR
+    return release(0);
+}
+
+/* test hook: launch one record of a DFFT_DRY_RUN plan (see dfft.h) */
+extern "C" int dfft_debug_launch_op(const char* op, const dfft_debug_op* rec, const char* second_op, const dfft_debug_op* second, int precision)
+{
+    if (!op || !rec) return fail(DFFT_EINVAL, "dfft_debug_launch_op: null record");
+    if (precision != DFFT_DOUBLE && precision != DFFT_FLOAT) return fail(DFFT_EINVAL, "dfft_debug_launch_op: bad precision");
+    if (!strcmp(op, "ovlZ") || !strcmp(op, "ovlY") || !strcmp(op, "ovlX"))
+        return fail(DFFT_EINVAL, "dfft_debug_launch_op: the single-kernel forward (%s) waits on its peers' arrival flags", op);
+    return precision == DFFT_DOUBLE ? replay_op<double>(op, rec, second_op, second, precision) : replay_op<float>(op, rec, second_op, second, precision);
+}
+
 extern "C" int dfft_plan_launches(dfft_plan p) { return p ? p->launches : 0; }
 extern "C" int dfft_plan_exchange(dfft_plan p) { return p ? p->xmode : 0; }
 /* bit 0 / 1 / 2: the un-chunked Z / Y / X pass of this plan runs on the TMA-pipelined kernel (fft_tma.cuh) */
@@ -2255,12 +2418,6 @@ struct dfft_lines_plan_s {
     cudaEvent_t ev[2] = {nullptr, nullptr};
     bool timed = false;
 };
-
-template <typename T> static void upload_lut_e(void** dst, const SizeEntry* e, bool contiguous)
-{
-    if (contiguous) upload_lut<T>(dst, e->z_nstages, e->z_rad);
-    else upload_lut<T>(dst, e->s_nstages, e->s_rad);
-}
 
 // a * b * c < 2^31 (the kernels' 32-bit row counts TileArgs::W / G), without overflow for any non-negative arguments.  Column
 // counts need no check: a strided pass's columns (nx*ny, ny*(nx/2+1)) are below 2^25 for every supported length

@@ -51,6 +51,9 @@ struct SizeEntry {
     int variant;          // 0 = default; > 0 = alternate tuning of the same length, selected with DFFT_VARIANT (experiments)
     int prec;             // 0 = double, 1 = float
     int z_C, s_C, p_C, x_C;   // lines per tile: contiguous (Z), strided local (Y), strided with peer/packed store, X passes
+    int ci_C, xo_C;           // lines per tile of the Y pass with the chunked (unpack) load and of the X pass with the chunked store:
+                              // s_C and x_C, halved where that tile, its twiddles and the chunk tables would not fit in one block's
+                              // shared memory (4096-point fp64); p_C is chosen the same way
     int z_nstages, z_rad[24];
     int s_nstages, s_rad[24];
     int x_nstages, x_rad[24];

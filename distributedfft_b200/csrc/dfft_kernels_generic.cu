@@ -137,7 +137,7 @@ const SizeEntry* generic_size_entry(int N, int prec)
     }
     SizeEntry* e = new SizeEntry{};
     e->N = N; e->prec = prec; e->variant = 0;
-    e->z_C = e->s_C = e->p_C = e->x_C = g->C;
+    e->z_C = e->s_C = e->p_C = e->x_C = e->ci_C = e->xo_C = g->C;
     e->f_zC = e->f_zCp = 0;
     e->z_nstages = e->s_nstages = e->x_nstages = g->nstages;
     for (int s = 0; s < g->nstages; s++) e->z_rad[s] = e->s_rad[s] = e->x_rad[s] = g->rad[s];

@@ -273,6 +273,15 @@ template <class OpA, class OpB, typename T, int MINB> constexpr FusedLaunchFn fu
     else return nullptr;
 }
 
+// lines per tile of a configuration whose load or store goes through the chunk tables: C, halved until the tile's exchange
+// buffer, its twiddles and the chunk tables fit in one block's shared memory (4096-point fp64: 2 -> 1; every other tuned
+// configuration keeps its C)
+template <class S, typename T, int C, bool PP> constexpr int chunked_C()
+{
+    if constexpr (C > 1 && TileSmem<S, T, C, PP>::bytes(true) > SMEM_OPTIN_MAX) return chunked_C<S, T, C / 2, PP>();
+    else return C;
+}
+
 template <class S> void fill_rad(int& n, int* rad)
 {
     n = S::NSTAGES;
@@ -292,13 +301,19 @@ template <class S_, int C_, bool TW_, int MB_, bool PP_> struct Cfg {
 // FH bit 0: the fused t0 kernels carry L2 eviction hints (first role: streamed input evict_first, intermediate evict_last;
 // second role: intermediate and output evict_first); FH bit 1: the contiguous role of the fused kernels synchronises per
 // line (named barriers) instead of per CTA -- experiments, see DESIGN.md
-template <typename T, class Z, class Y, class X = Y, class PEER = Y, int FH = 0>
+template <class G, int C_> using WithC = Cfg<typename G::S, C_, G::TW, G::MB, G::PP>;
+
+template <typename T, class Z, class Y, class X = Y, class PEER_ = Y, int FH = 0>
 SizeEntry make_entry(int variant = 0)
 {
     using ZS = typename Z::S;
     using SS = typename Y::S;
     using XS = typename X::S;
-    static_assert(std::is_same<typename PEER::S, SS>::value, "the peer-store configuration shares the Y schedule");
+    static_assert(std::is_same<typename PEER_::S, SS>::value, "the peer-store configuration shares the Y schedule");
+    // the chunked kinds in configurations that can be launched (chunked_C)
+    using PEER = WithC<PEER_, chunked_C<SS, T, PEER_::C, PEER_::PP>()>;
+    using YCI = WithC<Y, chunked_C<SS, T, Y::C, Y::PP>()>;
+    using XCO = WithC<X, chunked_C<XS, T, X::C, X::PP>()>;
     SizeEntry e{};
     e.N = ZS::N;
     e.variant = variant;
@@ -307,16 +322,18 @@ SizeEntry make_entry(int variant = 0)
     e.s_C = Y::C;
     e.p_C = PEER::C;
     e.x_C = X::C;
+    e.ci_C = YCI::C;
+    e.xo_C = XCO::C;
     fill_rad<ZS>(e.z_nstages, e.z_rad);
     fill_rad<SS>(e.s_nstages, e.s_rad);
     fill_rad<XS>(e.x_nstages, e.x_rad);
     e.launch[PK_Z] = launch_pass<ZS, T, Z::C, MAP_T, MAP_T, Z::TW, false, false, Z::MB, Z::PP>;
     e.launch[PK_Y] = launch_pass<SS, T, Y::C, MAP_C, MAP_C, Y::TW, false, false, Y::MB, Y::PP>;
     e.launch[PK_Y_CO] = launch_pass<SS, T, PEER::C, MAP_C, MAP_C, PEER::TW, false, true, PEER::MB, PEER::PP>;
-    e.launch[PK_Y_CI] = launch_pass<SS, T, Y::C, MAP_C, MAP_C, Y::TW, true, false, Y::MB, Y::PP>;
+    e.launch[PK_Y_CI] = launch_pass<SS, T, YCI::C, MAP_C, MAP_C, YCI::TW, true, false, YCI::MB, YCI::PP>;
     e.launch[PK_XF] = launch_pass<XS, T, X::C, MAP_C, MAP_T, X::TW, false, false, X::MB, X::PP>;
     e.launch[PK_XB] = launch_pass<XS, T, X::C, MAP_T, MAP_C, X::TW, false, false, X::MB, X::PP>;
-    e.launch[PK_XB_CO] = launch_pass<XS, T, X::C, MAP_T, MAP_C, X::TW, false, true, X::MB, X::PP>;
+    e.launch[PK_XB_CO] = launch_pass<XS, T, XCO::C, MAP_T, MAP_C, XCO::TW, false, true, XCO::MB, XCO::PP>;
     e.launch[PK_XF_TW] = launch_pass<XS, T, X::C, MAP_C, MAP_T, X::TW, false, false, X::MB, X::PP, true>;
     // real-data Z passes with the contiguous configuration (C line pairs per tile); default entries only -- the alternate
     // tunings are experiments on the C2C path.  Twiddles come from shared memory (TWREG off): the pair loads and the split
@@ -359,7 +376,7 @@ SizeEntry make_entry(int variant = 0)
     e.fused[FK_ZY] = fused_if_fits<OZ, OY2, T, Y::MB>();
     e.fused[FK_ZY_CO] = fused_if_fits<OZp, OYco, T, PEER::MB>();
     e.fused[FK_YZ] = fused_if_fits<OY, OZ2, T, Y::MB>();
-    e.fused[FK_YZ_CI] = fused_if_fits<OYci, OZ2, T, Y::MB>();
+    e.fused[FK_YZ_CI] = YCI::C == Y::C ? fused_if_fits<OYci, OZ2, T, Y::MB>() : nullptr;   // (the roles share Y's tile)
     // whole forward transform of a device in one kernel: needs the X role to fill the peer-store CTA shape
     e.fused3 = nullptr; e.fused_yx = nullptr;
     if constexpr (XS::T * X::C == NTP) {

@@ -114,6 +114,31 @@ long long dfft_debug_fused2_order(long long planes, int GA, int GB, int lag, lon
  * tables, symbolic buffer addresses: device d, buffer b at ((d+1) << 44) | (b << 40), b = 1 bufferDev1, 2 out, 3 receive/work,
  * 4 intermediate, 5 in).  Returns the number of bytes needed (including the terminator). */
 long long dfft_debug_plan_ops(dfft_plan plan, char* buf, long long cap);
+/* test hook: one record of dfft_debug_plan_ops with its symbolic addresses replaced by device pointers.  A side without a chunk
+ * table has nchunks = 0; `mult` is the multiplier of an "XCONV" / "XCONV_CO" record, NULL otherwise. */
+typedef struct dfft_debug_chunks {
+    int ediv, nchunks;
+    void* cptr[32];       /* at most 32 chunks, one per device */
+    long long SAq[32];
+} dfft_debug_chunks;
+typedef struct dfft_debug_op {
+    int N, C, G, W;
+    long long ntiles;
+    int inv, do_scale;
+    double scale;
+    long long tw_n;
+    void *in, *out, *mult;
+    long long ia[4], oa[4];
+    dfft_debug_chunks ci, co;
+} dfft_debug_op;
+/* test hook: launch the kernel of one record once on the current device's legacy default stream and wait for it, with the
+ * twiddle table its entry and kind use in a plan and no arrival flags (nothing waits, nothing is signalled).  `op` is the
+ * record's name: "Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW", "XCONV", "XCONV_CO", or the first record of a fused
+ * pair ("fusedZ" forward, "fusedY" backward) with the other record and its name in `second` / `second_op` (NULL otherwise); a
+ * pair runs as one two-role kernel on its own zeroed plane counters.  Plans never call it.  DFFT_EINVAL: an unknown name, a single-kernel forward
+ * record ("ovlZ" / "ovlY" / "ovlX"), a C other than the entry's for that kind, inconsistent tiling, a missing or superfluous
+ * chunk table, a null pointer, a bad precision; DFFT_EUNSUPPORTED: the entry has no such kernel. */
+int dfft_debug_launch_op(const char* op, const dfft_debug_op* rec, const char* second_op, const dfft_debug_op* second, int precision);
 /* test hook (host only): the passes a lines plan (1-D, 2-D when two_d != 0: n = nx, stride = ny, nlines = batch, or the
  * four-step plan of a long line) would launch, same JSON as dfft_debug_plan_ops: data = buffer 1, temporary = buffer 4 */
 long long dfft_debug_lines_ops(int n, long long stride, long long nlines, long long inner, long long inner_dist, long long outer_dist,

@@ -18,7 +18,7 @@ import pytest
 import distributedfft_b200 as dfft
 import ldfft
 from oracle import SlabGeometry
-from test_dry_run import BUF1, IN, OUT, Machine, decode, fake, run_alltoall, run_pass
+from test_dry_run import BUF1, IN, OUT, Machine, decode, fake, run_alltoall, run_pass, schedule
 from test_r2c_dry_run import run_real
 
 CANARY = 7.25e33
@@ -101,21 +101,15 @@ def simulate(n0, n1, n2, P, A, M, flags, real=False, inplace=False, mult_offset=
     for d, p in enumerate(plans):
         p.execute_convolve(fake(d, MULT) + 16 * mult_offset)
         ops.append(p.recorded_ops())
-    for phase in range(4):
-        for d in range(P):
-            for op in ops[d]:
-                if op["phase"] != phase or op["op"] == "alltoall":
-                    continue
-                if op["op"].startswith("XCONV"):
-                    run_conv(m, op)
-                elif op["op"] in ("Z_R2C", "Z_C2R"):
-                    run_real(m, op)
-                else:
-                    run_pass(m, op)
-        for d in range(P):
-            for op in ops[d]:
-                if op["phase"] == phase and op["op"] == "alltoall":
-                    run_alltoall(m, d, op)
+    for d, op in schedule(ops, 4):
+        if op["op"] == "alltoall":
+            run_alltoall(m, d, op)
+        elif op["op"].startswith("XCONV"):
+            run_conv(m, op)
+        elif op["op"] in ("Z_R2C", "Z_C2R"):
+            run_real(m, op)
+        else:
+            run_pass(m, op)
     res = []
     for d in range(P):
         outbuf = m.buf(d, IN if inplace else OUT)

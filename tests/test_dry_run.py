@@ -96,34 +96,45 @@ def run_alltoall(m, dev, op):
         dst[roff0 + ro: roff0 + ro + cnt] = src[soff + so: soff + so + cnt]
 
 
-def simulate(n0, n1, n2, P, direction, inputs, flags, inplace=False):
-    g = SlabGeometry(n0, n1, n2, P)
-    m = Machine(g)
-    plans = []
-    for d in range(P):
-        m.buf(d, BUF1)[: inputs[d].size] = inputs[d]      # the plan snapshots `in` into bufferDev1 (api.cpp:76-77)
-        out = None if inplace else fake(d, OUT)
-        plans.append(dfft.fft_mpi_plan_dft_c2c_3d(n0, n1, n2, fake(d, IN), out, None, d, P, direction, dfft.DOUBLE, flags | dfft.DRY_RUN))
+def schedule(ops, nphases=2):
+    """(device, record) in the order the interpreters run them: per phase, the passes of every device, then the phase's
+    all-to-alls (C2C plans record two phases, convolve plans four)"""
+    for phase in range(nphases):
+        for a2a in (False, True):
+            for d, o in enumerate(ops):
+                for op in o:
+                    if op["phase"] == phase and (op["op"] == "alltoall") == a2a:
+                        yield d, op
+
+
+def dry_ops(n0, n1, n2, P, direction, flags, precision=dfft.DOUBLE, inplace=False):
+    """the records of one execute of each of the P per-device DRY_RUN C2C plans, and whether each plan fuses its t0"""
+    plans = [dfft.fft_mpi_plan_dft_c2c_3d(n0, n1, n2, fake(d, IN), None if inplace else fake(d, OUT), None, d, P, direction, precision,
+                                          flags | dfft.DRY_RUN) for d in range(P)]
     ops = []
-    for d, p in enumerate(plans):
+    for p in plans:
         p.execute()
         ops.append(p.recorded_ops())
-    for phase in (0, 1):
-        for d in range(P):
-            for op in ops[d]:
-                if op["phase"] == phase and op["op"] != "alltoall":
-                    run_pass(m, op)
-        if phase == 0:
-            for d in range(P):
-                for op in ops[d]:
-                    if op["op"] == "alltoall":
-                        run_alltoall(m, d, op)
-    outb = IN if inplace else OUT
-    res = [m.buf(d, outb)[: g.max_count(d)].copy() for d in range(P)]
-    names = [[op["op"] for op in o] for o in ops]
     fused = [p.fused for p in plans]
     for p in plans:
         p.destroy()
+    return ops, fused
+
+
+def simulate(n0, n1, n2, P, direction, inputs, flags, inplace=False):
+    g = SlabGeometry(n0, n1, n2, P)
+    m = Machine(g)
+    for d in range(P):
+        m.buf(d, BUF1)[: inputs[d].size] = inputs[d]      # the plan snapshots `in` into bufferDev1 (api.cpp:76-77)
+    ops, fused = dry_ops(n0, n1, n2, P, direction, flags, inplace=inplace)
+    for d, op in schedule(ops):
+        if op["op"] == "alltoall":
+            run_alltoall(m, d, op)
+        else:
+            run_pass(m, op)
+    outb = IN if inplace else OUT
+    res = [m.buf(d, outb)[: g.max_count(d)].copy() for d in range(P)]
+    names = [[op["op"] for op in o] for o in ops]
     return res, names, fused
 
 

@@ -18,6 +18,7 @@ from numpy.lib.stride_tricks import as_strided
 
 import distributedfft_b200 as dfft
 from oracle import BACKWARD, FORWARD, SlabGeometry
+from test_dry_run import schedule
 
 BUF1, OUT, WORK, MID, IN = 1, 2, 3, 4, 5
 
@@ -122,6 +123,15 @@ def run_alltoall(fp, dev, op):
         fp.region(q, rbuf)[roff + ro: roff + ro + cnt] = 1
 
 
+def walk(fp, ops, nphases=2):
+    """every record of every device in the interpreters' order (test_dry_run.schedule) through the checks above"""
+    for d, op in schedule(ops, nphases):
+        if op["op"] == "alltoall":
+            run_alltoall(fp, d, op)
+        else:
+            run_pass(fp, op)
+
+
 def check(n0, n1, n2, P, direction, flags, precision=dfft.DOUBLE, mutate=None):
     need = 10 * n0 * n1 * n2            # one byte per element for ~4 buffers x (written + per-pass counts), all devices
     if need > 2 ** 30:
@@ -140,16 +150,7 @@ def check(n0, n1, n2, P, direction, flags, precision=dfft.DOUBLE, mutate=None):
         ops.append(p.recorded_ops())
     if mutate:
         mutate(ops)
-    for phase in (0, 1):
-        for d in range(P):
-            for op in ops[d]:
-                if op["phase"] == phase and op["op"] != "alltoall":
-                    run_pass(fp, op)
-        if phase == 0:
-            for d in range(P):
-                for op in ops[d]:
-                    if op["op"] == "alltoall":
-                        run_alltoall(fp, d, op)
+    walk(fp, ops)
     for d in range(P):
         cnt_out = g.out_count(d) if direction == FORWARD else g.in_count(d)
         out = fp.region(d, OUT)
