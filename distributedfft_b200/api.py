@@ -425,23 +425,13 @@ def memcpy_dtod(dst_ptr, src_ptr, nbytes):
     _check(lib().dfft_memcpy(dst_ptr, src_ptr, nbytes, 0), "dfft_memcpy")
 
 
-class LinesPlan:
-    """templateFFT engine surface (templateFFT.h:361-365): initializeFFT -> LinesPlan(...), launchFFTKernel -> execute,
-    deleteFFT -> destroy.  Batched 1-D lines (contiguous or strided), with `two_d=(nx, ny, batch)` batched 2-D, or with
-    `three_d=(nx, ny, nz, batch)` batched 3-D (numpy.fft.fftn over the last three axes of a[batch][nz][ny][nx])."""
+class _LinesPlanBase:
+    """what the three lines plan classes share: the plan handle, its stream, synchronize and destroy"""
 
-    def __init__(self, n=None, stride=1, nlines=0, inner=0, inner_dist=0, outer_dist=0, precision=DOUBLE, two_d=None, three_d=None):
+    def _create(self, name, *args):
         h = ctypes.c_void_p()
-        if three_d is not None:
-            _check(lib().dfft_lines_plan_create_3d(*three_d, precision, ctypes.byref(h)), "dfft_lines_plan_create_3d")
-        elif two_d is not None:
-            _check(lib().dfft_lines_plan_create_2d(two_d[0], two_d[1], two_d[2], precision, ctypes.byref(h)), "dfft_lines_plan_create_2d")
-        else:
-            _check(lib().dfft_lines_plan_create(n, stride, nlines, inner, inner_dist, outer_dist, precision, ctypes.byref(h)), "dfft_lines_plan_create")
+        _check(getattr(lib(), name)(*args, ctypes.byref(h)), name)
         self.handle = h
-
-    def execute(self, ptr, direction):
-        _check(lib().dfft_lines_execute(self.handle, ptr, direction), "dfft_lines_execute")
 
     def synchronize(self):
         _check(lib().dfft_lines_synchronize(self.handle), "dfft_lines_synchronize")
@@ -456,39 +446,42 @@ class LinesPlan:
             self.handle = None
 
 
-class RealLinesPlan:
+class LinesPlan(_LinesPlanBase):
+    """templateFFT engine surface (templateFFT.h:361-365): initializeFFT -> LinesPlan(...), launchFFTKernel -> execute,
+    deleteFFT -> destroy.  Batched 1-D lines (contiguous or strided), with `two_d=(nx, ny, batch)` batched 2-D, or with
+    `three_d=(nx, ny, nz, batch)` batched 3-D (numpy.fft.fftn over the last three axes of a[batch][nz][ny][nx])."""
+
+    def __init__(self, n=None, stride=1, nlines=0, inner=0, inner_dist=0, outer_dist=0, precision=DOUBLE, two_d=None, three_d=None):
+        if three_d is not None:
+            self._create("dfft_lines_plan_create_3d", *three_d, precision)
+        elif two_d is not None:
+            self._create("dfft_lines_plan_create_2d", two_d[0], two_d[1], two_d[2], precision)
+        else:
+            self._create("dfft_lines_plan_create", n, stride, nlines, inner, inner_dist, outer_dist, precision)
+
+    def execute(self, ptr, direction):
+        _check(lib().dfft_lines_execute(self.handle, ptr, direction), "dfft_lines_execute")
+
+
+class RealLinesPlan(_LinesPlanBase):
     """Real-data lines: R2C (FORWARD) / C2R (BACKWARD, unnormalised), out of place.  `nlines` densely packed real lines of `n`
     points <-> as many half spectra of n//2+1 complex points, or, with `two_d=(nx, ny, batch)`, `batch` row-major ny x nx real
     matrices <-> ny x (nx//2+1) complex matrices (numpy.fft.rfft2 layout), or, with `three_d=(nx, ny, nz, batch)`, nz x ny x nx
     real arrays <-> nz x ny x (nx//2+1) complex arrays (numpy.fft.rfftn layout)."""
 
     def __init__(self, n=None, nlines=0, precision=DOUBLE, two_d=None, three_d=None):
-        h = ctypes.c_void_p()
         if three_d is not None:
-            _check(lib().dfft_lines_plan_create_r2c_3d(*three_d, precision, ctypes.byref(h)), "dfft_lines_plan_create_r2c_3d")
+            self._create("dfft_lines_plan_create_r2c_3d", *three_d, precision)
         elif two_d is not None:
-            _check(lib().dfft_lines_plan_create_r2c_2d(two_d[0], two_d[1], two_d[2], precision, ctypes.byref(h)), "dfft_lines_plan_create_r2c_2d")
+            self._create("dfft_lines_plan_create_r2c_2d", two_d[0], two_d[1], two_d[2], precision)
         else:
-            _check(lib().dfft_lines_plan_create_r2c(n, nlines, precision, ctypes.byref(h)), "dfft_lines_plan_create_r2c")
-        self.handle = h
+            self._create("dfft_lines_plan_create_r2c", n, nlines, precision)
 
     def execute(self, in_ptr, out_ptr, direction):
         _check(lib().dfft_lines_execute_real(self.handle, in_ptr, out_ptr, direction), "dfft_lines_execute_real")
 
-    def synchronize(self):
-        _check(lib().dfft_lines_synchronize(self.handle), "dfft_lines_synchronize")
 
-    @property
-    def stream(self):
-        return lib().dfft_lines_stream(self.handle)
-
-    def destroy(self):
-        if self.handle:
-            lib().dfft_lines_destroy(self.handle)
-            self.handle = None
-
-
-class LinesConvolvePlan:
+class LinesConvolvePlan(_LinesPlanBase):
     """Batched 3-D spectral convolution, `three_d=(nx, ny, nz, batch)`: out = ifftn(fftn(in) * m) over the last three axes of
     a[batch][nz][ny][nx], unnormalised (x nx*ny*nz) unless flags=SCALE_BACKWARD; with real=True, real in / real out,
     out = irfftn(rfftn(in) * m, s=(nz, ny, nx)) * nx*ny*nz.  m is complex in the plan's precision, [nz][ny][nx] (real:
@@ -500,91 +493,55 @@ class LinesConvolvePlan:
     def __init__(self, three_d=None, precision=DOUBLE, real=False, flags=0, two_d=None):
         if (three_d is None) == (two_d is None):
             raise ValueError("give exactly one of three_d and two_d")
-        h = ctypes.c_void_p()
         dims = "3d" if two_d is None else "2d"
         name = ("dfft_lines_plan_create_convolve_r2c_" if real else "dfft_lines_plan_create_convolve_") + dims
-        _check(getattr(lib(), name)(*(three_d if two_d is None else two_d), precision, flags, ctypes.byref(h)), name)
-        self.handle = h
+        self._create(name, *(three_d if two_d is None else two_d), precision, flags)
 
     def execute(self, in_ptr, out_ptr, mult_ptr, mult_count=1):
         _check(lib().dfft_lines_execute_convolve(self.handle, in_ptr, out_ptr, mult_ptr, mult_count), "dfft_lines_execute_convolve")
 
-    def synchronize(self):
-        _check(lib().dfft_lines_synchronize(self.handle), "dfft_lines_synchronize")
 
-    @property
-    def stream(self):
-        return lib().dfft_lines_stream(self.handle)
-
-    def destroy(self):
-        if self.handle:
-            lib().dfft_lines_destroy(self.handle)
-            self.handle = None
+def _json_hook(fn, *args):
+    """the JSON records of a host-only test hook that returns the bytes it needs for (buf, cap) = (None, 0), < 0 on error"""
+    import json
+    need = fn(*args, None, 0)
+    if need < 0:
+        raise DfftError(f"{fn.__name__} failed ({need}): " + lib().dfft_last_error().decode())
+    buf = ctypes.create_string_buffer(int(need))
+    fn(*args, buf, need)
+    return json.loads(buf.value.decode())
 
 
 def lines_conv_3d_ops(nx, ny, nz, batch, precision=DOUBLE, real=False, flags=0, mult_count=1):
     """passes LinesConvolvePlan(three_d=(nx, ny, nz, batch), ...) would launch per execute (host-only test hook, see
     dfft_debug_lines_conv_3d_ops; in = buffer 5, out = 2, temporary = 4, multiplier = 8); read DFFT_NO_PLANE /
     DFFT_FORCE_PLANE / DFFT_GENERIC at the call, as plan creation does"""
-    import json
-    args = (nx, ny, nz, batch, precision, int(bool(real)), flags, mult_count)
-    need = lib().dfft_debug_lines_conv_3d_ops(*args, None, 0)
-    if need < 0:
-        raise DfftError(f"dfft_debug_lines_conv_3d_ops failed ({need}): " + lib().dfft_last_error().decode())
-    buf = ctypes.create_string_buffer(int(need))
-    lib().dfft_debug_lines_conv_3d_ops(*args, buf, need)
-    return json.loads(buf.value.decode())
+    return _json_hook(lib().dfft_debug_lines_conv_3d_ops, nx, ny, nz, batch, precision, int(bool(real)), flags, mult_count)
 
 
 def lines_conv_2d_ops(nx, ny, batch, precision=DOUBLE, real=False, flags=0, mult_count=1):
     """passes LinesConvolvePlan(two_d=(nx, ny, batch), ...) would launch per execute (host-only test hook, see
     dfft_debug_lines_conv_2d_ops; buffers as lines_conv_3d_ops); read DFFT_NO_PLANE / DFFT_FORCE_PLANE / DFFT_GENERIC at the
     call, as plan creation does"""
-    import json
-    args = (nx, ny, batch, precision, int(bool(real)), flags, mult_count)
-    need = lib().dfft_debug_lines_conv_2d_ops(*args, None, 0)
-    if need < 0:
-        raise DfftError(f"dfft_debug_lines_conv_2d_ops failed ({need}): " + lib().dfft_last_error().decode())
-    buf = ctypes.create_string_buffer(int(need))
-    lib().dfft_debug_lines_conv_2d_ops(*args, buf, need)
-    return json.loads(buf.value.decode())
+    return _json_hook(lib().dfft_debug_lines_conv_2d_ops, nx, ny, batch, precision, int(bool(real)), flags, mult_count)
 
 
 def real_lines_ops(n, nlines, direction, precision=DOUBLE, two_d=None):
     """passes a RealLinesPlan(n, nlines, precision, two_d) would launch for `direction` (host-only test hook, see
     dfft_debug_real_lines_ops)"""
-    import json
     args = (two_d[0], two_d[1], two_d[2], precision, direction, 1) if two_d is not None else (n, 1, nlines, precision, direction, 0)
-    need = lib().dfft_debug_real_lines_ops(*args, None, 0)
-    if need < 0:
-        raise DfftError(f"dfft_debug_real_lines_ops failed ({need}): " + lib().dfft_last_error().decode())
-    buf = ctypes.create_string_buffer(int(need))
-    lib().dfft_debug_real_lines_ops(*args, buf, need)
-    return json.loads(buf.value.decode())
+    return _json_hook(lib().dfft_debug_real_lines_ops, *args)
 
 
 def lines_3d_ops(nx, ny, nz, batch, direction, precision=DOUBLE, real=False):
     """passes LinesPlan(three_d=...) / RealLinesPlan(three_d=...) would launch for `direction` (host-only test hook, see
     dfft_debug_lines_3d_ops); read DFFT_NO_PLANE / DFFT_FORCE_PLANE / DFFT_GENERIC at the call, as plan creation does"""
-    import json
-    args = (nx, ny, nz, batch, precision, direction, int(bool(real)))
-    need = lib().dfft_debug_lines_3d_ops(*args, None, 0)
-    if need < 0:
-        raise DfftError(f"dfft_debug_lines_3d_ops failed ({need}): " + lib().dfft_last_error().decode())
-    buf = ctypes.create_string_buffer(int(need))
-    lib().dfft_debug_lines_3d_ops(*args, buf, need)
-    return json.loads(buf.value.decode())
+    return _json_hook(lib().dfft_debug_lines_3d_ops, nx, ny, nz, batch, precision, direction, int(bool(real)))
 
 
 def lines_ops(n, stride, nlines, inner, inner_dist, outer_dist, direction, precision=DOUBLE, two_d=False):
     """passes a lines plan would launch (host-only test hook, see dfft_debug_lines_ops)"""
-    import json
-    need = lib().dfft_debug_lines_ops(n, stride, nlines, inner, inner_dist, outer_dist, precision, direction, int(two_d), None, 0)
-    if need < 0:
-        raise DfftError("dfft_debug_lines_ops: " + lib().dfft_last_error().decode())
-    buf = ctypes.create_string_buffer(int(need))
-    lib().dfft_debug_lines_ops(n, stride, nlines, inner, inner_dist, outer_dist, precision, direction, int(two_d), buf, need)
-    return json.loads(buf.value.decode())
+    return _json_hook(lib().dfft_debug_lines_ops, n, stride, nlines, inner, inner_dist, outer_dist, precision, direction, int(two_d))
 
 
 def _debug_op(rec):

@@ -9,6 +9,7 @@
 #include <dlfcn.h>
 
 #include <algorithm>
+#include <cassert>
 #include <atomic>
 #include <cmath>
 #include <condition_variable>
@@ -564,11 +565,6 @@ template <typename T> static cudaError_t upload_lut_kind(void** dst, const SizeE
     if (kind == PK_Z) return upload_lut<T>(dst, e->z_nstages, e->z_rad);
     if (kind == PK_XF || kind == PK_XB || kind == PK_XB_CO || kind == PK_XF_TW) return upload_lut<T>(dst, e->x_nstages, e->x_rad);
     return upload_lut<T>(dst, e->s_nstages, e->s_rad);
-}
-
-template <typename T> static void upload_lut_e(void** dst, const SizeEntry* e, bool contiguous)
-{
-    upload_lut_kind<T>(dst, e, contiguous ? PK_Z : PK_Y);
 }
 
 static int share_pointer(dfft_plan p, void* mine, std::vector<void*>& peers)
@@ -2379,109 +2375,93 @@ extern "C" void* dfft_plan_stream(dfft_plan p) { return p ? (void*)p->stream : n
 // batched local transforms: plan / launch / delete, the templateFFT engine surface
 // (3dmpifft_opt/include/templateFFT.h:361-365 initializeFFT / launchFFTKernel / deleteFFT)
 // ------------------------------------------------------------------------------------------------
+// launches of the lines engine beyond the pass kinds: X + Y of whole e->N x e->N planes in one launch of e->plane (PlaneArgs),
+// and the whole 2-D convolution of whole images in one launch of e->plane_conv (PlaneConvArgs)
+enum { LK_PLANE = PK_COUNT, LK_PLANE_CONV };
+enum { LB_IN = 0, LB_TEMP = 1, LB_OUT = 2 };
 struct LinePass {
     const SizeEntry* e = nullptr;
-    int kind = PK_Z;
+    int kind = PK_Z;             // a PassKind, LK_PLANE or LK_PLANE_CONV
     void* lut = nullptr;
-    Affine ia{}, oa{};
+    Affine ia{}, oa{};           // plane kinds, for the records: plane (image), 0, row and point strides
     int G = 0, W = 0;
-    long long ntiles = 0;
+    long long ntiles = 0;        // plane kinds: planes (images)
     long long tw_n = 0;          // four-step twiddle modulus (PK_XF_TW)
-    int src = 0, dst = 0;        // LB_IN (the caller's data / a real plan's `in`), LB_TEMP (the plan's temporary), LB_OUT
+    int src = LB_IN, dst = LB_IN;   // LB_IN (the caller's data / a real or convolve plan's `in`), LB_TEMP (the plan's temporary), LB_OUT
     long long ld_in = 0, ld_out = 0;   // PK_Z_R2C / PK_Z_C2R: distance between the two lines of a pair (RealZArgs), each side's elements
-    bool plane = false;          // X + Y of ntiles whole e->N x e->N planes in one launch of e->plane (PlaneArgs); `kind` unused,
-                                 // except that kind == PK_XCONV is the whole 2-D convolution of ntiles images in one launch of
-                                 // e->plane_conv (PlaneConvArgs)
-    bool inv = false;            // convolve plans: this pass runs the inverse transform
+    bool inv = false;            // the inverse transform
 };
-enum { LB_IN = 0, LB_TEMP = 1, LB_OUT = 2 };
+// which execute runs a plan: dfft_lines_execute, dfft_lines_execute_real or dfft_lines_execute_convolve
+enum LinesForm { LF_COMPLEX, LF_REAL, LF_CONV };
 struct dfft_lines_plan_s {
-    int prec = 0, device = 0, sms = 132, npass = 0;
-    bool ordered = false;        // passes run in the same order for both directions (four-step)
+    int prec = 0, device = 0, sms = 132;
+    LinesForm form = LF_COMPLEX;
+    // the passes of one execute in order, [0] forward, [1] backward (a convolve plan has one list, [0]).  The create path launches
+    // them and the dfft_debug_lines*_ops hooks record them, both through line_pass
+    LinePass run[2][5];
+    int nrun[2] = {0, 0};
     void* temp = nullptr;
-    LinePass pass[3];
-    // real plans (dfft_lines_plan_create_r2c[_2d|_3d]): the passes of each direction in execution order, [0] forward, [1] backward;
-    // `pass` stays empty.  Read by dfft_lines_execute_real and dfft_debug_real_lines_ops alike
-    bool real = false;
-    int nreal = 0;
-    LinePass rpass[2][3];
+    size_t temp_bytes = 0;       // the temporary a plan needs, allocated by lines_create
+    struct Lut { const SizeEntry* e; int kind; void* d; };
+    std::vector<Lut> luts;       // twiddle tables, one per (entry, schedule), shared by the passes that run it
     long long rcount = 0, ccount = 0;   // reals and complex elements of the caller's real / complex buffer
-    // convolve plans (dfft_lines_plan_create_convolve_[r2c_]{2d,3d}): the passes of one execute in order, the multiply folded
-    // into the PK_XCONV pass; `pass` and `rpass` stay empty.  Read by dfft_lines_execute_convolve and the
-    // dfft_debug_lines_conv_{2d,3d}_ops hooks alike.  Inverse passes share their forward pass's twiddle table
-    bool conv = false;
-    int nconv = 0;
-    LinePass cpass[5];
-    long long batch = 0, mvol = 0;   // volumes (images); complex elements of one volume's (image's) multiplier
+    long long batch = 0, mvol = 0;   // convolve: volumes (images); complex elements of one volume's (image's) multiplier
     double scale = 0;                // DFFT_SCALE_BACKWARD: 1 / (elements of a volume or image), folded into the multiply; 0 = unnormalised
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[2] = {nullptr, nullptr};
-    bool timed = false;
 };
 
-// a * b * c < 2^31 (the kernels' 32-bit row counts TileArgs::W / G), without overflow for any non-negative arguments.  Column
-// counts need no check: a strided pass's columns (nx*ny, ny*(nx/2+1)) are below 2^25 for every supported length
-static bool fits_int(long long a, long long b, long long c = 1)
+static bool bad_precision(int precision) { return precision != DFFT_DOUBLE && precision != DFFT_FLOAT; }
+
+// a * b * c < 2^31 (the kernels' 32-bit row counts TileArgs::W / G), without overflow for any non-negative arguments
+static bool fits_int(long long a, long long b = 1, long long c = 1)
 {
     return (__int128)a * b * c <= 0x7fffffff;
 }
 
+// the plain pass kind whose tile size (kind_C) and twiddle schedule (upload_lut_kind) a lines pass has: the real kernels run the
+// contiguous configuration, the column convolve the strided one, and the plane kernels the contiguous schedule
+static int plain_kind(int kind)
+{
+    return kind == PK_XCONV ? PK_Y : (kind == PK_Z_R2C || kind == PK_Z_C2R || kind >= PK_COUNT) ? PK_Z : kind;
+}
+
+// one pass over `nlines` lines of n points: densely packed contiguous lines (stride 1, PK_Z) or columns (inner_dist 1, PK_Y).
+// The pass's row or column count W is a 32-bit kernel argument
 static int make_line_pass(LinePass& lp, int n, long long stride, long long nlines, long long inner, long long inner_dist, long long outer_dist,
-                          int precision, bool dry = false)
+                          int precision)
 {
     const SizeEntry* e = find_size_entry(n, precision);
     if (!e) return fail(DFFT_EUNSUPPORTED, "unsupported length %d", n);
     lp.e = e;
     if (stride == 1) {
         if (inner_dist != n || (inner != nlines && outer_dist != inner * n)) return fail(DFFT_EUNSUPPORTED, "contiguous lines must be densely packed");
+        if (!fits_int(nlines)) return fail(DFFT_EUNSUPPORTED, "%lld rows: at most 2^31 - 1 per plan", nlines);
         const int C = e->z_C;
-        lp.G = (int)cdiv(nlines, C); lp.W = (int)std::min<long long>(nlines, 0x7fffffff); lp.ntiles = lp.G;
+        lp.G = (int)cdiv(nlines, C); lp.W = (int)nlines; lp.ntiles = lp.G;
         lp.ia = Affine{0, (long long)C * n, n, 1};
         lp.oa = lp.ia;
         lp.kind = PK_Z;
     } else {
         if (inner_dist != 1 || inner < 1 || nlines % inner) return fail(DFFT_EUNSUPPORTED, "strided lines must be columns (inner_dist == 1)");
+        if (!fits_int(inner)) return fail(DFFT_EUNSUPPORTED, "%lld columns: at most 2^31 - 1 per pass", inner);
         const int C = e->s_C;
         lp.G = (int)cdiv(inner, C); lp.W = (int)inner; lp.ntiles = (nlines / inner) * lp.G;
         lp.ia = Affine{outer_dist, C, 1, stride};
         lp.oa = lp.ia;
         lp.kind = PK_Y;
     }
-    if (dry) return 0;
-    if (precision == DFFT_DOUBLE) upload_lut_e<double>(&lp.lut, e, stride == 1);
-    else upload_lut_e<float>(&lp.lut, e, stride == 1);
-    if (cudaGetLastError() != cudaSuccess || !lp.lut) return fail(DFFT_ECUDA, "twiddle table upload failed");
     return 0;
 }
 
-static int lines_plan_common(dfft_lines_plan p, int precision)
+// complex plans: the backward list is the forward list inverted, in reverse order (ordered, four-step: in the same order)
+static int complex_lists(dfft_lines_plan p, int n, bool ordered)
 {
-    p->prec = precision;
-    CU(cudaGetDevice(&p->device));
-    CU(cudaDeviceGetAttribute(&p->sms, cudaDevAttrMultiProcessorCount, p->device));
-    CU(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
-    for (auto& e : p->ev) CU(cudaEventCreate(&e));
-    return 0;
-}
-
-extern "C" int dfft_lines_destroy(dfft_lines_plan p)
-{
-    if (!p) return 0;
-    cudaSetDevice(p->device);
-    if (p->stream) cudaStreamSynchronize(p->stream);
-    for (auto& lp : p->pass) if (lp.lut) cudaFree(lp.lut);
-    for (auto& dir : p->rpass)
-        for (auto& lp : dir) if (lp.lut) cudaFree(lp.lut);
-    for (int k = 0; k < p->nconv; k++) {
-        bool shared = false;
-        for (int j = 0; j < k; j++) shared |= p->cpass[j].lut == p->cpass[k].lut;
-        if (p->cpass[k].lut && !shared) cudaFree(p->cpass[k].lut);
+    p->nrun[0] = p->nrun[1] = n;
+    for (int k = 0; k < n; k++) {
+        p->run[1][k] = p->run[0][ordered ? k : n - 1 - k];
+        p->run[1][k].inv = true;
     }
-    if (p->temp) cudaFree(p->temp);
-    for (auto& e : p->ev) if (e) cudaEventDestroy(e);
-    if (p->stream) cudaStreamDestroy(p->stream);
-    cudaGetLastError();
-    delete p;
     return 0;
 }
 
@@ -2491,8 +2471,9 @@ extern "C" int dfft_lines_destroy(dfft_lines_plan p)
 // -- what the reference does with its multi-upload axes and reorderFourStep = 1 (templateFFT.cpp:4007-4106, 5951).
 // Validated against numpy (tests/test_gpu_parity.py::test_four_step_long_lines);
 // DFFT_NO_LONG_LINES=1 restores the "unsupported length" answer.
-static int make_four_step(dfft_lines_plan p, int n, long long nlines, int precision, bool dry = false)
+static int make_four_step(dfft_lines_plan p, int n, long long nlines)
 {
+    const int precision = p->prec;
     long long best1 = 0;
     int best_score = -1;
     for (long long d = 2; d * d <= (long long)n * 4 && d < n; d++) {
@@ -2505,84 +2486,48 @@ static int make_four_step(dfft_lines_plan p, int n, long long nlines, int precis
         if (score > best_score) { best_score = score; best1 = d; }
     }
     if (!best1) return fail(DFFT_EUNSUPPORTED, "length %d cannot be split into two supported factors", n);
+    if (!fits_int(nlines)) return fail(DFFT_EUNSUPPORTED, "%lld rows: at most 2^31 - 1 per plan", nlines);
     const int n1 = (int)best1, n2 = n / n1;
-    const size_t esz = precision == DFFT_FLOAT ? 8 : 16;
-    if (dry) p->temp = fake_addr(0, 4);
-    else CU(cudaMalloc(&p->temp, (size_t)nlines * n * esz));
+    p->temp_bytes = (size_t)nlines * n * (precision == DFFT_FLOAT ? 8 : 16);
     // pass A: columns of the [n1][n2] matrix of every line, transposed store + twiddle
-    LinePass& a = p->pass[0];
+    LinePass& a = p->run[0][0];
     a.e = find_size_entry(n1, precision);
-    {
-        const int C = a.e->x_C;
-        a.G = (int)cdiv(n2, C); a.W = n2; a.ntiles = nlines * a.G;
-        a.ia = Affine{(long long)n, C, 1, n2};
-        a.oa = Affine{(long long)n, (long long)C * n1, n1, 1};
-        a.kind = PK_XF_TW; a.tw_n = n; a.src = 0; a.dst = 1;
-        if (dry) {}
-        else if (precision == DFFT_DOUBLE) upload_lut<double>(&a.lut, a.e->x_nstages, a.e->x_rad);
-        else upload_lut<float>(&a.lut, a.e->x_nstages, a.e->x_rad);
-    }
+    const int CA = a.e->x_C;
+    a.G = (int)cdiv(n2, CA); a.W = n2; a.ntiles = nlines * a.G;
+    a.ia = Affine{(long long)n, CA, 1, n2};
+    a.oa = Affine{(long long)n, (long long)CA * n1, n1, 1};
+    a.kind = PK_XF_TW; a.tw_n = n; a.src = LB_IN; a.dst = LB_TEMP;
     // pass B: columns of the [n2][n1] matrix in temp, natural-order result in the caller's buffer
-    LinePass& b = p->pass[1];
+    LinePass& b = p->run[0][1];
     b.e = find_size_entry(n2, precision);
-    {
-        const int C = b.e->s_C;
-        b.G = (int)cdiv(n1, C); b.W = n1; b.ntiles = nlines * b.G;
-        b.ia = Affine{(long long)n, C, 1, n1};
-        b.oa = b.ia;
-        b.kind = PK_Y; b.src = 1; b.dst = 0;
-        if (dry) {}
-        else if (precision == DFFT_DOUBLE) upload_lut<double>(&b.lut, b.e->s_nstages, b.e->s_rad);
-        else upload_lut<float>(&b.lut, b.e->s_nstages, b.e->s_rad);
-    }
-    if (!dry && (cudaGetLastError() != cudaSuccess || !a.lut || !b.lut)) return fail(DFFT_ECUDA, "twiddle table upload failed");
-    p->npass = 2;
-    p->ordered = true;
-    return 0;
+    const int CB = b.e->s_C;
+    b.G = (int)cdiv(n1, CB); b.W = n1; b.ntiles = nlines * b.G;
+    b.ia = Affine{(long long)n, CB, 1, n1};
+    b.oa = b.ia;
+    b.kind = PK_Y; b.src = LB_TEMP; b.dst = LB_IN;
+    return complex_lists(p, 2, true);
 }
 
-extern "C" int dfft_lines_plan_create(int n, long long stride, long long nlines, long long inner, long long inner_dist, long long outer_dist,
-                                      int precision, dfft_lines_plan* out)
+// 1-D lines in place (dfft_lines_plan_create): one pass, or, for a contiguous length beyond one shared-memory line and long_lines,
+// the four-step pair
+static int make_lines_1d(dfft_lines_plan p, int n, long long stride, long long nlines, long long inner, long long inner_dist, long long outer_dist,
+                         bool long_lines)
 {
-    if (!out) return fail(DFFT_EINVAL, "null plan pointer");
-    *out = nullptr;
-    if (n < 1 || nlines < 0 || stride < 1 || (precision != DFFT_DOUBLE && precision != DFFT_FLOAT)) return fail(DFFT_EINVAL, "bad arguments");
-    dfft_lines_plan p = new dfft_lines_plan_s;
-    int rc = lines_plan_common(p, precision);
-    const char* nolong = getenv("DFFT_NO_LONG_LINES");
-    if (!rc && !find_size_entry(n, precision) && stride == 1 && inner_dist == n && !(nolong && atoi(nolong) != 0)) {
-        rc = make_four_step(p, n, nlines, precision);
-    } else {
-        if (!rc) rc = make_line_pass(p->pass[0], n, stride, nlines, inner, inner_dist, outer_dist, precision);
-        p->npass = 1;
-    }
-    if (rc) { dfft_lines_destroy(p); return rc; }
-    *out = p;
-    return 0;
+    if (n < 1 || nlines < 0 || stride < 1 || bad_precision(p->prec)) return fail(DFFT_EINVAL, "bad arguments");
+    if (long_lines && !find_size_entry(n, p->prec) && stride == 1 && inner_dist == n) return make_four_step(p, n, nlines);
+    const int rc = make_line_pass(p->run[0][0], n, stride, nlines, inner, inner_dist, outer_dist, p->prec);
+    return rc ? rc : complex_lists(p, 1, false);
 }
 
 // batch ny x nx matrices (nx fastest), in place: X along the batch*ny rows, Y over the nx columns of every matrix (stride nx);
 // backward in reverse
-static int make_lines_2d(dfft_lines_plan p, int nx, int ny, long long batch, int precision, bool dry)
+static int make_lines_2d(dfft_lines_plan p, int nx, int ny, long long batch)
 {
-    int rc = make_line_pass(p->pass[0], nx, 1, (long long)ny * batch, (long long)ny * batch, nx, 0, precision, dry);
-    if (!rc) rc = make_line_pass(p->pass[1], ny, nx, (long long)nx * batch, nx, 1, (long long)nx * ny, precision, dry);
-    p->npass = 2;
-    return rc;
-}
-
-/* batch of 2-D transforms, nx fastest: the reference's FFTdim = 2 application (Test_2D.cpp: size = {X, Y, Z}) */
-extern "C" int dfft_lines_plan_create_2d(int nx, int ny, long long batch, int precision, dfft_lines_plan* out)
-{
-    if (!out) return fail(DFFT_EINVAL, "null plan pointer");
-    *out = nullptr;
-    if (nx < 1 || ny < 1 || batch < 0 || (precision != DFFT_DOUBLE && precision != DFFT_FLOAT)) return fail(DFFT_EINVAL, "bad arguments");
-    dfft_lines_plan p = new dfft_lines_plan_s;
-    int rc = lines_plan_common(p, precision);
-    if (!rc) rc = make_lines_2d(p, nx, ny, batch, precision, false);
-    if (rc) { dfft_lines_destroy(p); return rc; }
-    *out = p;
-    return 0;
+    if (nx < 1 || ny < 1 || batch < 0 || bad_precision(p->prec)) return fail(DFFT_EINVAL, "bad arguments");
+    if (!fits_int(ny, batch)) return fail(DFFT_EUNSUPPORTED, "%d x %lld rows: at most 2^31 - 1 per plan", ny, batch);
+    int rc = make_line_pass(p->run[0][0], nx, 1, (long long)ny * batch, (long long)ny * batch, nx, 0, p->prec);
+    if (!rc) rc = make_line_pass(p->run[0][1], ny, nx, (long long)nx * batch, nx, 1, (long long)nx * ny, p->prec);
+    return rc ? rc : complex_lists(p, 2, false);
 }
 
 static bool env_on(const char* name)
@@ -2595,119 +2540,26 @@ static bool env_on(const char* name)
 // nx), Z over the nx*ny columns of every volume (stride nx*ny); backward in reverse.  Where nx == ny and the entry has a plane
 // kernel that is the default for its shape (plane_default; DFFT_FORCE_PLANE=1: wherever instantiated), X and Y are one launch
 // of it over the batch*nz planes.  DFFT_NO_PLANE=1 keeps the separate passes.  Read at plan creation
-static int make_lines_3d(dfft_lines_plan p, int nx, int ny, int nz, long long batch, int precision, bool dry)
+static int make_lines_3d(dfft_lines_plan p, int nx, int ny, int nz, long long batch)
 {
-    if (nx < 1 || ny < 1 || nz < 1 || batch < 0 || (precision != DFFT_DOUBLE && precision != DFFT_FLOAT)) return fail(DFFT_EINVAL, "bad arguments");
+    const int precision = p->prec;
+    if (nx < 1 || ny < 1 || nz < 1 || batch < 0 || bad_precision(precision)) return fail(DFFT_EINVAL, "bad arguments");
     if (!fits_int(ny, nz, batch)) return fail(DFFT_EUNSUPPORTED, "%d x %d x %lld rows: at most 2^31 - 1 per plan", ny, nz, batch);
     const long long planes = (long long)nz * batch, rows = planes * ny, plane = (long long)nx * ny;
     const SizeEntry* ex = find_size_entry(nx, precision);
     const bool use_plane = ex && nx == ny && ex->plane && !env_on("DFFT_NO_PLANE") && (plane_default(nx, precision) || env_on("DFFT_FORCE_PLANE"));
+    LinePass* f = p->run[0];
     int rc = 0, k = 0;
     if (use_plane) {
-        LinePass& lp = p->pass[k++];
-        lp.e = ex; lp.plane = true; lp.ntiles = planes;
-        lp.ia = lp.oa = Affine{plane, 0, nx, 1};   // for the records: plane, row and point strides
-        if (!dry) {
-            if (precision == DFFT_DOUBLE) upload_lut_e<double>(&lp.lut, ex, true);
-            else upload_lut_e<float>(&lp.lut, ex, true);
-            if (cudaGetLastError() != cudaSuccess || !lp.lut) return fail(DFFT_ECUDA, "twiddle table upload failed");
-        }
+        LinePass& lp = f[k++];
+        lp.e = ex; lp.kind = LK_PLANE; lp.ntiles = planes;
+        lp.ia = lp.oa = Affine{plane, 0, nx, 1};
     } else {
-        rc = make_line_pass(p->pass[k++], nx, 1, rows, rows, nx, 0, precision, dry);
-        if (!rc) rc = make_line_pass(p->pass[k++], ny, nx, nx * planes, nx, 1, plane, precision, dry);
+        rc = make_line_pass(f[k++], nx, 1, rows, rows, nx, 0, precision);
+        if (!rc) rc = make_line_pass(f[k++], ny, nx, nx * planes, nx, 1, plane, precision);
     }
-    if (!rc) rc = make_line_pass(p->pass[k++], nz, plane, plane * batch, plane, 1, plane * nz, precision, dry);
-    if (rc) return rc;
-    p->npass = k;
-    return 0;
-}
-
-extern "C" int dfft_lines_plan_create_3d(int nx, int ny, int nz, long long batch, int precision, dfft_lines_plan* out)
-{
-    if (!out) return fail(DFFT_EINVAL, "null plan pointer");
-    *out = nullptr;
-    if (precision != DFFT_DOUBLE && precision != DFFT_FLOAT) return fail(DFFT_EINVAL, "bad arguments");
-    dfft_lines_plan p = new dfft_lines_plan_s;
-    int rc = lines_plan_common(p, precision);
-    if (!rc) rc = make_lines_3d(p, nx, ny, nz, batch, precision, false);
-    if (rc) { dfft_lines_destroy(p); return rc; }
-    *out = p;
-    return 0;
-}
-
-template <typename T> static int lines_execute_impl(dfft_lines_plan p, void* data, int direction)
-{
-    CU(cudaEventRecord(p->ev[0], p->stream));
-    for (int k = 0; k < p->npass; k++) {
-        const LinePass& lp = p->pass[(direction == DFFT_BACKWARD && !p->ordered) ? p->npass - 1 - k : k];
-        if (lp.ntiles <= 0) continue;
-        cudaError_t err;
-        if (lp.plane) {
-            const PlaneArgs<T> pa{(const cx<T>*)data, (cx<T>*)data, (const cx<T>*)lp.lut, lp.ntiles, direction == DFFT_BACKWARD ? 1 : 0};
-            err = lp.e->plane(&pa, p->sms, p->stream);
-        } else {
-            TileArgs<T> a{};
-            a.in = (const cx<T>*)(lp.src ? p->temp : data); a.out = (cx<T>*)(lp.dst ? p->temp : data); a.lut = (const cx<T>*)lp.lut;
-            a.ia = lp.ia; a.oa = lp.oa; a.G = lp.G; a.W = lp.W; a.ntiles = lp.ntiles;
-            a.inv = direction == DFFT_BACKWARD; a.gen = lp.e->gen; a.tw_n = lp.tw_n;
-            err = lp.e->launch[lp.kind](&a, p->sms, p->stream);
-        }
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "line pass launch failed: %s", cudaGetErrorString(err));
-    }
-    CU(cudaEventRecord(p->ev[1], p->stream));
-    p->timed = true;
-    return 0;
-}
-
-extern "C" int dfft_lines_execute(dfft_lines_plan p, void* data, int direction)
-{
-    if (!p || !data || (direction != DFFT_FORWARD && direction != DFFT_BACKWARD)) return fail(DFFT_EINVAL, "bad arguments");
-    if (p->conv) return fail(DFFT_EINVAL, "a convolve lines plan runs with dfft_lines_execute_convolve");
-    if (p->real) return fail(DFFT_EINVAL, "a real lines plan runs with dfft_lines_execute_real");
-    CU(cudaSetDevice(p->device));
-    return p->prec == DFFT_DOUBLE ? lines_execute_impl<double>(p, data, direction) : lines_execute_impl<float>(p, data, direction);
-}
-
-extern "C" int dfft_lines_synchronize(dfft_lines_plan p)
-{
-    if (!p) return fail(DFFT_EINVAL, "null plan");
-    CU(cudaSetDevice(p->device));
-    CU(cudaStreamSynchronize(p->stream));
-    return 0;
-}
-
-extern "C" void* dfft_lines_stream(dfft_lines_plan p) { return p ? (void*)p->stream : nullptr; }
-
-/* test hook (host only): the passes a lines plan would launch for `direction`, as JSON (same format as dfft_debug_plan_ops;
- * the caller's data is buffer 1 of device 0, the plan's temporary buffer 4); two_d != 0: 2-D plan (n = nx, stride = ny,
- * nlines = batch).  Long lines always use the four-step plan here.  Returns the bytes needed, < 0 on error. */
-extern "C" long long dfft_debug_lines_ops(int n, long long stride, long long nlines, long long inner, long long inner_dist, long long outer_dist,
-                                          int precision, int direction, int two_d, char* buf, long long cap)
-{
-    dfft_lines_plan_s lp;
-    std::vector<std::string> ops;
-    lp.prec = precision;
-    int rc = 0;
-    if (two_d) {
-        rc = make_lines_2d(&lp, n, (int)stride, nlines, precision, true);
-    } else if (!find_size_entry(n, precision) && stride == 1 && inner_dist == n) {
-        rc = make_four_step(&lp, n, nlines, precision, true);
-    } else {
-        rc = make_line_pass(lp.pass[0], n, stride, nlines, inner, inner_dist, outer_dist, precision, true);
-        lp.npass = 1;
-    }
-    if (rc) return rc;
-    for (int k = 0; k < lp.npass; k++) {
-        const LinePass& ps = lp.pass[(direction == DFFT_BACKWARD && !lp.ordered) ? lp.npass - 1 - k : k];
-        TileArgs<double> a{};
-        a.in = (const double2*)(ps.src ? lp.temp : fake_addr(0, 1)); a.out = (double2*)(ps.dst ? lp.temp : fake_addr(0, 1));
-        a.ia = ps.ia; a.oa = ps.oa; a.G = ps.G; a.W = ps.W; a.ntiles = ps.ntiles;
-        a.inv = direction == DFFT_BACKWARD; a.tw_n = ps.tw_n;
-        const int C = ps.kind == PK_Z ? ps.e->z_C : (ps.kind == PK_Y ? ps.e->s_C : ps.e->x_C);
-        record_op<double>(ops, kPassNames[ps.kind], k, ps.e->N, C, false, false, ps.kind == PK_XF_TW, a);
-    }
-    lp.temp = nullptr;
-    return ops_json(ops, buf, cap);
+    if (!rc) rc = make_line_pass(f[k++], nz, plane, plane * batch, plane, 1, plane * nz, precision);
+    return rc ? rc : complex_lists(p, k, false);
 }
 
 // ---- real lines: R2C / C2R over densely packed lines (1-D) and the rows of row-major matrices (2-D) --------------------------
@@ -2728,10 +2580,10 @@ static void make_real_pass(LinePass& lp, const SizeEntry* e, long long nlines, b
 
 // 1-D: `batch` lines of n points (ny, nz unused).  2-D: `batch` ny x n matrices, rows real <-> rows of n/2+1 complex points.
 // 3-D: `batch` nz x ny x n volumes, likewise
-static int make_real_lines(dfft_lines_plan p, int n, int ny, int nz, long long batch, int precision, int dims, bool dry)
+static int make_real_lines(dfft_lines_plan p, int n, int ny, int nz, long long batch, int dims)
 {
-    if (batch < 0 || (dims >= 2 && ny < 1) || (dims == 3 && nz < 1) || (precision != DFFT_DOUBLE && precision != DFFT_FLOAT))
-        return fail(DFFT_EINVAL, "bad arguments");
+    const int precision = p->prec;
+    if (batch < 0 || (dims >= 2 && ny < 1) || (dims == 3 && nz < 1) || bad_precision(precision)) return fail(DFFT_EINVAL, "bad arguments");
     const SizeEntry* e = n < 2 ? nullptr : find_size_entry(n, precision);
     if (!e) return fail(DFFT_EUNSUPPORTED, "real lines of %d points: the length must be 2..13-smooth and fit one shared-memory line", n);
     if (!e->launch[PK_Z_R2C] || !e->launch[PK_Z_C2R]) return fail(DFFT_EUNSUPPORTED, "the kernel entry of length %d has no real-data kernels", n);
@@ -2739,188 +2591,33 @@ static int make_real_lines(dfft_lines_plan p, int n, int ny, int nz, long long b
     if (!fits_int(my, mz, batch)) return fail(DFFT_EUNSUPPORTED, "%lld x %lld x %lld real lines: at most 2^31 - 1 per plan", my, mz, batch);
     const long long rows = my * mz * batch;
     const long long H = n / 2 + 1;
-    p->real = true;
-    p->prec = precision;
+    p->form = LF_REAL;
     p->rcount = rows * n;
     p->ccount = rows * H;
-    LinePass* f = p->rpass[0];
-    LinePass* b = p->rpass[1];
+    LinePass* f = p->run[0];
+    LinePass* b = p->run[1];
     make_real_pass(f[0], e, rows, true, LB_IN, LB_OUT);
     if (dims == 1) {
         make_real_pass(b[0], e, rows, false, LB_IN, LB_OUT);
-        p->nreal = 1;
     } else {
         // along ny: the H columns of every half-spectrum matrix, matrices ny*H apart; along nz (3-D): the ny*H columns of every
         // volume, volumes nz*ny*H apart.  Forward in place in `out` after the real pass; backward the strided passes in reverse,
         // the first from `in` into the temporary, so that `in` is never written, the rest in place there
         const int ns = dims - 1;   // strided passes: f[1..ns] forward, b[0..ns-1] backward (the same passes in reverse)
-        auto along_y = [&](LinePass& lp) { return make_line_pass(lp, ny, H, H * mz * batch, H, 1, H * ny, precision, dry); };
-        auto along_z = [&](LinePass& lp) { return make_line_pass(lp, nz, H * ny, H * ny * batch, H * ny, 1, H * ny * nz, precision, dry); };
-        int rc = along_y(f[1]);
-        if (!rc) rc = along_y(b[ns - 1]);
-        if (!rc && dims == 3) rc = along_z(f[2]);
-        if (!rc && dims == 3) rc = along_z(b[0]);
+        int rc = make_line_pass(f[1], ny, H, H * mz * batch, H, 1, H * ny, precision);
+        if (!rc && dims == 3) rc = make_line_pass(f[2], nz, H * ny, H * ny * batch, H * ny, 1, H * ny * nz, precision);
         if (rc) return rc;
-        for (int k = 0; k < ns; k++) { b[k].src = k == 0 ? LB_IN : LB_TEMP; b[k].dst = LB_TEMP; }
-        for (int k = 1; k <= ns; k++) f[k].src = f[k].dst = LB_OUT;
+        for (int k = 1; k <= ns; k++) {
+            f[k].src = f[k].dst = LB_OUT;
+            b[ns - k] = f[k];
+            b[ns - k].src = k == ns ? LB_IN : LB_TEMP; b[ns - k].dst = LB_TEMP;
+        }
         make_real_pass(b[ns], e, rows, false, LB_TEMP, LB_OUT);
-        p->nreal = dims;
-        const size_t esz = precision == DFFT_FLOAT ? 8 : 16;
-        if (dry) p->temp = fake_addr(0, 4);
-        else if (p->ccount > 0) CU(cudaMalloc(&p->temp, (size_t)p->ccount * esz));
+        p->temp_bytes = (size_t)p->ccount * (precision == DFFT_FLOAT ? 8 : 16);
     }
-    if (dry) return 0;
-    for (auto& dir : p->rpass)
-        for (int k = 0; k < p->nreal; k++) {
-            LinePass& lp = dir[k];
-            if (lp.kind != PK_Z_R2C && lp.kind != PK_Z_C2R) continue;
-            if (precision == DFFT_DOUBLE) upload_lut_e<double>(&lp.lut, e, true);
-            else upload_lut_e<float>(&lp.lut, e, true);
-            if (!lp.lut) break;
-        }
-    if (cudaGetLastError() != cudaSuccess || !f[0].lut || !b[p->nreal - 1].lut) return fail(DFFT_ECUDA, "twiddle table upload failed");
+    p->nrun[0] = p->nrun[1] = dims;
+    for (int k = 0; k < dims; k++) b[k].inv = true;
     return 0;
-}
-
-static inline void* line_buf(int which, const void* in, void* out, void* temp)
-{
-    return which == LB_TEMP ? temp : (which == LB_OUT ? out : const_cast<void*>(in));
-}
-
-// the kernel arguments of one pass of a real plan (a C2C pass uses r.t alone)
-template <typename T> static void real_line_args(const LinePass& lp, const void* src, void* dst, int direction, RealZArgs<T>& r)
-{
-    TileArgs<T>& a = r.t;
-    a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)lp.lut;
-    a.ia = lp.ia; a.oa = lp.oa; a.G = lp.G; a.W = lp.W; a.ntiles = lp.ntiles;
-    a.inv = direction == DFFT_BACKWARD; a.gen = lp.e->gen; a.tw_n = lp.tw_n;
-    r.rin = (const T*)src; r.rout = (T*)dst;
-    r.ld_in = lp.ld_in; r.ld_out = lp.ld_out;
-}
-
-static int real_plan_create(int n, int ny, int nz, long long batch, int precision, int dims, dfft_lines_plan* out)
-{
-    if (!out) return fail(DFFT_EINVAL, "null plan pointer");
-    *out = nullptr;
-    dfft_lines_plan p = new dfft_lines_plan_s;
-    int rc = lines_plan_common(p, precision);
-    if (!rc) rc = make_real_lines(p, n, ny, nz, batch, precision, dims, false);
-    if (rc) { dfft_lines_destroy(p); return rc; }
-    *out = p;
-    return 0;
-}
-
-extern "C" int dfft_lines_plan_create_r2c(int n, long long nlines, int precision, dfft_lines_plan* plan)
-{
-    return real_plan_create(n, 1, 1, nlines, precision, 1, plan);
-}
-
-extern "C" int dfft_lines_plan_create_r2c_2d(int nx, int ny, long long batch, int precision, dfft_lines_plan* plan)
-{
-    return real_plan_create(nx, ny, 1, batch, precision, 2, plan);
-}
-
-extern "C" int dfft_lines_plan_create_r2c_3d(int nx, int ny, int nz, long long batch, int precision, dfft_lines_plan* plan)
-{
-    return real_plan_create(nx, ny, nz, batch, precision, 3, plan);
-}
-
-template <typename T> static int lines_execute_real_impl(dfft_lines_plan p, const void* in, void* out, int direction)
-{
-    const int d = direction == DFFT_FORWARD ? 0 : 1;
-    CU(cudaEventRecord(p->ev[0], p->stream));
-    for (int k = 0; k < p->nreal; k++) {
-        const LinePass& lp = p->rpass[d][k];
-        if (lp.ntiles <= 0) continue;
-        RealZArgs<T> r{};
-        real_line_args<T>(lp, line_buf(lp.src, in, out, p->temp), line_buf(lp.dst, in, out, p->temp), direction, r);
-        const bool realk = lp.kind == PK_Z_R2C || lp.kind == PK_Z_C2R;
-        cudaError_t err = lp.e->launch[lp.kind](realk ? (const void*)&r : (const void*)&r.t, p->sms, p->stream);
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "real line pass launch failed: %s", cudaGetErrorString(err));
-    }
-    CU(cudaEventRecord(p->ev[1], p->stream));
-    p->timed = true;
-    return 0;
-}
-
-extern "C" int dfft_lines_execute_real(dfft_lines_plan p, const void* in, void* out, int direction)
-{
-    if (!p || !in || !out || (direction != DFFT_FORWARD && direction != DFFT_BACKWARD)) return fail(DFFT_EINVAL, "bad arguments");
-    if (p->conv) return fail(DFFT_EINVAL, "a convolve lines plan runs with dfft_lines_execute_convolve");
-    if (!p->real) return fail(DFFT_EINVAL, "a complex lines plan runs with dfft_lines_execute");
-    const size_t rsz = p->prec == DFFT_FLOAT ? 4 : 8, csz = 2 * rsz;
-    const bool fwd = direction == DFFT_FORWARD;
-    const uintptr_t ri = (uintptr_t)(fwd ? in : out), ci = (uintptr_t)(fwd ? out : in);
-    if (ri % rsz || ci % csz) return fail(DFFT_EINVAL, "a %s buffer is not aligned to its element size", ri % rsz ? "real" : "complex");
-    const uintptr_t a = (uintptr_t)in, b = (uintptr_t)out;
-    const uintptr_t a_end = a + (fwd ? p->rcount * rsz : p->ccount * csz), b_end = b + (fwd ? p->ccount * csz : p->rcount * rsz);
-    if (a == b || (a < b_end && b < a_end)) return fail(DFFT_EINVAL, "`in` and `out` overlap (real lines are out of place)");
-    CU(cudaSetDevice(p->device));
-    return p->prec == DFFT_DOUBLE ? lines_execute_real_impl<double>(p, in, out, direction) : lines_execute_real_impl<float>(p, in, out, direction);
-}
-
-/* test hook (host only): the passes of a real lines plan for `direction`, JSON as dfft_debug_lines_ops; in = buffer 5, out = 2,
- * temporary = 4 of device 0.  Real passes carry "nzh" and "pair" as the 3-D plan's Z_R2C / Z_C2R records */
-extern "C" long long dfft_debug_real_lines_ops(int n, int ny, long long batch, int precision, int direction, int two_d, char* buf, long long cap)
-{
-    if (direction != DFFT_FORWARD && direction != DFFT_BACKWARD) return fail(DFFT_EINVAL, "bad direction");
-    dfft_lines_plan_s lp;
-    std::vector<std::string> ops;
-    const int rc = make_real_lines(&lp, n, ny, 1, batch, precision, two_d ? 2 : 1, true);
-    if (rc) return rc;
-    const int d = direction == DFFT_FORWARD ? 0 : 1;
-    for (int k = 0; k < lp.nreal; k++) {
-        const LinePass& ps = lp.rpass[d][k];
-        RealZArgs<double> r{};
-        real_line_args<double>(ps, line_buf(ps.src, fake_addr(0, 5), fake_addr(0, 2), lp.temp), line_buf(ps.dst, fake_addr(0, 5), fake_addr(0, 2), lp.temp),
-                               direction, r);
-        const bool realk = ps.kind == PK_Z_R2C || ps.kind == PK_Z_C2R;
-        char extra[128] = "";
-        if (realk) snprintf(extra, sizeof(extra), ", \"nzh\": %d, \"pair\": [%lld, %lld]", ps.e->N / 2 + 1, ps.ld_in, ps.ld_out);
-        record_op<double>(ops, kPassNames[ps.kind], k, ps.e->N, realk ? ps.e->z_C : ps.e->s_C, false, false, false, r.t, extra);
-    }
-    lp.temp = nullptr;
-    return ops_json(ops, buf, cap);
-}
-
-/* test hook (host only): the passes of a 3-D lines plan for `direction`, JSON as dfft_debug_lines_ops (complex: the caller's data
- * is buffer 1) or dfft_debug_real_lines_ops (real != 0: in = buffer 5, out = 2, temporary = 4).  The plane kernel's record is
- * "XY_PLANE" with ntiles = planes and ia = oa = [plane, 0, row, point] strides */
-extern "C" long long dfft_debug_lines_3d_ops(int nx, int ny, int nz, long long batch, int precision, int direction, int real, char* buf, long long cap)
-{
-    if (direction != DFFT_FORWARD && direction != DFFT_BACKWARD) return fail(DFFT_EINVAL, "bad direction");
-    dfft_lines_plan_s lp;
-    std::vector<std::string> ops;
-    if (real) {
-        const int rc = make_real_lines(&lp, nx, ny, nz, batch, precision, 3, true);
-        if (rc) return rc;
-        const int d = direction == DFFT_FORWARD ? 0 : 1;
-        for (int k = 0; k < lp.nreal; k++) {
-            const LinePass& ps = lp.rpass[d][k];
-            RealZArgs<double> r{};
-            real_line_args<double>(ps, line_buf(ps.src, fake_addr(0, 5), fake_addr(0, 2), lp.temp), line_buf(ps.dst, fake_addr(0, 5), fake_addr(0, 2), lp.temp),
-                                   direction, r);
-            const bool realk = ps.kind == PK_Z_R2C || ps.kind == PK_Z_C2R;
-            char extra[128] = "";
-            if (realk) snprintf(extra, sizeof(extra), ", \"nzh\": %d, \"pair\": [%lld, %lld]", ps.e->N / 2 + 1, ps.ld_in, ps.ld_out);
-            record_op<double>(ops, kPassNames[ps.kind], k, ps.e->N, realk ? ps.e->z_C : ps.e->s_C, false, false, false, r.t, extra);
-        }
-    } else {
-        lp.prec = precision;
-        const int rc = make_lines_3d(&lp, nx, ny, nz, batch, precision, true);
-        if (rc) return rc;
-        for (int k = 0; k < lp.npass; k++) {
-            const LinePass& ps = lp.pass[direction == DFFT_BACKWARD ? lp.npass - 1 - k : k];
-            TileArgs<double> a{};
-            a.in = (const double2*)fake_addr(0, 1); a.out = (double2*)fake_addr(0, 1);
-            a.ia = ps.ia; a.oa = ps.oa; a.G = ps.G; a.W = ps.W; a.ntiles = ps.ntiles;
-            a.inv = direction == DFFT_BACKWARD;
-            const int C = ps.plane ? ps.e->N : (ps.kind == PK_Z ? ps.e->z_C : ps.e->s_C);
-            record_op<double>(ops, ps.plane ? "XY_PLANE" : kPassNames[ps.kind], k, ps.e->N, C, false, false, false, a);
-        }
-    }
-    lp.temp = nullptr;
-    return ops_json(ops, buf, cap);
 }
 
 // ---- batched 2-D and 3-D spectral convolution on the lines engine: out = ifftn(fftn(in) * m) per image / volume ---------------
@@ -2938,59 +2635,43 @@ extern "C" long long dfft_debug_lines_3d_ops(int nx, int ny, int nz, long long b
 // Everything after the first pass is in place in `out` (C2C) or the plan's temporary (R2C), so `in` is only read and in == out
 // works.  The convolved length (ny in 2-D, nz in 3-D) needs the convolve kernel: a tuned default entry (launch[PK_XCONV], as
 // dfft_plan_convolve_* asks of x)
-static int make_lines_conv(dfft_lines_plan p, int dims, int nx, int ny, int nz, long long batch, int precision, bool real, unsigned flags, bool dry)
+static int make_lines_conv(dfft_lines_plan p, int dims, int nx, int ny, int nz, long long batch, bool real, unsigned flags)
 {
     if (flags & ~DFFT_SCALE_BACKWARD) return fail(DFFT_EINVAL, "convolve lines plans take no flag but DFFT_SCALE_BACKWARD");
-    const int nc = dims == 3 ? nz : ny;   // the convolved axis
-    int rc;
-    if (real) {
-        rc = make_real_lines(p, nx, ny, nz, batch, precision, dims, dry);
-    } else if (dims == 3) {
-        rc = make_lines_3d(p, nx, ny, nz, batch, precision, dry);
-    } else {
-        if (nx < 1 || ny < 1 || batch < 0 || (precision != DFFT_DOUBLE && precision != DFFT_FLOAT)) return fail(DFFT_EINVAL, "bad arguments");
-        if (!fits_int(ny, batch)) return fail(DFFT_EUNSUPPORTED, "%d x %lld rows: at most 2^31 - 1 per plan", ny, batch);
-        rc = make_lines_2d(p, nx, ny, batch, precision, dry);
-    }
+    const int rc = real ? make_real_lines(p, nx, ny, nz, batch, dims) : dims == 3 ? make_lines_3d(p, nx, ny, nz, batch) : make_lines_2d(p, nx, ny, batch);
     if (rc) return rc;
-    LinePass* f = real ? p->rpass[0] : p->pass;   // forward passes in execution order, the convolved axis last
-    const int nf = real ? p->nreal : p->npass;
+    const LinePass* f = p->run[0];   // forward passes in execution order, the convolved axis last
+    const int nf = p->nrun[0];
+    assert(nf >= 2 && nf <= 3);      // X + Y or the plane pass (2-D), then Z (3-D): the list below has 2 * nf - 1 <= 5 passes
     const LinePass& z = f[nf - 1];
     if (z.kind != PK_Y || z.e->gen || !z.e->launch[PK_XCONV])
         return fail(DFFT_EUNSUPPORTED, "the %c length %d has no convolution kernel (it needs a tuned length, dfft_length_kind == 2, of the default kernel table)",
-                    dims == 3 ? 'z' : 'y', nc);
+                    dims == 3 ? 'z' : 'y', dims == 3 ? nz : ny);
     const int buf = real ? LB_TEMP : LB_OUT;
+    LinePass c[5];
     int k = 0;
     for (int j = 0; j < nf; j++) {
-        LinePass& lp = p->cpass[k++] = f[j];
-        lp.src = j == 0 ? LB_IN : buf; lp.dst = buf;
+        c[k] = f[j];
+        c[k].src = j == 0 ? LB_IN : buf; c[k++].dst = buf;
     }
-    p->cpass[nf - 1].kind = PK_XCONV;
+    c[nf - 1].kind = PK_XCONV;
     for (int j = nf - 2; j >= (real ? 1 : 0); j--) {
-        LinePass& lp = p->cpass[k++] = f[j];
-        lp.src = lp.dst = buf; lp.inv = true;
+        c[k] = f[j];
+        c[k].src = c[k].dst = buf; c[k++].inv = true;
     }
-    if (real) p->cpass[k++] = p->rpass[1][nf - 1];   // Z_C2R temp -> out
-    const SizeEntry* ex = f[0].e;
-    if (dims == 2 && !real && nx == ny && ex->plane_conv && !env_on("DFFT_NO_PLANE") && (plane_conv_default(nx, precision) || env_on("DFFT_FORCE_PLANE"))) {
-        // the three passes become one: the X pass's contiguous twiddle table serves both roles (one Sched at these lengths)
-        LinePass& lp = p->cpass[0];
-        lp.plane = true; lp.kind = PK_XCONV; lp.ntiles = batch;
-        lp.ia = lp.oa = Affine{(long long)nx * ny, 0, nx, 1};   // for the records: image, row and point strides
-        for (int j = 1; j < k; j++) p->cpass[j] = LinePass{};
+    const long long vol = (long long)nx * ny * (dims == 3 ? nz : 1);
+    if (real) make_real_pass(c[k++], f[0].e, vol / nx * batch, false, LB_TEMP, LB_OUT);   // Z_C2R temp -> out
+    if (dims == 2 && !real && nx == ny && f[0].e->plane_conv && !env_on("DFFT_NO_PLANE") && (plane_conv_default(nx, p->prec) || env_on("DFFT_FORCE_PLANE"))) {
+        // the three passes become one, on the X pass's buffers and contiguous twiddle table (one Sched at these lengths)
+        c[0].kind = LK_PLANE_CONV; c[0].ntiles = batch;
+        c[0].ia = c[0].oa = Affine{(long long)nx * ny, 0, nx, 1};
         k = 1;
     }
-    p->nconv = k;
-    // the builders' passes the schedule does not use give back their twiddle tables
-    auto used = [&](void* t) { for (int j = 0; j < k; j++) if (p->cpass[j].lut == t) return true; return false; };
-    for (auto& lp : p->pass) { if (lp.lut && !used(lp.lut)) cudaFree(lp.lut); lp = LinePass{}; }
-    for (auto& dir : p->rpass)
-        for (auto& lp : dir) { if (lp.lut && !used(lp.lut)) cudaFree(lp.lut); lp = LinePass{}; }
-    p->npass = p->nreal = 0;
-    p->conv = true;
-    p->real = real;
+    std::copy(c, c + k, p->run[0]);
+    p->nrun[0] = k;
+    p->nrun[1] = 0;
+    p->form = LF_CONV;
     p->batch = batch;
-    const long long vol = (long long)nx * ny * (dims == 3 ? nz : 1);
     p->mvol = real ? vol / nx * (nx / 2 + 1) : vol;
     if (real) p->rcount = vol * batch;
     else p->ccount = vol * batch;
@@ -2998,120 +2679,275 @@ static int make_lines_conv(dfft_lines_plan p, int dims, int nx, int ny, int nz, 
     return 0;
 }
 
-static int conv_plan_create(int dims, int nx, int ny, int nz, long long batch, int precision, bool real, unsigned flags, dfft_lines_plan* out)
+static int lines_plan_common(dfft_lines_plan p, int precision)
+{
+    p->prec = precision;
+    CU(cudaGetDevice(&p->device));
+    CU(cudaDeviceGetAttribute(&p->sms, cudaDevAttrMultiProcessorCount, p->device));
+    CU(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
+    for (auto& e : p->ev) CU(cudaEventCreate(&e));
+    return 0;
+}
+
+// the device twiddle table of lp's entry and schedule, uploaded in the plan's precision when a pass first asks for it
+static int lines_lut(dfft_lines_plan p, LinePass& lp)
+{
+    const int kind = plain_kind(lp.kind);
+    for (const auto& t : p->luts)
+        if (t.e == lp.e && t.kind == kind) { lp.lut = t.d; return 0; }
+    const cudaError_t err = p->prec == DFFT_DOUBLE ? upload_lut_kind<double>(&lp.lut, lp.e, kind) : upload_lut_kind<float>(&lp.lut, lp.e, kind);
+    if (lp.lut) p->luts.push_back({lp.e, kind, lp.lut});
+    if (err != cudaSuccess || !lp.lut) return fail(DFFT_ECUDA, "twiddle table upload failed");
+    return 0;
+}
+
+extern "C" int dfft_lines_destroy(dfft_lines_plan p)
+{
+    if (!p) return 0;
+    cudaSetDevice(p->device);
+    if (p->stream) cudaStreamSynchronize(p->stream);
+    for (const auto& t : p->luts) cudaFree(t.d);
+    if (p->temp) cudaFree(p->temp);
+    for (auto& e : p->ev) if (e) cudaEventDestroy(e);
+    if (p->stream) cudaStreamDestroy(p->stream);
+    cudaGetLastError();
+    delete p;
+    return 0;
+}
+
+// a plan laid out by `build` (which validates the arguments), with its twiddle tables and temporary; destroyed again on failure
+template <class Build> static int lines_create(dfft_lines_plan* out, int precision, Build build)
 {
     if (!out) return fail(DFFT_EINVAL, "null plan pointer");
     *out = nullptr;
-    if (precision != DFFT_DOUBLE && precision != DFFT_FLOAT) return fail(DFFT_EINVAL, "bad arguments");
     dfft_lines_plan p = new dfft_lines_plan_s;
     int rc = lines_plan_common(p, precision);
-    if (!rc) rc = make_lines_conv(p, dims, nx, ny, nz, batch, precision, real, flags, false);
+    if (!rc) rc = build(p);
+    for (int d = 0; d < 2; d++)
+        for (int k = 0; k < p->nrun[d] && !rc; k++) rc = lines_lut(p, p->run[d][k]);
+    if (!rc && p->temp_bytes) {
+        const cudaError_t err = cudaMalloc(&p->temp, p->temp_bytes);
+        if (err != cudaSuccess) rc = fail(DFFT_ECUDA, "temporary allocation failed: %s", cudaGetErrorString(err));
+    }
     if (rc) { dfft_lines_destroy(p); return rc; }
     *out = p;
     return 0;
 }
 
+extern "C" int dfft_lines_plan_create(int n, long long stride, long long nlines, long long inner, long long inner_dist, long long outer_dist,
+                                      int precision, dfft_lines_plan* out)
+{
+    return lines_create(out, precision, [&](dfft_lines_plan p) {
+        return make_lines_1d(p, n, stride, nlines, inner, inner_dist, outer_dist, !env_on("DFFT_NO_LONG_LINES"));
+    });
+}
+
+/* batch of 2-D transforms, nx fastest: the reference's FFTdim = 2 application (Test_2D.cpp: size = {X, Y, Z}) */
+extern "C" int dfft_lines_plan_create_2d(int nx, int ny, long long batch, int precision, dfft_lines_plan* out)
+{
+    return lines_create(out, precision, [&](dfft_lines_plan p) { return make_lines_2d(p, nx, ny, batch); });
+}
+
+extern "C" int dfft_lines_plan_create_3d(int nx, int ny, int nz, long long batch, int precision, dfft_lines_plan* out)
+{
+    return lines_create(out, precision, [&](dfft_lines_plan p) { return make_lines_3d(p, nx, ny, nz, batch); });
+}
+
+extern "C" int dfft_lines_plan_create_r2c(int n, long long nlines, int precision, dfft_lines_plan* plan)
+{
+    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_real_lines(p, n, 1, 1, nlines, 1); });
+}
+
+extern "C" int dfft_lines_plan_create_r2c_2d(int nx, int ny, long long batch, int precision, dfft_lines_plan* plan)
+{
+    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_real_lines(p, nx, ny, 1, batch, 2); });
+}
+
+extern "C" int dfft_lines_plan_create_r2c_3d(int nx, int ny, int nz, long long batch, int precision, dfft_lines_plan* plan)
+{
+    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_real_lines(p, nx, ny, nz, batch, 3); });
+}
+
 extern "C" int dfft_lines_plan_create_convolve_3d(int nx, int ny, int nz, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
 {
-    return conv_plan_create(3, nx, ny, nz, batch, precision, false, flags, plan);
+    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv(p, 3, nx, ny, nz, batch, false, flags); });
 }
 
 extern "C" int dfft_lines_plan_create_convolve_r2c_3d(int nx, int ny, int nz, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
 {
-    return conv_plan_create(3, nx, ny, nz, batch, precision, true, flags, plan);
+    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv(p, 3, nx, ny, nz, batch, true, flags); });
 }
 
 extern "C" int dfft_lines_plan_create_convolve_2d(int nx, int ny, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
 {
-    return conv_plan_create(2, nx, ny, 1, batch, precision, false, flags, plan);
+    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv(p, 2, nx, ny, 1, batch, false, flags); });
 }
 
 extern "C" int dfft_lines_plan_create_convolve_r2c_2d(int nx, int ny, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
 {
-    return conv_plan_create(2, nx, ny, 1, batch, precision, true, flags, plan);
+    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv(p, 2, nx, ny, 1, batch, true, flags); });
 }
 
-// pass k of a convolve lines plan: launched on the plan's stream, or (ops) only recorded, phase = k
-template <typename T>
-static cudaError_t conv_line_pass(const dfft_lines_plan_s* p, int k, const void* in, void* out, const void* mult, bool shared,
-                                  std::vector<std::string>* ops = nullptr)
+static inline void* line_buf(int which, const void* in, void* out, void* temp)
 {
-    const LinePass& lp = p->cpass[k];
+    return which == LB_TEMP ? temp : (which == LB_OUT ? out : const_cast<void*>(in));
+}
+
+// pass `lp` of a lines plan, at position `phase` of its list: launched on the plan's stream, or (ops) only recorded.  The one
+// place that builds a lines pass's kernel arguments and its record; the launch path allocates nothing
+template <typename T>
+static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int phase, const void* in, void* out, const void* mult, bool shared,
+                             std::vector<std::string>* ops = nullptr)
+{
+    const void* src = line_buf(lp.src, in, out, p->temp);
+    void* dst = line_buf(lp.dst, in, out, p->temp);
+    const bool conv = lp.kind == PK_XCONV || lp.kind == LK_PLANE_CONV, realk = lp.kind == PK_Z_R2C || lp.kind == PK_Z_C2R;
     ConvArgs<T> c{};
-    RealZArgs<T> r{};
-    real_line_args<T>(lp, line_buf(lp.src, in, out, p->temp), line_buf(lp.dst, in, out, p->temp), lp.inv ? DFFT_BACKWARD : DFFT_FORWARD, r);
-    const bool realk = lp.kind == PK_Z_R2C || lp.kind == PK_Z_C2R;
-    if (lp.plane && lp.kind == PK_XCONV) {
-        const long long n = lp.e->N;
-        const PlaneConvArgs<T> pc{{r.t.in, r.t.out, r.t.lut, lp.ntiles, 0}, (const cx<T>*)mult, shared ? 0 : n * n, (T)p->scale, p->scale != 0 ? 1 : 0};
-        if (ops) {
-            r.t.do_scale = pc.do_scale; r.t.scale = pc.scale;
-            char extra[128];
-            snprintf(extra, sizeof(extra), ", \"mult\": %llu, \"shared\": %d", (unsigned long long)(size_t)mult, shared ? 1 : 0);
-            record_op<T>(*ops, "XY_PLANE_CONV", k, lp.e->N, lp.e->N, false, false, false, r.t, extra);
-            return cudaSuccess;
-        }
-        return lp.e->plane_conv(&pc, p->sms, p->stream);
-    }
-    if (lp.plane) {
-        const PlaneArgs<T> pa{r.t.in, r.t.out, r.t.lut, lp.ntiles, r.t.inv};
-        if (ops) record_op<T>(*ops, "XY_PLANE", k, lp.e->N, lp.e->N, false, false, false, r.t);
-        return ops ? cudaSuccess : lp.e->plane(&pa, p->sms, p->stream);
-    }
-    if (lp.kind == PK_XCONV) {
-        c.t = r.t;
-        c.t.do_scale = p->scale != 0; c.t.scale = (T)p->scale;
+    TileArgs<T>& a = c.t;
+    a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)lp.lut;
+    a.ia = lp.ia; a.oa = lp.oa; a.G = lp.G; a.W = lp.W; a.ntiles = lp.ntiles;
+    a.inv = lp.inv; a.gen = lp.e->gen; a.tw_n = lp.tw_n;
+    if (conv) {
+        a.do_scale = p->scale != 0; a.scale = (T)p->scale;
         c.mult = (const cx<T>*)mult; c.mult_shared = shared ? 1 : 0;
     }
     if (ops) {
         char extra[128] = "";
         if (realk) snprintf(extra, sizeof(extra), ", \"nzh\": %d, \"pair\": [%lld, %lld]", lp.e->N / 2 + 1, lp.ld_in, lp.ld_out);
-        if (lp.kind == PK_XCONV) snprintf(extra, sizeof(extra), ", \"mult\": %llu, \"shared\": %d", (unsigned long long)(size_t)mult, shared ? 1 : 0);
-        const int C = realk || lp.kind == PK_Z ? lp.e->z_C : lp.e->s_C;
-        record_op<T>(*ops, kPassNames[lp.kind], k, lp.e->N, C, false, false, false, lp.kind == PK_XCONV ? c.t : r.t, extra);
+        if (conv) snprintf(extra, sizeof(extra), ", \"mult\": %llu, \"shared\": %d", (unsigned long long)(size_t)mult, shared ? 1 : 0);
+        const bool plane = lp.kind >= PK_COUNT;
+        const char* name = lp.kind == LK_PLANE ? "XY_PLANE" : lp.kind == LK_PLANE_CONV ? "XY_PLANE_CONV" : kPassNames[lp.kind];
+        record_op<T>(*ops, name, phase, lp.e->N, plane ? lp.e->N : kind_C(lp.e, plain_kind(lp.kind)), false, false, lp.kind == PK_XF_TW, a, extra);
         return cudaSuccess;
     }
-    const void* args = realk ? (const void*)&r : lp.kind == PK_XCONV ? (const void*)&c : (const void*)&r.t;
-    return lp.e->launch[lp.kind](args, p->sms, p->stream);
+    switch (lp.kind) {
+    case LK_PLANE: {
+        const PlaneArgs<T> pa{a.in, a.out, a.lut, lp.ntiles, a.inv};
+        return lp.e->plane(&pa, p->sms, p->stream);
+    }
+    case LK_PLANE_CONV: {
+        const long long n = lp.e->N;
+        const PlaneConvArgs<T> pc{{a.in, a.out, a.lut, lp.ntiles, 0}, c.mult, shared ? 0 : n * n, a.scale, a.do_scale};
+        return lp.e->plane_conv(&pc, p->sms, p->stream);
+    }
+    case PK_Z_R2C: case PK_Z_C2R: {
+        const RealZArgs<T> r{a, (const T*)src, (T*)dst, lp.ld_in, lp.ld_out};
+        return lp.e->launch[lp.kind](&r, p->sms, p->stream);
+    }
+    default:
+        return lp.e->launch[lp.kind](conv ? (const void*)&c : (const void*)&a, p->sms, p->stream);
+    }
 }
 
-template <typename T> static int lines_execute_conv_impl(dfft_lines_plan p, const void* in, void* out, const void* mult, bool shared)
+// one execute: the passes of run[list] between the plan's two events
+template <typename T> static int lines_run(dfft_lines_plan p, int list, const void* in, void* out, const void* mult = nullptr, bool shared = false)
 {
+    CU(cudaSetDevice(p->device));
     CU(cudaEventRecord(p->ev[0], p->stream));
-    for (int k = 0; k < p->nconv; k++) {
-        if (p->cpass[k].ntiles <= 0) continue;
-        const cudaError_t err = conv_line_pass<T>(p, k, in, out, mult, shared);
-        if (err != cudaSuccess) return fail(DFFT_ECUDA, "convolve line pass launch failed: %s", cudaGetErrorString(err));
+    for (int k = 0; k < p->nrun[list]; k++) {
+        const LinePass& lp = p->run[list][k];
+        if (lp.ntiles <= 0) continue;
+        const cudaError_t err = line_pass<T>(p, lp, k, in, out, mult, shared);
+        if (err != cudaSuccess) return fail(DFFT_ECUDA, "line pass launch failed: %s", cudaGetErrorString(err));
     }
     CU(cudaEventRecord(p->ev[1], p->stream));
-    p->timed = true;
     return 0;
+}
+
+extern "C" int dfft_lines_execute(dfft_lines_plan p, void* data, int direction)
+{
+    if (!p || !data || (direction != DFFT_FORWARD && direction != DFFT_BACKWARD)) return fail(DFFT_EINVAL, "bad arguments");
+    if (p->form == LF_CONV) return fail(DFFT_EINVAL, "a convolve lines plan runs with dfft_lines_execute_convolve");
+    if (p->form == LF_REAL) return fail(DFFT_EINVAL, "a real lines plan runs with dfft_lines_execute_real");
+    const int list = direction == DFFT_BACKWARD;
+    return p->prec == DFFT_DOUBLE ? lines_run<double>(p, list, data, data) : lines_run<float>(p, list, data, data);
+}
+
+extern "C" int dfft_lines_execute_real(dfft_lines_plan p, const void* in, void* out, int direction)
+{
+    if (!p || !in || !out || (direction != DFFT_FORWARD && direction != DFFT_BACKWARD)) return fail(DFFT_EINVAL, "bad arguments");
+    if (p->form == LF_CONV) return fail(DFFT_EINVAL, "a convolve lines plan runs with dfft_lines_execute_convolve");
+    if (p->form != LF_REAL) return fail(DFFT_EINVAL, "a complex lines plan runs with dfft_lines_execute");
+    const size_t rsz = p->prec == DFFT_FLOAT ? 4 : 8, csz = 2 * rsz;
+    const bool fwd = direction == DFFT_FORWARD;
+    const uintptr_t ri = (uintptr_t)(fwd ? in : out), ci = (uintptr_t)(fwd ? out : in);
+    if (ri % rsz || ci % csz) return fail(DFFT_EINVAL, "a %s buffer is not aligned to its element size", ri % rsz ? "real" : "complex");
+    const uintptr_t a = (uintptr_t)in, b = (uintptr_t)out;
+    const uintptr_t a_end = a + (fwd ? p->rcount * rsz : p->ccount * csz), b_end = b + (fwd ? p->ccount * csz : p->rcount * rsz);
+    if (a == b || (a < b_end && b < a_end)) return fail(DFFT_EINVAL, "`in` and `out` overlap (real lines are out of place)");
+    const int list = fwd ? 0 : 1;
+    return p->prec == DFFT_DOUBLE ? lines_run<double>(p, list, in, out) : lines_run<float>(p, list, in, out);
 }
 
 extern "C" int dfft_lines_execute_convolve(dfft_lines_plan p, const void* in, void* out, const void* mult, long long mult_count)
 {
     if (!p || !in || !out || !mult) return fail(DFFT_EINVAL, "bad arguments");
-    if (!p->conv) return fail(DFFT_EINVAL, "dfft_lines_execute_convolve needs a plan from dfft_lines_plan_create_convolve_[r2c_]2d / _3d");
+    if (p->form != LF_CONV) return fail(DFFT_EINVAL, "dfft_lines_execute_convolve needs a plan from dfft_lines_plan_create_convolve_[r2c_]2d / _3d");
     if (mult_count != 1 && mult_count != p->batch) return fail(DFFT_EINVAL, "mult_count must be 1 or the plan's batch (%lld), not %lld", p->batch, mult_count);
-    const size_t rsz = p->prec == DFFT_FLOAT ? 4 : 8, csz = 2 * rsz, esz = p->real ? rsz : csz;
+    const bool real = p->run[0][0].kind == PK_Z_R2C;   // a real plan's first pass is the R2C pass
+    const size_t rsz = p->prec == DFFT_FLOAT ? 4 : 8, csz = 2 * rsz, esz = real ? rsz : csz;
     const uintptr_t a = (uintptr_t)in, b = (uintptr_t)out, m = (uintptr_t)mult;
     if (a % esz || b % esz || m % csz) return fail(DFFT_EINVAL, "a buffer is not aligned to its element size");
-    const uintptr_t io = (uintptr_t)((p->real ? p->rcount : p->ccount) * esz), mb = (uintptr_t)(mult_count * p->mvol * csz);
+    const uintptr_t io = (uintptr_t)((real ? p->rcount : p->ccount) * esz), mb = (uintptr_t)(mult_count * p->mvol * csz);
     if (a != b && a < b + io && b < a + io) return fail(DFFT_EINVAL, "`in` and `out` overlap without being the same buffer");
     if (m < b + io && b < m + mb) return fail(DFFT_EINVAL, "the multiplier overlaps `out`");
-    CU(cudaSetDevice(p->device));
     const bool shared = mult_count == 1;
-    return p->prec == DFFT_DOUBLE ? lines_execute_conv_impl<double>(p, in, out, mult, shared) : lines_execute_conv_impl<float>(p, in, out, mult, shared);
+    return p->prec == DFFT_DOUBLE ? lines_run<double>(p, 0, in, out, mult, shared) : lines_run<float>(p, 0, in, out, mult, shared);
 }
 
-// the records of a dry convolve lines plan's passes (in = buffer 5, out = 2, temporary = 4, multiplier = 8), through conv_line_pass
-static long long conv_ops_json(dfft_lines_plan_s& lp, long long batch, long long mult_count, char* buf, long long cap)
+extern "C" int dfft_lines_synchronize(dfft_lines_plan p)
 {
-    if (mult_count != 1 && mult_count != batch) return fail(DFFT_EINVAL, "mult_count must be 1 or the plan's batch");
+    if (!p) return fail(DFFT_EINVAL, "null plan");
+    CU(cudaSetDevice(p->device));
+    CU(cudaStreamSynchronize(p->stream));
+    return 0;
+}
+
+extern "C" void* dfft_lines_stream(dfft_lines_plan p) { return p ? (void*)p->stream : nullptr; }
+
+// the records of list `list` of the describe-only plan `build` lays out, in the hooks' JSON; buffers of device 0: `in`, `out`, the
+// temporary 4, the multiplier 8
+template <class Build> static long long lines_ops_json(int precision, Build build, int list, int in, int out, bool shared, char* buf, long long cap)
+{
+    dfft_lines_plan_s p;
+    p.prec = precision;
+    p.temp = fake_addr(0, 4);
+    const int rc = build(&p);
+    if (rc) return rc;
     std::vector<std::string> ops;
-    for (int k = 0; k < lp.nconv; k++) conv_line_pass<double>(&lp, k, fake_addr(0, 5), fake_addr(0, 2), fake_addr(0, 8), mult_count == 1, &ops);
-    lp.temp = nullptr;
+    for (int k = 0; k < p.nrun[list]; k++) line_pass<double>(&p, p.run[list][k], k, fake_addr(0, in), fake_addr(0, out), fake_addr(0, 8), shared, &ops);
     return ops_json(ops, buf, cap);
+}
+
+/* test hook (host only): the passes a lines plan would launch for `direction`, as JSON (same format as dfft_debug_plan_ops;
+ * the caller's data is buffer 1 of device 0, the plan's temporary buffer 4); two_d != 0: 2-D plan (n = nx, stride = ny,
+ * nlines = batch).  Long lines always use the four-step plan here.  Returns the bytes needed, < 0 on error. */
+extern "C" long long dfft_debug_lines_ops(int n, long long stride, long long nlines, long long inner, long long inner_dist, long long outer_dist,
+                                          int precision, int direction, int two_d, char* buf, long long cap)
+{
+    auto build = [&](dfft_lines_plan p) {
+        return two_d ? make_lines_2d(p, n, (int)stride, nlines) : make_lines_1d(p, n, stride, nlines, inner, inner_dist, outer_dist, true);
+    };
+    return lines_ops_json(precision, build, direction == DFFT_BACKWARD, 1, 1, false, buf, cap);
+}
+
+/* test hook (host only): the passes of a real lines plan for `direction`, JSON as dfft_debug_lines_ops; in = buffer 5, out = 2,
+ * temporary = 4 of device 0.  Real passes carry "nzh" and "pair" as the 3-D plan's Z_R2C / Z_C2R records */
+extern "C" long long dfft_debug_real_lines_ops(int n, int ny, long long batch, int precision, int direction, int two_d, char* buf, long long cap)
+{
+    if (direction != DFFT_FORWARD && direction != DFFT_BACKWARD) return fail(DFFT_EINVAL, "bad direction");
+    auto build = [&](dfft_lines_plan p) { return make_real_lines(p, n, ny, 1, batch, two_d ? 2 : 1); };
+    return lines_ops_json(precision, build, direction == DFFT_BACKWARD, 5, 2, false, buf, cap);
+}
+
+/* test hook (host only): the passes of a 3-D lines plan for `direction`, JSON as dfft_debug_lines_ops (complex: the caller's data
+ * is buffer 1) or dfft_debug_real_lines_ops (real != 0: in = buffer 5, out = 2, temporary = 4).  The plane kernel's record is
+ * "XY_PLANE" with ntiles = planes and ia = oa = [plane, 0, row, point] strides */
+extern "C" long long dfft_debug_lines_3d_ops(int nx, int ny, int nz, long long batch, int precision, int direction, int real, char* buf, long long cap)
+{
+    if (direction != DFFT_FORWARD && direction != DFFT_BACKWARD) return fail(DFFT_EINVAL, "bad direction");
+    auto build = [&](dfft_lines_plan p) { return real ? make_real_lines(p, nx, ny, nz, batch, 3) : make_lines_3d(p, nx, ny, nz, batch); };
+    return lines_ops_json(precision, build, direction == DFFT_BACKWARD, real ? 5 : 1, real ? 2 : 1, false, buf, cap);
 }
 
 /* test hook (host only): the passes of a convolve lines plan, JSON as dfft_debug_lines_3d_ops; in = buffer 5, out = 2,
@@ -3119,11 +2955,11 @@ static long long conv_ops_json(dfft_lines_plan_s& lp, long long batch, long long
 extern "C" long long dfft_debug_lines_conv_3d_ops(int nx, int ny, int nz, long long batch, int precision, int real, unsigned flags,
                                                   long long mult_count, char* buf, long long cap)
 {
-    dfft_lines_plan_s lp;
-    lp.prec = precision;
-    const int rc = make_lines_conv(&lp, 3, nx, ny, nz, batch, precision, real != 0, flags, true);
-    if (rc) return rc;
-    return conv_ops_json(lp, batch, mult_count, buf, cap);
+    auto build = [&](dfft_lines_plan p) {
+        const int rc = make_lines_conv(p, 3, nx, ny, nz, batch, real != 0, flags);
+        return rc || mult_count == 1 || mult_count == batch ? rc : fail(DFFT_EINVAL, "mult_count must be 1 or the plan's batch");
+    };
+    return lines_ops_json(precision, build, 0, 5, 2, mult_count == 1, buf, cap);
 }
 
 /* test hook (host only): the passes of a 2-D convolve lines plan, JSON as dfft_debug_lines_conv_3d_ops.  The plane-convolve
@@ -3131,11 +2967,11 @@ extern "C" long long dfft_debug_lines_conv_3d_ops(int nx, int ny, int nz, long l
 extern "C" long long dfft_debug_lines_conv_2d_ops(int nx, int ny, long long batch, int precision, int real, unsigned flags,
                                                   long long mult_count, char* buf, long long cap)
 {
-    dfft_lines_plan_s lp;
-    lp.prec = precision;
-    const int rc = make_lines_conv(&lp, 2, nx, ny, 1, batch, precision, real != 0, flags, true);
-    if (rc) return rc;
-    return conv_ops_json(lp, batch, mult_count, buf, cap);
+    auto build = [&](dfft_lines_plan p) {
+        const int rc = make_lines_conv(p, 2, nx, ny, 1, batch, real != 0, flags);
+        return rc || mult_count == 1 || mult_count == batch ? rc : fail(DFFT_EINVAL, "mult_count must be 1 or the plan's batch");
+    };
+    return lines_ops_json(precision, build, 0, 5, 2, mult_count == 1, buf, cap);
 }
 
 extern "C" int dfft_fft_lines(void* data, int n, long long stride, long long nlines, long long inner, long long inner_dist,

@@ -326,6 +326,21 @@ def test_lines_plan_schedules_1d_and_2d():
         assert np.abs(m.view(fake(0, BUF1))[0].reshape(a.shape) - ref).max() <= 1e-11 * np.abs(ref).max()
 
 
+def test_lines_plans_take_at_most_2_31_minus_1_rows():
+    """A pass's row (or column) count is a 32-bit kernel argument: 1-D and 2-D plans with more are DFFT_EUNSUPPORTED, as the
+    3-D, real and convolve plans are, rather than transforming only the rows below the limit."""
+    rows = 1 << 31
+    ops = dfft.lines_ops(2, 1, rows - 1, rows - 1, 2, 0, FORWARD)
+    assert [(o["op"], o["W"]) for o in ops] == [("Z", rows - 1)]
+    for args, two_d in (((2, 1, rows, rows, 2, 0), False),            # contiguous lines
+                        ((2, rows, rows, rows, 1, 0), False),         # strided columns
+                        ((65536, 1, rows, rows, 65536, 0), False),    # four-step long lines
+                        ((2, 2, rows >> 1, 0, 0, 0), True),           # 2-D: ny * batch rows
+                        ((16, 16, 1 << 60, 0, 0, 0), True)):          # 2-D: ny * batch beyond 64 bits
+        with pytest.raises(dfft.DfftError, match=r"\(-3\)"):
+            dfft.lines_ops(*args, FORWARD, two_d=two_d)
+
+
 def test_random_geometries_all_exchanges(co):
     """Seeded random sweep over device counts, tuned and generic lengths, even and uneven splits, both directions."""
     rng = np.random.default_rng(2026)
