@@ -90,9 +90,11 @@ static cudaError_t launch_tma_fused_zy(const void* vargs, const FusedCtl* ctl, c
     long long grid = sm_count;
     if (grid > total) grid = total;
     FusedCtl c = *ctl;
-    // the Z role runs ahead of the Y role by the tiles the rings hold (TMA_NSLOT per CTA): 4 planes at 512 points on 132 SMs.
-    // One plane more, as fft_fused2_kernel's default adds, measured 0.1 ms slower on H100 (more of the L2 holds intermediate)
-    if (c.lag <= 0) c.lag = (int)((grid * TMA_NSLOT + c.GA + c.GB - 1) / ((long long)c.GA + c.GB));
+    // the Z role runs ahead of the Y role by the tiles the rings hold beside the one each CTA is transforming
+    // (TMA_NSLOT - 1 per CTA): 3 planes at 512 points on 132 SMs.  Each plane more keeps another 4 MiB of intermediate in
+    // the L2; with the mover publishing Z tiles as soon as it is idle, lag 4 measured 0.02 ms and lag 5 0.17 ms slower on
+    // H100 (DESIGN.md 3.4)
+    if (c.lag <= 0) c.lag = (int)((grid * (TMA_NSLOT - 1) + c.GA + c.GB - 1) / ((long long)c.GA + c.GB));
     kern<<<(unsigned)grid, G_::NT + 32, G_::SMEM, st>>>(a, c, *reinterpret_cast<const CUtensorMap*>(map_mid));
     return cudaGetLastError();
 }

@@ -73,7 +73,7 @@ template <int LAY, int N, int C> __device__ __forceinline__ int tma_idx(int c, i
 }
 
 // CTA-wide barrier of the threads that transform a tile: the whole CTA in the pass kernels; in the fused kernel, whose
-// producer warp has left the loop, the NT consumer threads on named barrier 1
+// mover warp has left the loop, the NT consumer threads on named barrier 1
 template <bool CONS, int NT> __device__ __forceinline__ void tma_sync()
 {
     if constexpr (CONS) asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory");
@@ -216,19 +216,27 @@ __global__ void __launch_bounds__(S::T* C, 1) fft_tma_pass_kernel(const TmaArgs<
 // fft_fused2_kernel (fused2_decode: Z runs `lag` planes ahead of Y) and the same monotonic per-plane counters.
 //   Z role: src -> mid, C contiguous lines per tile, 1-D bulk copies (TMA_Z's tile and thread map)
 //   Y role: mid -> mid in place, C columns per tile, 3-D tensor copies through map_mid (TMA_Y's tile, map and thread map)
-// The CTA is NT consumer threads and one producer warp.  The producer (one lane) draws a ticket only when it owns an empty
-// ring slot, and issues that tile's load at once -- for a Y tile after its plane's counter has reached the target (it may
-// block there).  Consumers transform the slots in order; thread 0 issues the stores and retires a tile (frees its slot,
-// and for a Z tile publishes it on the plane counter) once its store is complete.
+// The CTA is NT consumer threads and one mover warp, of which one lane works.  The consumers only transform: they take the
+// slots in ring order as they land (mbarrier `full`) and hand each back (mbarrier `done`).  The mover does all the rest in
+// one polling loop that never blocks on anything but its own bulk groups:
+//   - a handed-back tile: issue its store, wait until the store has READ the slot (cp.async.bulk.wait_group.read) and
+//     count the slot free; a Z tile's store stays pending, and is published (plane counter += 1) as soon as the mover has
+//     nothing else to do (wait_group 0), or when a later store has been issued and everything older is complete (wait_group 1);
+//   - a free slot: draw a ticket and issue its load -- a Y tile's only after its plane's counter has reached the target,
+//     polled, so that a Y tile waiting for its plane holds up neither the stores nor the publications of this CTA;
+// Why a mover (csrc/tools/t0_profile.py, DESIGN.md 3.4): when consumer thread 0 issued the stores, it waited for the
+// previous store's completion before every tile, and each slot stayed held until its store was complete; at 512^3 fp64 the
+// transform itself then took less than half of the time per tile.  Here the consumers never wait for a store, and a slot
+// is refilled as soon as its store has read it.
 // Deadlock freedom, whatever the residency: a Y ticket waits only for Z tickets of its plane, and all of them are lower.
-// Each of those was drawn by a running producer with an empty slot, so its load is in flight; the tiles ahead of it in
-// that CTA's ring have still lower tickets (tickets rise per CTA), so by induction they complete; and the Z tile itself is
-// retired as soon as its store completes, because thread 0 never blocks on the next slot while a tile is unretired: it
-// polls the next slot and retires the previous tile in the meantime (the next slot may hold exactly the Y tile that waits
-// for it).  Moving the producer into the consumer loop, as in fft_tma_pass_kernel, breaks this: a blocked Y load would
-// then hold back the retirement of the Z tiles in front of it.
-// Proxy order of the hand-over: producer of the Z tile: store's wait_group, fence.proxy.async, __threadfence, counter add;
-// producer of the Y tile: ld.acquire.gpu of the counter, fence.proxy.async, tensor load.
+// Each of those was drawn by a running mover with a free slot, so its load is in flight; the tiles ahead of it in that CTA's
+// ring have still lower tickets (tickets rise per CTA), so by induction they land, and the consumers, who wait for nothing
+// but landed slots, hand them back in order.  The Z tile's store is then issued, and it is published without waiting for a
+// later tile to land: the mover publishes it the first time it finds nothing else to do, which it must while the next
+// ticket is a Y tile still waiting for its plane (perhaps for exactly this tile), and at the latest with the next store.
+// Proxy order of the hand-over: consumers' smem writes, fence.proxy.async.shared::cta, named barrier, `done` arrive; the
+// mover's mbarrier test_wait, then its TMA store.  Z tile: store's wait_group, fence.proxy.async, __threadfence, counter add;
+// Y tile: ld.acquire.gpu of the counter, fence.proxy.async, tensor load.
 // L2 policy per instruction (createpolicy): the slab is read once and the finished Y columns are not read again by this
 // kernel, so the Z loads and the Y stores are evict_first; the Z stores of the intermediate are evict_last, so that they
 // survive until their Y tiles read them.  At 512^3 fp64 on H100 the three hints together take t0 from 2.90 to 2.30 ms at
@@ -237,7 +245,27 @@ template <typename T> struct TmaFusedArgs {
     const cx<T>* src;    // Z role input (dense planes of N x N)
     cx<T>* mid;          // Z role output, Y role input and output (described by map_mid)
     const cx<T>* lut;
+    unsigned long long* stamps;   // FZY_STAMPS instantiations only: FZY_NSTAMP words per ticket; null in the library
 };
+
+// Measurement instantiations of fft_tma_fused_zy_kernel (PROBE bits; the library instantiates PROBE = 0 only, and
+// csrc/tools/t0_profile.py builds the others):
+//   FZY_MOVE   the movement-only twin: same tickets, plane counters, ring, loads, stores and L2 hints, but the consumers copy
+//              the slot through unchanged (no butterflies, no exchanges) -- its time is what the ring, the hand-off through
+//              the plane counters and the L2 traffic allow without any arithmetic
+//   FZY_STAMPS %globaltimer stamps per tile into A.stamps[ticket * FZY_NSTAMP + field], fields FZS_*
+enum { FZY_MOVE = 1, FZY_STAMPS = 2 };
+enum { FZS_WHO = 0,        // blockIdx.x * 2 + (Y tile ? 1 : 0)
+       FZS_TICKET,         // mover: ticket drawn
+       FZS_DEP,            // mover: plane counter satisfied (a Z tile: = FZS_TICKET)
+       FZS_LOAD,           // mover: load issued
+       FZS_READY,          // consumer thread 0: done with the previous tile, starts waiting for this slot
+       FZS_FULL,           // consumer thread 0: slot full
+       FZS_DONE,           // consumer thread 0: transform done (after the consumers' barrier), tile handed to the mover
+       FZS_STORE,          // mover: store issued
+       FZS_FREED,          // mover: the store has read the slot, slot freed
+       FZS_RETIRED,        // mover: a Z tile's store is complete and the tile published (a Y tile: just after FZS_FREED)
+       FZY_NSTAMP };
 
 __device__ __forceinline__ uint64_t l2_policy_evict_first()
 {
@@ -270,23 +298,39 @@ __device__ __forceinline__ void tma_mbar_arrive(uint64_t* bar)
 {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// non-blocking test of a phase (mbarrier.try_wait may suspend the thread for a while; a thread that polls several things must not)
+__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t phase)
+{
+    uint32_t ok;
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
+        "selp.u32 %0, 1, 0, p;\n"
+        "}\n" : "=r"(ok) : "r"(smem_u32(bar)), "r"(phase) : "memory");
+    return ok != 0;
+}
 
-template <class S, typename T, int C>
-__global__ void __launch_bounds__(S::T* C + 32, 1) fft_tma_fused_zy_kernel(const TmaFusedArgs<T> A, const FusedCtl F,
-                                                                            const __grid_constant__ CUtensorMap map_mid)
+template <class S, typename T, int C, int PROBE>
+__device__ __forceinline__ void tma_fused_zy_body(const TmaFusedArgs<T>& A, const FusedCtl& F, const CUtensorMap* map_mid)
 {
     using G_ = TmaGeom<S, T, C>;
     constexpr int N = S::N, NT = G_::NT, TT = S::T, ROWS = G_::ROWS, NBOX = G_::NBOX;
+    constexpr bool STAMPS = (PROBE & FZY_STAMPS) != 0;
     extern __shared__ __align__(128) unsigned char tma_raw[];
     cx<T>* const lut_s = reinterpret_cast<cx<T>*>(tma_raw + (size_t)TMA_NSLOT * G_::TILE_BYTES);
     uint64_t* const full = reinterpret_cast<uint64_t*>(tma_raw + (size_t)TMA_NSLOT * G_::TILE_BYTES + G_::LUT_BYTES);
-    uint64_t* const empty = full + TMA_NSLOT;
-    int* const desc = reinterpret_cast<int*>(empty + TMA_NSLOT);   // per slot: role (-1 end, 0 Z, 1 Y), plane, tile
-    static_assert(2 * TMA_NSLOT * sizeof(uint64_t) + 3 * TMA_NSLOT * sizeof(int) <= 128, "ring control words exceed the reserve");
+    uint64_t* const done = full + TMA_NSLOT;   // per slot: the consumers have written the tile back into it
+    int* const desc = reinterpret_cast<int*>(done + TMA_NSLOT);   // per slot: role (-1 end, 0 Z, 1 Y), plane, tile
+    unsigned* const slot_ticket = reinterpret_cast<unsigned*>(desc + 3 * TMA_NSLOT);   // per slot: ticket (FZY_STAMPS only)
+    static_assert(2 * TMA_NSLOT * sizeof(uint64_t) + 4 * TMA_NSLOT * sizeof(int) <= 128, "ring control words exceed the reserve");
     auto slot = [&](int i) { return reinterpret_cast<cx<T>*>(tma_raw + (size_t)i * G_::TILE_BYTES); };
+    auto stamp = [&](unsigned t, int f) {
+        if constexpr (STAMPS) A.stamps[(size_t)t * FZY_NSTAMP + f] = gtime_ns();
+    };
     const int tid = threadIdx.x;
     if (tid == 0) {
-        for (int i = 0; i < TMA_NSLOT; i++) { mbar_init(full + i, 1); mbar_init(empty + i, 1); }
+        for (int i = 0; i < TMA_NSLOT; i++) { mbar_init(full + i, 1); mbar_init(done + i, 1); }
         fence_barrier_init();
     }
     for (int i = tid; i < S::lut_size(); i += NT + 32) lut_s[i] = A.lut[i];
@@ -294,68 +338,135 @@ __global__ void __launch_bounds__(S::T* C + 32, 1) fft_tma_fused_zy_kernel(const
     const Fused2Order o = fused2_prepare(F);
 
     if (tid >= NT) {
-        // ---- producer: one lane, up to TMA_NSLOT tiles ahead of the consumers ----
+        // ---- mover: one lane draws the tickets, issues every load and store, frees the slots and publishes the Z tiles ----
         if (tid == NT) {
-            const uint64_t read_once = l2_policy_evict_first();
-            for (unsigned n = 0;; n++) {
-                const int s = (int)(n % TMA_NSLOT);
-                if (n >= TMA_NSLOT) mbar_wait(empty + s, ((n / TMA_NSLOT) - 1) & 1);   // the slot's previous tile is retired
-                const unsigned t = atomicAdd(F.ticket, 1u);
-                if (t >= o.total) { desc[s * 3] = -1; tma_mbar_arrive(full + s); break; }   // end marker, no bytes
-                bool z;
-                unsigned plane, idx;
-                fused2_decode(o, t, z, plane, idx);
-                desc[s * 3 + 0] = z ? 0 : 1; desc[s * 3 + 1] = (int)plane; desc[s * 3 + 2] = (int)idx;
-                if (!z) {   // every Z tile of the plane is stored
-                    unsigned long long v;
-                    SpinGuard guard;
-                    for (;;) {
-                        asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(F.plane_done + plane) : "memory");
-                        if (v >= F.target) break;
-                        __nanosleep(64);
-                        guard.tick();
-                    }
-                    asm volatile("fence.proxy.async;" ::: "memory");   // the acquired data is read through the async proxy
-                }
-                mbar_expect_tx(full + s, G_::TILE_BYTES);
-                if (z) tma_bulk_g2s_hint(slot(s), A.src + ((long long)plane * o.GA + idx) * (C * N), G_::TILE_BYTES, full + s, read_once);
-                else {
+            unsigned n_load = 0;    // ring position of the next ticket
+            unsigned n_store = 0;   // ring position of the next tile the consumers hand back; every earlier slot is free
+            bool waiting = false;   // the ticket at n_load is a Y tile whose plane is not complete yet
+            bool ended = false;     // the end marker is in the ring
+            bool pend = false;      // the last store issued is a Z tile's, not yet known complete
+            unsigned pend_plane = 0, pend_ticket = 0;
+            auto publish = [&]() {   // the pending tile's store is complete
+                stamp(pend_ticket, FZS_RETIRED);
+                asm volatile("fence.proxy.async;" ::: "memory");
+                __threadfence();
+                atomicAdd(F.plane_done + pend_plane, 1ull);
+                pend = false;
+            };
+            SpinGuard guard;
+            for (;;) {
+                bool acted = false;
+                // a transformed tile: store it, and free its slot as soon as the store has read it
+                const int ss = (int)(n_store % TMA_NSLOT);
+                if (n_store < n_load && mbar_test_wait(done + ss, (n_store / TMA_NSLOT) & 1)) {
+                    const int role = desc[ss * 3 + 0], plane = desc[ss * 3 + 1], idx = desc[ss * 3 + 2];
+                    if (role < 0) break;
+                    const unsigned t = STAMPS ? slot_ticket[ss] : 0u;
+                    cx<T>* buf = slot(ss);
+                    // policies made at the point of use: held across the loop they cost spill slots
+                    if (role == 0) tma_bulk_s2g_hint(A.mid + ((long long)plane * o.GA + idx) * (C * N), buf, G_::TILE_BYTES, l2_policy_evict_last());
+                    else {
+                        const uint64_t write_once = l2_policy_evict_first();
 #pragma unroll
-                    for (int r = 0; r < NBOX; r++) tma_tensor_g2s_3d(slot(s) + r * ROWS * C, &map_mid, (int)idx * C * 2, r * ROWS, (int)plane, full + s);
+                        for (int r = 0; r < NBOX; r++) tma_tensor_s2g_3d_hint(map_mid, idx * C * 2, r * ROWS, plane, buf + r * ROWS * C, write_once);
+                    }
+                    tma_commit();
+                    stamp(t, FZS_STORE);
+                    tma_wait_read<0>();
+                    stamp(t, FZS_FREED);
+                    if (pend) { tma_wait_all<1>(); publish(); }   // the pending tile's store is older than this one: complete
+                    if (role == 0) { pend = true; pend_plane = (unsigned)plane; pend_ticket = t; }
+                    else stamp(t, FZS_RETIRED);   // nothing waits for a Y tile's completion but the kernel's end
+                    n_store++;
+                    acted = true;
+                }
+                // a free slot: draw the next ticket and load its tile (a Y tile once its plane is complete)
+                if (!ended && !waiting && n_load < n_store + TMA_NSLOT) {
+                    const int s = (int)(n_load % TMA_NSLOT);
+                    const unsigned t = atomicAdd(F.ticket, 1u);
+                    if (t >= o.total) {   // end marker, no bytes
+                        desc[s * 3] = -1;
+                        tma_mbar_arrive(full + s);
+                        ended = true;
+                        n_load++;
+                    } else {
+                        bool z;
+                        unsigned plane, idx;
+                        fused2_decode(o, t, z, plane, idx);
+                        desc[s * 3 + 0] = z ? 0 : 1; desc[s * 3 + 1] = (int)plane; desc[s * 3 + 2] = (int)idx;
+                        if constexpr (STAMPS) {
+                            slot_ticket[s] = t;
+                            A.stamps[(size_t)t * FZY_NSTAMP + FZS_WHO] = blockIdx.x * 2u + (z ? 0u : 1u);
+                            stamp(t, FZS_TICKET);
+                        }
+                        if (z) {
+                            stamp(t, FZS_DEP);
+                            mbar_expect_tx(full + s, G_::TILE_BYTES);
+                            tma_bulk_g2s_hint(slot(s), A.src + ((long long)plane * o.GA + idx) * (C * N), G_::TILE_BYTES, full + s, l2_policy_evict_first());
+                            stamp(t, FZS_LOAD);
+                            n_load++;
+                        } else waiting = true;
+                    }
+                    acted = true;
+                }
+                if (waiting) {   // every Z tile of the plane is stored
+                    const int s = (int)(n_load % TMA_NSLOT);
+                    unsigned long long v;
+                    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(F.plane_done + desc[s * 3 + 1]) : "memory");
+                    if (v >= F.target) {
+                        asm volatile("fence.proxy.async;" ::: "memory");   // the acquired data is read through the async proxy
+                        stamp(slot_ticket[s], FZS_DEP);
+                        mbar_expect_tx(full + s, G_::TILE_BYTES);
+#pragma unroll
+                        for (int r = 0; r < NBOX; r++)
+                            tma_tensor_g2s_3d(slot(s) + r * ROWS * C, map_mid, desc[s * 3 + 2] * C * 2, r * ROWS, desc[s * 3 + 1], full + s);
+                        stamp(slot_ticket[s], FZS_LOAD);
+                        waiting = false;
+                        n_load++;
+                        acted = true;
+                    }
+                }
+                if (acted) { guard = SpinGuard{}; continue; }
+                // nothing to do: publish the pending tile now rather than with the next store, since Y tiles of other CTAs
+                // (or the very Y ticket this CTA waits on) may be waiting for it
+                if (pend) {
+                    tma_wait_all<0>();
+                    publish();
+                } else {
+                    if (waiting) __nanosleep(64);
+                    guard.tick();
                 }
             }
+            tma_wait_all<0>();
+            if (pend) publish();
+            const unsigned left = atomicAdd(F.ticket + 1, 1u);   // the last CTA to leave re-arms the ticket counter
+            if (left == gridDim.x - 1) { F.ticket[0] = 0; F.ticket[1] = 0; __threadfence(); }
         }
         return;
     }
 
-    // ---- consumers ----
-    int prev_role = -1, prev_slot = 0;
-    unsigned prev_plane = 0;
-    auto retire_prev = [&]() {   // thread 0, the previous tile's store is complete
-        tma_mbar_arrive(empty + prev_slot);
-        if (prev_role == 0) {
-            asm volatile("fence.proxy.async;" ::: "memory");
-            __threadfence();
-            atomicAdd(F.plane_done + prev_plane, 1ull);
-        }
-        prev_role = -1;
-    };
+    // ---- consumers: transform the slots in ring order and hand each back to the mover ----
     for (unsigned n = 0;; n++) {
         const int s = (int)(n % TMA_NSLOT);
-        const uint32_t ph = (n / TMA_NSLOT) & 1;
-        if (tid == 0) {
-            SpinGuard guard;
-            while (!mbar_try_wait(full + s, ph)) {
-                if (prev_role >= 0) { tma_wait_all<0>(); retire_prev(); }
-                guard.tick();
+        unsigned long long ready = 0;
+        if constexpr (STAMPS) ready = gtime_ns();
+        mbar_wait(full + s, (n / TMA_NSLOT) & 1);
+        const int role = desc[s * 3 + 0];
+        if (role < 0) {   // end marker: pass it on, so that the mover stops after the last store
+            if (tid == 0) tma_mbar_arrive(done + s);
+            break;
+        }
+        if constexpr (STAMPS) {
+            if (tid == 0) {
+                A.stamps[(size_t)slot_ticket[s] * FZY_NSTAMP + FZS_READY] = ready;
+                stamp(slot_ticket[s], FZS_FULL);
             }
         }
-        mbar_wait(full + s, ph);
-        const int role = desc[s * 3 + 0], plane = desc[s * 3 + 1], idx = desc[s * 3 + 2];
-        if (role < 0) break;
         cx<T>* buf = slot(s);
         cx<T> v[S::R];
-        if (role == 0) {
+        if constexpr ((PROBE & FZY_MOVE) != 0) {
+            // the twin: the slot leaves as it arrived
+        } else if (role == 0) {
             const int t = tid % TT, c = tid / TT;
 #pragma unroll
             for (int u = 0; u < S::R; u++) v[u] = buf[tma_idx<LAY_LINE, N, C>(c, t + u * TT)];
@@ -370,27 +481,28 @@ __global__ void __launch_bounds__(S::T* C + 32, 1) fft_tma_fused_zy_kernel(const
 #pragma unroll
             for (int u = 0; u < S::R; u++) buf[tma_idx<LAY_COL, N, C>(c, t + u * TT)] = v[u];
         }
-        tma_fence_smem_writes();
+        tma_fence_smem_writes();   // generic-proxy writes -> visible to the mover's TMA store
         tma_sync<true, NT>();
         if (tid == 0) {
-            // policies made at the point of use: held across the loop they cost thread 0 spill slots
-            if (role == 0) tma_bulk_s2g_hint(A.mid + ((long long)plane * o.GA + idx) * (C * N), buf, G_::TILE_BYTES, l2_policy_evict_last());
-            else {
-                const uint64_t read_once = l2_policy_evict_first();
-#pragma unroll
-                for (int r = 0; r < NBOX; r++) tma_tensor_s2g_3d_hint(&map_mid, idx * C * 2, r * ROWS, plane, buf + r * ROWS * C, read_once);
-            }
-            tma_commit();
-            if (prev_role >= 0) { tma_wait_all<1>(); retire_prev(); }
-            prev_role = role; prev_plane = (unsigned)plane; prev_slot = s;
+            stamp(slot_ticket[s], FZS_DONE);
+            tma_mbar_arrive(done + s);
         }
     }
-    if (tid == 0) {
-        tma_wait_all<0>();
-        if (prev_role >= 0) retire_prev();
-        const unsigned left = atomicAdd(F.ticket + 1, 1u);   // the last CTA to leave re-arms the ticket counter
-        if (left == gridDim.x - 1) { F.ticket[0] = 0; F.ticket[1] = 0; __threadfence(); }
-    }
+}
+
+template <class S, typename T, int C>
+__global__ void __launch_bounds__(S::T* C + 32, 1) fft_tma_fused_zy_kernel(const TmaFusedArgs<T> A, const FusedCtl F,
+                                                                            const __grid_constant__ CUtensorMap map_mid)
+{
+    tma_fused_zy_body<S, T, C, 0>(A, F, &map_mid);
+}
+
+// the measurement instantiations (FZY_MOVE, FZY_STAMPS), launched like fft_tma_fused_zy_kernel
+template <class S, typename T, int C, int PROBE>
+__global__ void __launch_bounds__(S::T* C + 32, 1) fft_tma_fused_zy_probe_kernel(const TmaFusedArgs<T> A, const FusedCtl F,
+                                                                                  const __grid_constant__ CUtensorMap map_mid)
+{
+    tma_fused_zy_body<S, T, C, PROBE>(A, F, &map_mid);
 }
 
 }  // namespace dfft
