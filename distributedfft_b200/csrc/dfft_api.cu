@@ -2376,19 +2376,20 @@ extern "C" void* dfft_plan_stream(dfft_plan p) { return p ? (void*)p->stream : n
 // (3dmpifft_opt/include/templateFFT.h:361-365 initializeFFT / launchFFTKernel / deleteFFT)
 // ------------------------------------------------------------------------------------------------
 // launches of the lines engine beyond the pass kinds: X + Y of whole e->N x e->N planes in one launch of e->plane (PlaneArgs),
-// and the whole 2-D convolution of whole images in one launch of e->plane_conv (PlaneConvArgs)
-enum { LK_PLANE = PK_COUNT, LK_PLANE_CONV };
+// the whole 2-D convolution of whole images in one launch of e->plane_conv (PlaneConvArgs), and the whole 1-D convolution of
+// contiguous lines in one launch of e->line_conv (LineConvArgs) or, real lines, e->line_conv_r2c (RealLineConvArgs)
+enum { LK_PLANE = PK_COUNT, LK_PLANE_CONV, LK_LINE_CONV, LK_LINE_CONV_R2C };
 enum { LB_IN = 0, LB_TEMP = 1, LB_OUT = 2 };
 struct LinePass {
     const SizeEntry* e = nullptr;
-    int kind = PK_Z;             // a PassKind, LK_PLANE or LK_PLANE_CONV
+    int kind = PK_Z;             // a PassKind or an LK_ launch kind
     void* lut = nullptr;
     Affine ia{}, oa{};           // plane kinds, for the records: plane (image), 0, row and point strides
     int G = 0, W = 0;
     long long ntiles = 0;        // plane kinds: planes (images)
     long long tw_n = 0;          // four-step twiddle modulus (PK_XF_TW)
     int src = LB_IN, dst = LB_IN;   // LB_IN (the caller's data / a real or convolve plan's `in`), LB_TEMP (the plan's temporary), LB_OUT
-    long long ld_in = 0, ld_out = 0;   // PK_Z_R2C / PK_Z_C2R: distance between the two lines of a pair (RealZArgs), each side's elements
+    long long ld_in = 0, ld_out = 0;   // PK_Z_R2C / PK_Z_C2R / LK_LINE_CONV_R2C: distance between the two lines of a pair (RealZArgs), each side's elements
     bool inv = false;            // the inverse transform
 };
 // which execute runs a plan: dfft_lines_execute, dfft_lines_execute_real or dfft_lines_execute_convolve
@@ -2396,6 +2397,7 @@ enum LinesForm { LF_COMPLEX, LF_REAL, LF_CONV };
 struct dfft_lines_plan_s {
     int prec = 0, device = 0, sms = 132;
     LinesForm form = LF_COMPLEX;
+    bool real = false;           // convolve: real in / real out (dfft_lines_execute_convolve's element size and buffer extents)
     // the passes of one execute in order, [0] forward, [1] backward (a convolve plan has one list, [0]).  The create path launches
     // them and the dfft_debug_lines*_ops hooks record them, both through line_pass
     LinePass run[2][5];
@@ -2420,7 +2422,8 @@ static bool fits_int(long long a, long long b = 1, long long c = 1)
 }
 
 // the plain pass kind whose tile size (kind_C) and twiddle schedule (upload_lut_kind) a lines pass has: the real kernels run the
-// contiguous configuration, the column convolve the strided one, and the plane kernels the contiguous schedule
+// contiguous configuration, the column convolve the strided one, the plane kernels the contiguous schedule and the line convolve
+// kernels the contiguous configuration
 static int plain_kind(int kind)
 {
     return kind == PK_XCONV ? PK_Y : (kind == PK_Z_R2C || kind == PK_Z_C2R || kind >= PK_COUNT) ? PK_Z : kind;
@@ -2671,11 +2674,55 @@ static int make_lines_conv(dfft_lines_plan p, int dims, int nx, int ny, int nz, 
     p->nrun[0] = k;
     p->nrun[1] = 0;
     p->form = LF_CONV;
+    p->real = real;
     p->batch = batch;
     p->mvol = real ? vol / nx * (nx / 2 + 1) : vol;
     if (real) p->rcount = vol * batch;
     else p->ccount = vol * batch;
     p->scale = (flags & DFFT_SCALE_BACKWARD) ? 1.0 / (double)vol : 0.0;
+    return 0;
+}
+
+// ---- batched 1-D spectral convolution on the lines engine: out = ifft(fft(in) * m) per line, or irfft(rfft(in) * m, n) -------
+// `nlines` densely packed lines of n points, convolved in ONE pass in -> out: LINE_CONV (fft_line_conv_kernel, C lines per tile)
+// or LINE_CONV_R2C (fft_line_conv_r2c_kernel, C line pairs per tile, as the real lines plan's R2C pass).  One sweep of the batch
+// in, one out, and the multiplier.  n needs a tuned default entry (dfft_length_kind == 2); generic lengths and lines longer than
+// one shared-memory line (the four-step plan) have no line-convolution kernel.  The plan needs no temporary
+static int make_lines_conv_1d(dfft_lines_plan p, int n, long long nlines, bool real, unsigned flags)
+{
+    if (flags & ~DFFT_SCALE_BACKWARD) return fail(DFFT_EINVAL, "convolve lines plans take no flag but DFFT_SCALE_BACKWARD");
+    if (n < 1 || nlines < 0 || bad_precision(p->prec)) return fail(DFFT_EINVAL, "bad arguments");
+    if (real && n < 2) return fail(DFFT_EUNSUPPORTED, "real lines of %d points: a real convolution needs at least 2", n);
+    const SizeEntry* e = find_size_entry(n, p->prec);
+    if (!e || e->gen || !(real ? e->line_conv_r2c : e->line_conv))
+        return fail(DFFT_EUNSUPPORTED, "length %d has no line-convolution kernel: it needs a tuned length (dfft_length_kind == 2) of the default "
+                    "kernel table; generic lengths and lines longer than one shared-memory line are not convolved", n);
+    if (!fits_int(nlines)) return fail(DFFT_EUNSUPPORTED, "%lld lines: at most 2^31 - 1 per plan", nlines);
+    const int C = e->z_C;
+    LinePass& lp = p->run[0][0];
+    lp.e = e;
+    lp.src = LB_IN; lp.dst = LB_OUT;
+    lp.W = (int)nlines;
+    if (real) {
+        lp.kind = LK_LINE_CONV_R2C;
+        lp.G = (int)cdiv(cdiv(nlines, 2), C);
+        lp.ia = lp.oa = Affine{0, 2LL * C * n, 2LL * n, 1};   // tile, pair and point strides (reals)
+        lp.ld_in = lp.ld_out = n;
+    } else {
+        lp.kind = LK_LINE_CONV;
+        lp.G = (int)cdiv(nlines, C);
+        lp.ia = lp.oa = Affine{0, (long long)C * n, n, 1};
+    }
+    lp.ntiles = lp.G;
+    p->nrun[0] = 1;
+    p->nrun[1] = 0;
+    p->form = LF_CONV;
+    p->real = real;
+    p->batch = nlines;
+    p->mvol = real ? n / 2 + 1 : n;
+    if (real) p->rcount = nlines * n;
+    else p->ccount = nlines * n;
+    p->scale = (flags & DFFT_SCALE_BACKWARD) ? 1.0 / (double)n : 0.0;
     return 0;
 }
 
@@ -2778,6 +2825,16 @@ extern "C" int dfft_lines_plan_create_convolve_r2c_3d(int nx, int ny, int nz, lo
     return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv(p, 3, nx, ny, nz, batch, true, flags); });
 }
 
+extern "C" int dfft_lines_plan_create_convolve_1d(int n, long long nlines, int precision, unsigned flags, dfft_lines_plan* plan)
+{
+    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv_1d(p, n, nlines, false, flags); });
+}
+
+extern "C" int dfft_lines_plan_create_convolve_r2c_1d(int n, long long nlines, int precision, unsigned flags, dfft_lines_plan* plan)
+{
+    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv_1d(p, n, nlines, true, flags); });
+}
+
 extern "C" int dfft_lines_plan_create_convolve_2d(int nx, int ny, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
 {
     return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv(p, 2, nx, ny, 1, batch, false, flags); });
@@ -2801,7 +2858,8 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
 {
     const void* src = line_buf(lp.src, in, out, p->temp);
     void* dst = line_buf(lp.dst, in, out, p->temp);
-    const bool conv = lp.kind == PK_XCONV || lp.kind == LK_PLANE_CONV, realk = lp.kind == PK_Z_R2C || lp.kind == PK_Z_C2R;
+    const bool conv = lp.kind == PK_XCONV || lp.kind == LK_PLANE_CONV || lp.kind == LK_LINE_CONV || lp.kind == LK_LINE_CONV_R2C;
+    const bool realk = lp.kind == PK_Z_R2C || lp.kind == PK_Z_C2R || lp.kind == LK_LINE_CONV_R2C;
     ConvArgs<T> c{};
     TileArgs<T>& a = c.t;
     a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)lp.lut;
@@ -2812,11 +2870,13 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
         c.mult = (const cx<T>*)mult; c.mult_shared = shared ? 1 : 0;
     }
     if (ops) {
-        char extra[128] = "";
-        if (realk) snprintf(extra, sizeof(extra), ", \"nzh\": %d, \"pair\": [%lld, %lld]", lp.e->N / 2 + 1, lp.ld_in, lp.ld_out);
-        if (conv) snprintf(extra, sizeof(extra), ", \"mult\": %llu, \"shared\": %d", (unsigned long long)(size_t)mult, shared ? 1 : 0);
-        const bool plane = lp.kind >= PK_COUNT;
-        const char* name = lp.kind == LK_PLANE ? "XY_PLANE" : lp.kind == LK_PLANE_CONV ? "XY_PLANE_CONV" : kPassNames[lp.kind];
+        char extra[192] = "";
+        int len = 0;
+        if (realk) len = snprintf(extra, sizeof(extra), ", \"nzh\": %d, \"pair\": [%lld, %lld]", lp.e->N / 2 + 1, lp.ld_in, lp.ld_out);
+        if (conv) snprintf(extra + len, sizeof(extra) - len, ", \"mult\": %llu, \"shared\": %d", (unsigned long long)(size_t)mult, shared ? 1 : 0);
+        const bool plane = lp.kind == LK_PLANE || lp.kind == LK_PLANE_CONV;
+        const char* name = lp.kind == LK_PLANE ? "XY_PLANE" : lp.kind == LK_PLANE_CONV ? "XY_PLANE_CONV" : lp.kind == LK_LINE_CONV ? "LINE_CONV"
+                         : lp.kind == LK_LINE_CONV_R2C ? "LINE_CONV_R2C" : kPassNames[lp.kind];
         record_op<T>(*ops, name, phase, lp.e->N, plane ? lp.e->N : kind_C(lp.e, plain_kind(lp.kind)), false, false, lp.kind == PK_XF_TW, a, extra);
         return cudaSuccess;
     }
@@ -2833,6 +2893,14 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
     case PK_Z_R2C: case PK_Z_C2R: {
         const RealZArgs<T> r{a, (const T*)src, (T*)dst, lp.ld_in, lp.ld_out};
         return lp.e->launch[lp.kind](&r, p->sms, p->stream);
+    }
+    case LK_LINE_CONV: {
+        const LineConvArgs<T> lc{a, c.mult, shared ? 0 : (long long)lp.e->N};
+        return lp.e->line_conv(&lc, p->sms, p->stream);
+    }
+    case LK_LINE_CONV_R2C: {
+        const RealLineConvArgs<T> lc{{a, (const T*)src, (T*)dst, lp.ld_in, lp.ld_out}, c.mult, shared ? 0 : (long long)(lp.e->N / 2 + 1)};
+        return lp.e->line_conv_r2c(&lc, p->sms, p->stream);
     }
     default:
         return lp.e->launch[lp.kind](conv ? (const void*)&c : (const void*)&a, p->sms, p->stream);
@@ -2882,9 +2950,9 @@ extern "C" int dfft_lines_execute_real(dfft_lines_plan p, const void* in, void* 
 extern "C" int dfft_lines_execute_convolve(dfft_lines_plan p, const void* in, void* out, const void* mult, long long mult_count)
 {
     if (!p || !in || !out || !mult) return fail(DFFT_EINVAL, "bad arguments");
-    if (p->form != LF_CONV) return fail(DFFT_EINVAL, "dfft_lines_execute_convolve needs a plan from dfft_lines_plan_create_convolve_[r2c_]2d / _3d");
+    if (p->form != LF_CONV) return fail(DFFT_EINVAL, "dfft_lines_execute_convolve needs a plan from dfft_lines_plan_create_convolve_[r2c_]1d / _2d / _3d");
     if (mult_count != 1 && mult_count != p->batch) return fail(DFFT_EINVAL, "mult_count must be 1 or the plan's batch (%lld), not %lld", p->batch, mult_count);
-    const bool real = p->run[0][0].kind == PK_Z_R2C;   // a real plan's first pass is the R2C pass
+    const bool real = p->real;
     const size_t rsz = p->prec == DFFT_FLOAT ? 4 : 8, csz = 2 * rsz, esz = real ? rsz : csz;
     const uintptr_t a = (uintptr_t)in, b = (uintptr_t)out, m = (uintptr_t)mult;
     if (a % esz || b % esz || m % csz) return fail(DFFT_EINVAL, "a buffer is not aligned to its element size");
@@ -2970,6 +3038,19 @@ extern "C" long long dfft_debug_lines_conv_2d_ops(int nx, int ny, long long batc
     auto build = [&](dfft_lines_plan p) {
         const int rc = make_lines_conv(p, 2, nx, ny, 1, batch, real != 0, flags);
         return rc || mult_count == 1 || mult_count == batch ? rc : fail(DFFT_EINVAL, "mult_count must be 1 or the plan's batch");
+    };
+    return lines_ops_json(precision, build, 0, 5, 2, mult_count == 1, buf, cap);
+}
+
+/* test hook (host only): the pass of a 1-D convolve lines plan, JSON as dfft_debug_lines_conv_3d_ops (in = buffer 5, out = 2,
+ * multiplier = 8 of device 0).  The record is "LINE_CONV" (real != 0: "LINE_CONV_R2C", which also carries "nzh" and "pair") with
+ * C = lines (line pairs) per tile, G = ntiles tiles, W = lines, "mult" and "shared" */
+extern "C" long long dfft_debug_lines_conv_1d_ops(int n, long long nlines, int precision, int real, unsigned flags, long long mult_count,
+                                                  char* buf, long long cap)
+{
+    auto build = [&](dfft_lines_plan p) {
+        const int rc = make_lines_conv_1d(p, n, nlines, real != 0, flags);
+        return rc || mult_count == 1 || mult_count == nlines ? rc : fail(DFFT_EINVAL, "mult_count must be 1 or the plan's line count");
     };
     return lines_ops_json(precision, build, 0, 5, 2, mult_count == 1, buf, cap);
 }

@@ -67,6 +67,9 @@ struct SizeEntry {
                           // default entries of N = 16, 32, 64 only (both roles share one schedule there), else nullptr
     PlaneLaunchFn plane_conv;   // set where `plane` is: the 2-D convolution of whole N x N images in one kernel
                                 // (fft_plane_conv_kernel, args = PlaneConvArgs<T>), else nullptr
+    // 1-D convolution of contiguous lines in one pass, in the contiguous configuration; default entries only, else nullptr
+    PassLaunchFn line_conv;       // complex lines (fft_line_conv_kernel, args = LineConvArgs<T>)
+    PassLaunchFn line_conv_r2c;   // real lines, two per complex transform (fft_line_conv_r2c_kernel, args = RealLineConvArgs<T>)
 };
 
 // whether fft_plane_kernel is the default for (N, prec) (measured against the two separate passes, dfft_kernels_common.cu)

@@ -105,6 +105,38 @@ cudaError_t launch_conv(const void* vargs, int sm_count, cudaStream_t st)
     return launch_conv_k<S, T, C, TW, CO, MINB, PP, false>(a, sm_count, st);
 }
 
+// 1-D convolution of contiguous lines (fft_line_conv_kernel: vargs is a LineConvArgs<T>; R2C: fft_line_conv_r2c_kernel, vargs is
+// a RealLineConvArgs<T>)
+template <class S, typename T, int C, bool TW, int MINB, bool PP, bool R2C>
+cudaError_t launch_line_conv(const void* vargs, int sm_count, cudaStream_t st)
+{
+    const TileArgs<T>& a = R2C ? reinterpret_cast<const RealLineConvArgs<T>*>(vargs)->r.t : reinterpret_cast<const LineConvArgs<T>*>(vargs)->t;
+    auto kern = [] {   // only the kernel of this kind is instantiated
+        if constexpr (R2C) return fft_line_conv_r2c_kernel<S, T, C, TW, MINB, PP>;
+        else return fft_line_conv_kernel<S, T, C, TW, MINB, PP>;
+    }();
+    constexpr size_t smem = TileSmem<S, T, C, PP>::bytes(false);
+    static std::atomic<int> occ_cache[64];
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    int occ = occ_cache[dev & 63].load();
+    if (occ == 0) {
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, S::T * C, smem);
+        if (e != cudaSuccess) return e;
+        if (occ < 1) return cudaErrorLaunchOutOfResources;
+        occ_cache[dev & 63].store(occ);
+    }
+    if (a.ntiles <= 0) return cudaSuccess;
+    long long grid = (long long)sm_count * occ;
+    if (grid > a.ntiles) grid = a.ntiles;
+    if constexpr (R2C) kern<<<(unsigned)grid, S::T * C, smem, st>>>(*reinterpret_cast<const RealLineConvArgs<T>*>(vargs));
+    else kern<<<(unsigned)grid, S::T * C, smem, st>>>(*reinterpret_cast<const LineConvArgs<T>*>(vargs));
+    return cudaGetLastError();
+}
+
 // X + Y passes of square planes (fft_plane_kernel): vargs is a PlaneArgs<T>; P planes per CTA
 template <class S, typename T, int P, int MINB>
 cudaError_t launch_plane(const void* vargs, int sm_count, cudaStream_t st)
@@ -346,6 +378,10 @@ SizeEntry make_entry(int variant = 0)
         // spectral convolution along x (the X axis of a convolve plan uses this entry's strided schedule and twiddle table)
         e.launch[PK_XCONV] = launch_conv<SS, T, Y::C, Y::TW, false, Y::MB, Y::PP>;
         e.launch[PK_XCONV_CO] = launch_conv<SS, T, PEER::C, PEER::TW, true, PEER::MB, PEER::PP>;
+        // 1-D convolution of contiguous lines in the contiguous configuration: the complex kernel with the Z pass's register
+        // budget, the real one with the real kernels' (shared-memory twiddles, MBI)
+        e.line_conv = launch_line_conv<ZS, T, Z::C, Z::TW, Z::MB, Z::PP, false>;
+        e.line_conv_r2c = launch_line_conv<ZS, T, Z::C, false, MBI, Z::PP, true>;
         // X and Y passes of whole square planes in one kernel, where both roles share one schedule (and so one twiddle table).
         // Register budget: 64 per thread (2 CTAs of 512 / 4 of 256 threads), except 32-point fp64, which spills at 64 and is
         // given 85 (3 CTAs of 256); 64-point fp64 keeps 2 CTAs of 512 with a small spill (DESIGN.md section 3.8)

@@ -504,6 +504,62 @@ __global__ void __launch_bounds__(S::T* C, MINB) fft_conv_shared_kernel(const Co
 }
 
 // ------------------------------------------------------------------------------------------
+// 1-D spectral convolution of contiguous lines: forward FFT, pointwise multiply and inverse FFT of every line in ONE pass (the 1-D
+// convolve lines plans).  The contiguous (Z) configuration with MAP_T on both sides: after the last stage thread (t, c) holds the
+// points t + u*T of line c, the points it loaded, so the multiplier element of each register is m[line * mult_line + t + u*T] and
+// the inverse run starts from the same register layout -- conv_tiles' argument, along the line instead of across columns.  Tile
+// `tile` holds lines tile*C + c at  base + tile*SB + c*cs + e*es;  lines from W on load zero, read no multiplier and store nothing.
+// Unnormalised (x N); TileArgs::do_scale folds TileArgs::scale into the multiply; TileArgs::inv is unused.  Every element of a
+// tile is in registers before any of it is stored, so in == out is safe.  A kernel of its own: conv_tiles is left as it is.
+// ------------------------------------------------------------------------------------------
+template <typename T> struct LineConvArgs {
+    TileArgs<T> t;
+    const cx<T>* mult;
+    long long mult_line;   // multiplier elements between lines: 0 (one multiplier for every line) or N
+};
+
+template <class S, typename T, int C, bool TWREG, int MINB, bool PINGPONG>
+__global__ void __launch_bounds__(S::T* C, MINB) fft_line_conv_kernel(const LineConvArgs<T> R)
+{
+    static_assert(S::valid(), "bad schedule");
+    using Op = TileOp<S, T, C, MAP_T, MAP_T, TWREG, false, false, PINGPONG>;
+    constexpr int RR = S::R, TT = S::T;
+    const TileArgs<T>& A = R.t;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    typename Op::Ctx k;
+    Op::setup(A, smem_raw, smem_raw + Op::SM::exch_bytes, k);
+    cx<T> twr[Op::NTW];
+    Op::load_twiddles(k, twr);
+    const int t = k.t_in, c = k.c_in;   // MAP_T on both sides: t_out == t_in, c_out == c_in
+    const bool do_scale = A.do_scale != 0;
+    for (long long tile = blockIdx.x; tile < A.ntiles; tile += gridDim.x) {
+        const long long line = tile * C + c;
+        const bool ok = line < A.W;
+        const cx<T>* p = A.in + tile * A.ia.SB + c * A.ia.cs + (long long)t * A.ia.es;
+        const cx<T>* mp = R.mult + line * R.mult_line + t;
+        cx<T> v[RR];
+#pragma unroll
+        for (int u = 0; u < RR; u++) v[u] = ok ? ld_stream(p + (long long)u * TT * A.ia.es) : mk<T>(0, 0);
+        StageRunner<S, 0, T, C, MAP_T, MAP_T, TWREG, PINGPONG>::run(v, t, c, t, c, k.exch, k.pp, k.lut_s, twr, [] {});
+        // multiply, then the inverse as swap -> forward -> swap (the swap-in is folded into the multiply's result)
+#pragma unroll
+        for (int u = 0; u < RR; u++) {
+            cx<T> m = ok ? ld_stream(mp + u * TT) : mk<T>(0, 0);
+            if (do_scale) { m.x *= A.scale; m.y *= A.scale; }
+            v[u] = cswap(cmul(v[u], m));
+        }
+        // the inverse run's first scatter reuses the exchange buffer: every thread's last gather of the forward run is done
+        __syncthreads();
+        StageRunner<S, 0, T, C, MAP_T, MAP_T, TWREG, PINGPONG>::run(v, t, c, t, c, k.exch, k.pp, k.lut_s, twr, [] {});
+        if (ok) {
+            cx<T>* q = A.out + tile * A.oa.SB + c * A.oa.cs + (long long)t * A.oa.es;
+#pragma unroll
+            for (int u = 0; u < RR; u++) st_stream(q + (long long)u * TT * A.oa.es, cswap(v[u]));
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------
 // Two dependent passes over the same planes in ONE persistent kernel (t0 = Z then Y forward, Y then Z
 // backward): the reference runs them as two launches per plane (fft_mpi_3d_api.cpp:496-502), we ran
 // them as two full HBM sweeps; here a plane's intermediate is produced and consumed while it is still

@@ -1,19 +1,19 @@
 #!/usr/bin/env python
-"""Batched 3-D (or, with --dims 2, 2-D) spectral convolution: the convolve lines plan against the three calls it replaces, one
-GPU (developer tool).
+"""Batched 3-D (or, with --dims 2 / --dims 1, 2-D / 1-D) spectral convolution: the convolve lines plan against the three calls it
+replaces, one GPU (developer tool).
 
-    python distributedfft_b200/csrc/tools/lines_conv_bench.py [--dims 3|2] [--steps 30] [--rounds 3] [--warmup 5] [--case NAME]
+    python distributedfft_b200/csrc/tools/lines_conv_bench.py [--dims 3|2|1] [--steps 30] [--rounds 3] [--warmup 5] [--case NAME]
 
-Every case convolves `batch` volumes (images) with one multiplier of unit modulus / N (so repeated in-place steps keep their
-magnitude).  The arms get the same seeded data:
+Every case convolves `batch` volumes (images, lines) with one multiplier of unit modulus / N (so repeated in-place steps keep
+their magnitude).  The arms get the same seeded data:
   shared   LinesConvolvePlan, one multiplier for every volume (mult_count = 1), out of place
   pervol   the same plan with `batch` identical copies of the multiplier (mult_count = batch)
   noplane  (--dims 2, square 16 / 32 / 64 images) the plan created under DFFT_NO_PLANE=1 (X, XCONV, inverse X), shared
            multiplier; the shared and pervol plans are then created under DFFT_FORCE_PLANE=1, so that the one-kernel
            convolution is timed whatever kPlaneConvUse says
-  3call    LinesPlan(three_d=... / two_d=...) forward in place, torch multiply by the shared multiplier, LinesPlan backward
+  3call    LinesPlan(three_d=... / two_d=... / n, nlines) forward in place, torch multiply by the shared multiplier, LinesPlan backward
            (real: RealLinesPlan forward into a spectrum buffer, multiply, backward into the output)
-  torch    torch.fft.fftn * m -> ifftn (rfftn / irfftn for real cases; cuFFT, for context)
+  torch    torch.fft.fftn * m -> ifftn over the last 3 / 2 / 1 axes (rfftn / irfftn for real cases; cuFFT, for context)
 Before timing, the outputs of all arms are compared: shared against pervol and noplane with torch.equal (bit-identical by
 construction), 3call and torch by rel_l2 against shared.  Each round times `steps` executes of each arm with CUDA events on the
 arm's own stream (the plans' streams; torch's current stream for torch), arms alternating, after `warmup` untimed executes.
@@ -26,6 +26,8 @@ of each arm in bytes with its GB/s at the measured time (V = one sweep of the ba
   2-D C2C plane shape  conv 2V + M      noplane 6V + M    3call 10V + M
   2-D C2C other        conv 6V + M      3call 10V + M
   2-D real             conv 2Vr + 4Vc + M   3call 2Vr + 8Vc + M
+  1-D C2C              conv 2V + M      3call 6V + M
+  1-D real             conv 2Vr + M     3call 2Vr + 4Vc + M
 Card name, power limit and SM clock (nvidia-smi, read-only query) are printed before and after."""
 import argparse
 import json
@@ -54,6 +56,12 @@ CASES_2D = [
     ("48^2x16384", "d", (48, 48, 16384), False), ("256^2x1024", "d", (256, 256, 1024), False),
     ("1024^2x64", "d", (1024, 1024, 64), False),
     ("real-64^2x16384", "d", (64, 64, 16384), True), ("real-512^2x256", "d", (512, 512, 256), True),
+]
+# --dims 1: (n, nlines), about 2^26 complex elements per batch; 768 is mixed radix
+CASES_1D = [
+    ("256x262144", "d", (256, 262144), False), ("1024x65536", "d", (1024, 65536), False), ("4096x16384", "d", (4096, 16384), False),
+    ("1024x65536-f32", "f", (1024, 65536), False), ("768x87381", "d", (768, 87381), False),
+    ("real-1024x65536", "d", (1024, 65536), True), ("real-4096x16384", "d", (4096, 16384), True),
 ]
 
 
@@ -92,10 +100,10 @@ def make_conv(dfft, key, shape, prec, real, env):
 
 def run_case(torch, np, dfft, case, args):
     name, p, shape, real = case
-    two = len(shape) == 3
+    two, one = len(shape) == 3, len(shape) == 2
     nx, batch = shape[0], shape[-1]
-    spatial = tuple(reversed(shape[:-1]))                                             # (nz, ny, nx) or (ny, nx)
-    key = "two_d" if two else "three_d"
+    spatial = tuple(reversed(shape[:-1]))                                             # (nz, ny, nx), (ny, nx) or (n,)
+    key = "one_d" if one else "two_d" if two else "three_d"
     prec = dfft.FLOAT if p == "f" else dfft.DOUBLE
     rdt, cdt = (torch.float32, torch.complex64) if p == "f" else (torch.float64, torch.complex128)
     er = 4 if p == "f" else 8
@@ -113,7 +121,10 @@ def run_case(torch, np, dfft, case, args):
     plane_shape = two and not real and shape[0] == shape[1] and shape[0] in (16, 32, 64)
     conv = make_conv(dfft, key, shape, prec, real, "DFFT_FORCE_PLANE" if plane_shape else None)
     noplane = make_conv(dfft, key, shape, prec, real, "DFFT_NO_PLANE") if plane_shape else None
-    fwd = dfft.RealLinesPlan(**{key: shape}, precision=prec) if real else dfft.LinesPlan(**{key: shape}, precision=prec)
+    if one:
+        fwd = dfft.RealLinesPlan(nx, batch, precision=prec) if real else dfft.LinesPlan(nx, 1, batch, batch, nx, 0, precision=prec)
+    else:
+        fwd = dfft.RealLinesPlan(**{key: shape}, precision=prec) if real else dfft.LinesPlan(**{key: shape}, precision=prec)
     try:
         y = {k: torch.empty_like(x) for k in ("shared", "pervol") + (("noplane",) if noplane else ())}
         z = x.clone()                                                                 # the three-call arm's buffer
@@ -178,7 +189,9 @@ def run_case(torch, np, dfft, case, args):
         if noplane:
             noplane.destroy()
     med = {k: float(np.median([r[k] for r in rounds])) for k in rounds[0]}
-    if two:
+    if one:
+        plane = False
+    elif two:
         plane = plane_shape
     else:
         plane = dfft.lines_conv_3d_ops(*shape, prec, real)[0]["op"] == "XY_PLANE"
@@ -186,11 +199,18 @@ def run_case(torch, np, dfft, case, args):
     Msh, Mpv = Mimg, Mimg * batch
     if real:
         Vr, Vc = er * N * batch, ec * N // nx * H * batch
-        conv_b, call_b = (2 * Vr + 4 * Vc, 2 * Vr + 8 * Vc) if two else (2 * Vr + 8 * Vc, 2 * Vr + 12 * Vc)
-        model = "conv 2Vr+4Vc+M, 3call 2Vr+8Vc+M" if two else "conv 2Vr+8Vc+M, 3call 2Vr+12Vc+M"
+        if one:
+            conv_b, call_b = 2 * Vr, 2 * Vr + 4 * Vc
+            model = "conv 2Vr+M, 3call 2Vr+4Vc+M"
+        else:
+            conv_b, call_b = (2 * Vr + 4 * Vc, 2 * Vr + 8 * Vc) if two else (2 * Vr + 8 * Vc, 2 * Vr + 12 * Vc)
+            model = "conv 2Vr+4Vc+M, 3call 2Vr+8Vc+M" if two else "conv 2Vr+8Vc+M, 3call 2Vr+12Vc+M"
     else:
         V = ec * N * batch
-        if two:
+        if one:
+            conv_b, call_b = 2 * V, 6 * V
+            model = "conv 2V+M, 3call 6V+M"
+        elif two:
             conv_b, call_b = (2 * V if plane else 6 * V), 10 * V
             model = "conv 2V+M, noplane 6V+M, 3call 10V+M" if plane else "conv 6V+M, 3call 10V+M"
         else:
@@ -217,7 +237,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--case", action="append", help="run only these cases (default: all)")
-    ap.add_argument("--dims", type=int, choices=(2, 3), default=3, help="3-D volumes (default) or 2-D images")
+    ap.add_argument("--dims", type=int, choices=(1, 2, 3), default=3, help="3-D volumes (default), 2-D images or 1-D lines")
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -228,7 +248,7 @@ def main():
         os.environ.pop(var, None)
     print(json.dumps({"gpu_before": gpu_state()}), flush=True)
     results = []
-    for case in (CASES_2D if args.dims == 2 else CASES):
+    for case in {1: CASES_1D, 2: CASES_2D, 3: CASES}[args.dims]:
         if args.case and case[0] not in args.case:
             continue
         r = run_case(torch, np, dfft, case, args)

@@ -363,7 +363,20 @@ int dfft_lines_plan_create_convolve_r2c_3d(int nx, int ny, int nz, long long bat
  * dfft_lines_execute_convolve, under the same rules as the 3-D plans. */
 int dfft_lines_plan_create_convolve_2d(int nx, int ny, long long batch, int precision, unsigned flags, dfft_lines_plan* plan);
 int dfft_lines_plan_create_convolve_r2c_2d(int nx, int ny, long long batch, int precision, unsigned flags, dfft_lines_plan* plan);
-/* mult_count = 1: one multiplier shared by every image / volume; = batch: one each, densely packed.  in == out (in place) or
+/* Batched 1-D spectral convolution on the lines engine: nlines densely packed lines of n points,
+ *   C2C: out = ifft(fft(in) * m) per line, unnormalised (x n) unless DFFT_SCALE_BACKWARD;
+ *   R2C: out = irfft(rfft(in) * m, n) * n, real in / real out (the imaginary parts of m[0] and, for even n, m[n/2] are ignored,
+ *        numpy's C2R convention, as in the 2-D and 3-D R2C convolve plans).
+ * m is complex in the plan's precision: [n] (C2C) or [n/2+1] (R2C) per line.  One execute is one launch that reads the batch
+ * once, writes it once and reads the multiplier: forward transform, multiply and inverse transform of every line in registers
+ * and shared memory (R2C: two real lines per complex transform).  No temporary.
+ * Lengths: n needs a tuned kernel of the default table (dfft_length_kind(n, precision) == 2); generic lengths, DFFT_GENERIC and
+ * DFFT_VARIANT entries and lines longer than one shared-memory line are DFFT_EUNSUPPORTED, as is R2C with n < 2.  2^31 or more
+ * lines are DFFT_EUNSUPPORTED.  Flags: DFFT_SCALE_BACKWARD folds 1/n into the multiply; any other bit is DFFT_EINVAL.  Executed
+ * with dfft_lines_execute_convolve (batch = nlines), under the same rules as the 2-D and 3-D plans. */
+int dfft_lines_plan_create_convolve_1d(int n, long long nlines, int precision, unsigned flags, dfft_lines_plan* plan);
+int dfft_lines_plan_create_convolve_r2c_1d(int n, long long nlines, int precision, unsigned flags, dfft_lines_plan* plan);
+/* mult_count = 1: one multiplier shared by every line / image / volume; = batch: one each, densely packed.  in == out (in place) or
  * disjoint buffers; `in` is never written when they are distinct, `mult` never.  DFFT_EINVAL: a null pointer, a buffer not
  * aligned to its element size (fp32 complex at an 8-byte offset is fine), a partial overlap of in and out, a multiplier that
  * overlaps out, another mult_count, and a plan that is not a convolve lines plan (dfft_lines_execute / dfft_lines_execute_real
@@ -377,6 +390,10 @@ long long dfft_debug_lines_conv_3d_ops(int nx, int ny, int nz, long long batch, 
  * ia = oa = [image, 0, row, point] strides, "mult" and "shared" */
 long long dfft_debug_lines_conv_2d_ops(int nx, int ny, long long batch, int precision, int real, unsigned flags,
                                        long long mult_count, char* buf, long long cap);
+/* the same for the 1-D convolve lines plans: one "LINE_CONV" record (real != 0: "LINE_CONV_R2C", which also carries "nzh" and
+ * "pair" as the real lines records) with C lines (line pairs) per tile, ntiles = G tiles, W = nlines, "mult" and "shared" */
+long long dfft_debug_lines_conv_1d_ops(int n, long long nlines, int precision, int real, unsigned flags, long long mult_count,
+                                       char* buf, long long cap);
 /* one-shot convenience (plan + execute + synchronize + destroy), used by the per-axis parity tests */
 int dfft_fft_lines(void* data, int n, long long stride, long long nlines, long long inner, long long inner_dist,
                    long long outer_dist, int direction, int precision);
