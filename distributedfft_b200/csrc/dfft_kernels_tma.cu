@@ -28,6 +28,10 @@ bool tma_available() { return encode_fn() != nullptr; }
 
 // 3-D tensor of complex elements: dim0 (fastest, contiguous) d0, dim1 d1 with stride s1, dim2 d2 with stride s2 (strides in complex
 // elements); box (b0, b1, b2).  `map` points to 128 bytes, 64-byte aligned (a CUtensorMap).
+// L2 promotion: 256 B, except for 128-byte box rows, which are promoted to one row.  Measured on H100 (DESIGN.md 3.4): at
+// 512^3 fp64 (C = 8, 128-byte rows) 256 B took the fused t0 2.08 against 2.05-2.06 ms and the TMA_XF pass 1.61 against
+// 1.58 ms, and 512^3 fp32 (C = 16) was a tie.  Narrower rows (64 B) were not measured apart from run-to-run noise, so they
+// keep 256 B
 int tma_encode_3d(void* map, void* base, int prec, long long d0, long long d1, long long d2, long long s1, long long s2, int b0, int b1, int b2)
 {
     EncodeTiledFn fn = encode_fn();
@@ -37,8 +41,9 @@ int tma_encode_3d(void* map, void* base, int prec, long long d0, long long d1, l
     cuuint64_t strides[2] = {(cuuint64_t)s1 * esz, (cuuint64_t)s2 * esz};
     cuuint32_t box[3] = {(cuuint32_t)b0 * 2, (cuuint32_t)b1, (cuuint32_t)b2};
     cuuint32_t estr[3] = {1, 1, 1};
+    const CUtensorMapL2promotion promo = (size_t)b0 * esz == 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
     const CUresult r = fn((CUtensorMap*)map, prec == 0 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT64 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, base, dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
@@ -58,8 +63,8 @@ static cudaError_t launch_tma(int mode, const void* vargs, const void* map_in, c
     {                                                                                                                       \
         auto kern = fft_tma_pass_kernel<S, T, C, M>;                                                                        \
         static bool attr = false;                                                                                           \
-        if (!attr) { e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_::SMEM); if (e != cudaSuccess) return e; attr = true; } \
-        kern<<<(unsigned)grid, S::T * C, G_::SMEM, st>>>(a, mi, mo);                                                        \
+        if (!attr) { e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_::PASS_SMEM); if (e != cudaSuccess) return e; attr = true; } \
+        kern<<<(unsigned)grid, S::T * C, G_::PASS_SMEM, st>>>(a, mi, mo);                                                   \
     }
     switch (mode) {
         case TMA_Z: DFFT_TMA_LAUNCH(TMA_Z) break;
@@ -90,12 +95,11 @@ static cudaError_t launch_tma_fused_zy(const void* vargs, const FusedCtl* ctl, c
     long long grid = sm_count;
     if (grid > total) grid = total;
     FusedCtl c = *ctl;
-    // the Z role runs ahead of the Y role by the tiles the rings hold beside the one each CTA is transforming
-    // (TMA_NSLOT - 1 per CTA): 3 planes at 512 points on 132 SMs.  Each plane more keeps another 4 MiB of intermediate in
-    // the L2; with the mover publishing Z tiles as soon as it is idle, lag 4 measured 0.02 ms and lag 5 0.17 ms slower on
-    // H100 (DESIGN.md 3.4)
-    if (c.lag <= 0) c.lag = (int)((grid * (TMA_NSLOT - 1) + c.GA + c.GB - 1) / ((long long)c.GA + c.GB));
-    kern<<<(unsigned)grid, G_::NT + 32, G_::SMEM, st>>>(a, c, *reinterpret_cast<const CUtensorMap*>(map_mid));
+    // the Z role runs ahead of the Y role by the tiles the rings hold beside the ones each CTA is transforming
+    // (NSLOT - NGROUP per CTA): 3 planes at 512 points on 132 SMs.  Each plane more keeps another 4 MiB of intermediate in
+    // the L2; on tma_ring at 512^3 fp64 on H100, lag 2 measured 0.15 ms and lag 4 0.03 ms slower than lag 3 (DESIGN.md 3.4)
+    if (c.lag <= 0) c.lag = (int)((grid * (G_::NSLOT - G_::NGROUP) + c.GA + c.GB - 1) / ((long long)c.GA + c.GB));
+    kern<<<(unsigned)grid, TMA_CONSUMERS + 32, G_::SMEM, st>>>(a, c, *reinterpret_cast<const CUtensorMap*>(map_mid));
     return cudaGetLastError();
 }
 

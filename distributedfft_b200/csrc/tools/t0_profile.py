@@ -1,22 +1,24 @@
 #!/usr/bin/env python
-"""Where the time of the fused forward t0 goes (fft_tma_fused_zy_kernel, 512^3 fp64, one GPU; developer tool).
+"""Where the time of the TMA ring kernels goes at 512^3 fp64 on one GPU: the fused forward t0 (fft_tma_fused_zy_kernel) and
+the forward X pass (fft_tma_pass_kernel<TMA_XF>) (developer tool).
 
-    python distributedfft_b200/csrc/tools/t0_profile.py [--lag 4 --lag 3 ...] [--reps 20] [--rounds 3] [--out DIR]
+    python distributedfft_b200/csrc/tools/t0_profile.py [--lag 3 --lag 4 ...] [--reps 20] [--rounds 3] [--out DIR]
 
-Builds t0_profile.cu (the fused kernel's body as the library instantiates it, its movement-only twin and their stamped
-variants, plus a plain TMA copy of the slab) against libdfft.so (run `python -m distributedfft_b200.build` first) into a
-temporary directory, runs it and prints one JSON object:
+Builds t0_profile.cu (the kernel bodies as the library instantiates them at C = 8 and C = 4, their movement-only twins and
+stamped variants, the X pass's pre-mover structure without arithmetic, and a plain TMA copy of the slab) against libdfft.so
+(run `python -m distributedfft_b200.build` first) into a temporary directory, runs it and prints one JSON object:
   - the card's name, power limit and SM clock (nvidia-smi, read-only query) before and after;
-  - ms per launch of the kernel and of its twin at every lag, of the TMA copy and of cudaMemcpyAsync, per round;
-  - from one stamped launch of each at the first lag, per role (Z, Y): median and p90 in microseconds of
-      load_wait     consumer thread 0 waiting for the slot to land (FZS_FULL - FZS_READY)
-      dep_wait      mover waiting for the plane counter (FZS_DEP - FZS_TICKET; 0 for Z tiles)
-      load_latency  load issued to the consumers taking the slot (FZS_FULL - FZS_LOAD; FZS_FULL is when thread 0 saw it full)
-      transform     slot full to transform done (FZS_DONE - FZS_FULL)
-      store_read    store issued to the store having read the slot, which frees it (FZS_FREED - FZS_STORE)
-      store_retire  store issued to complete and published (FZS_RETIRED - FZS_STORE; a Y tile: to its slot freed)
+  - ms per launch of every variant, per round (the rounds alternate the variants), and per variant the min and max;
+  - from one stamped launch of each ring kernel (the fused kernel and its twin at the first lag), per role (Z, Y; the X
+    pass is all role Z): median and p90 in microseconds of
+      load_wait     the consumer group waiting for the slot to land (TMS_FULL - TMS_READY)
+      dep_wait      mover waiting for the plane counter (TMS_DEP - TMS_TICKET; 0 for Z tiles)
+      load_latency  load issued to the consumers taking the slot (TMS_FULL - TMS_LOAD)
+      transform     slot full to transform done (TMS_DONE - TMS_FULL)
+      store_read    store issued to the store having read the slot, which frees it (TMS_FREED - TMS_STORE)
+      store_retire  store issued to complete and published (TMS_RETIRED - TMS_STORE; other tiles: to their slot freed)
     and the ring occupancy: the mean number of tiles a CTA holds in each state over the launch (time in state / span), and the
-    share of the span in which its consumers wait for a load.
+    share of the span in which its consumer groups wait for a load (summed over groups).
 The stamps are %globaltimer values; the tick the card shows is printed as `timer_tick_ns`."""
 import argparse
 import json
@@ -29,7 +31,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.dirname(os.path.dirname(HERE))
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
-WHO, TICKET, DEP, LOAD, READY, FULL, DONE, STORE, FREED, RETIRED, NSTAMP = range(11)   # FZS_* in fft_tma.cuh
+WHO, TICKET, DEP, LOAD, READY, FULL, DONE, STORE, FREED, RETIRED, NSTAMP = range(11)   # TMS_* in fft_tma.cuh
 
 
 def gpu_state():
@@ -79,11 +81,12 @@ def analyse(path):
     }
     out = {"span_ms": round(span / 1e6, 4)}
     for role, m in (("Z", ~y), ("Y", y)):
-        out[role] = {k: stats(v[m]) for k, v in d.items()}
+        if m.any():
+            out[role] = {k: stats(v[m]) for k, v in d.items()}
     # mean tiles per CTA in each state (Little's law: total time in the state / span / CTAs)
     states = {
         "dep_wait": (TICKET, DEP), "issued_to_taken": (LOAD, FULL), "transforming": (FULL, DONE),
-        "store_to_freed": (STORE, FREED), "held": (TICKET, FREED),
+        "done_to_store": (DONE, STORE), "store_to_freed": (STORE, FREED), "held": (TICKET, FREED),
     }
     occ = {}
     for k, (a, b) in states.items():
@@ -109,7 +112,7 @@ def main():
         os.makedirs(out, exist_ok=True)
         before = gpu_state()
         cmd = [exe, "--out", out, "--reps", str(args.reps), "--rounds", str(args.rounds)]
-        for lag in args.lag or [4]:
+        for lag in args.lag or [3]:
             cmd += ["--lag", str(lag)]
         r = subprocess.run(cmd, capture_output=True, text=True)
         after = gpu_state()
@@ -117,8 +120,10 @@ def main():
             sys.exit("t0_profile failed:\n" + r.stdout + r.stderr)
         res = json.loads(r.stdout)
         res["gpu_before"], res["gpu_after"] = before, after
-        res["profile_fused"] = analyse(os.path.join(out, "stamps_fused.bin"))
-        res["profile_twin"] = analyse(os.path.join(out, "stamps_twin.bin"))
+        names = res["rounds"][0].keys()
+        res["spread"] = {k: [min(r[k] for r in res["rounds"]), max(r[k] for r in res["rounds"])] for k in names}
+        for st in res["stamped"]:
+            res["profile_" + st["name"]] = analyse(os.path.join(out, "stamps_%s.bin" % st["name"]))
     print(json.dumps(res, indent=1))
 
 
