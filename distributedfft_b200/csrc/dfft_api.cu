@@ -2429,8 +2429,24 @@ static int plain_kind(int kind)
     return kind == PK_XCONV ? PK_Y : (kind == PK_Z_R2C || kind == PK_Z_C2R || kind >= PK_COUNT) ? PK_Z : kind;
 }
 
-// one pass over `nlines` lines of n points: densely packed contiguous lines (stride 1, PK_Z) or columns (inner_dist 1, PK_Y).
-// The pass's row or column count W is a 32-bit kernel argument
+// columns that touch no element twice: the (extent, stride) pairs (inner, 1), (n, stride) and (mats, outer_dist), sorted by
+// stride, each have a stride at least the span of the ones before (the usual test for a non-overlapping strided tensor; pairs of
+// extent 1 take no part, so a single matrix ignores outer_dist).  A negative outer_dist over two or more matrices fails it.
+static bool columns_disjoint(int n, long long stride, long long inner, long long mats, long long outer_dist)
+{
+    struct Dim { long long extent, stride; } d[3] = {{inner, 1}, {n, stride}, {mats, outer_dist}};
+    std::sort(d, d + 3, [](const Dim& a, const Dim& b) { return a.stride < b.stride; });
+    __int128 span = 1;
+    for (const Dim& x : d) {
+        if (x.extent <= 1) continue;
+        if (x.stride < span) return false;
+        span += (__int128)(x.extent - 1) * x.stride;
+    }
+    return true;
+}
+
+// one pass over `nlines` lines of n points: densely packed contiguous lines (stride 1, PK_Z) or disjoint columns (inner_dist 1,
+// PK_Y).  The pass's row or column count W is a 32-bit kernel argument
 static int make_line_pass(LinePass& lp, int n, long long stride, long long nlines, long long inner, long long inner_dist, long long outer_dist,
                           int precision)
 {
@@ -2448,6 +2464,8 @@ static int make_line_pass(LinePass& lp, int n, long long stride, long long nline
     } else {
         if (inner_dist != 1 || inner < 1 || nlines % inner) return fail(DFFT_EUNSUPPORTED, "strided lines must be columns (inner_dist == 1)");
         if (!fits_int(inner)) return fail(DFFT_EUNSUPPORTED, "%lld columns: at most 2^31 - 1 per pass", inner);
+        if (!columns_disjoint(n, stride, inner, nlines / inner, outer_dist))
+            return fail(DFFT_EINVAL, "columns overlap: %lld columns, n = %d, stride %lld, outer_dist %lld", inner, n, stride, outer_dist);
         const int C = e->s_C;
         lp.G = (int)cdiv(inner, C); lp.W = (int)inner; lp.ntiles = (nlines / inner) * lp.G;
         lp.ia = Affine{outer_dist, C, 1, stride};
@@ -2517,7 +2535,11 @@ static int make_lines_1d(dfft_lines_plan p, int n, long long stride, long long n
                          bool long_lines)
 {
     if (n < 1 || nlines < 0 || stride < 1 || bad_precision(p->prec)) return fail(DFFT_EINVAL, "bad arguments");
-    if (long_lines && !find_size_entry(n, p->prec) && stride == 1 && inner_dist == n) return make_four_step(p, n, nlines);
+    if (long_lines && !find_size_entry(n, p->prec) && stride == 1 && inner_dist == n) {
+        // the four-step passes address the lines as one dense block, as the contiguous pass does
+        if (inner != nlines && outer_dist != inner * n) return fail(DFFT_EUNSUPPORTED, "contiguous lines must be densely packed");
+        return make_four_step(p, n, nlines);
+    }
     const int rc = make_line_pass(p->run[0][0], n, stride, nlines, inner, inner_dist, outer_dist, p->prec);
     return rc ? rc : complex_lists(p, 1, false);
 }

@@ -288,7 +288,12 @@ int dfft_memcpy(void* dst, const void* src, size_t bytes, int kind);
  *    Line l starts at data + (l / inner) * outer_dist + (l % inner) * inner_dist (in elements), points are
  *    `stride` elements apart.  Supported shapes: stride == 1 with densely packed lines (inner_dist == n), or
  *    stride > 1 with inner_dist == 1 (columns of row-major matrices: `inner` columns per matrix, matrices
- *    `outer_dist` apart).  The 2-D plan transforms `batch` row-major ny x nx matrices (nx fastest), the
+ *    `outer_dist` apart; padded rows, gaps between matrices and interleaved matrices are fine).  Columns must not
+ *    overlap: the (extent, stride) pairs (inner, 1), (n, stride) and (nlines / inner, outer_dist), sorted by stride,
+ *    each need a stride at least the span of the ones before ((extent - 1) * stride summed, plus one); pairs of
+ *    extent 1 are left out, so a single matrix (nlines == inner) ignores outer_dist.  An overlapping layout, or a
+ *    negative outer_dist over two or more matrices, is DFFT_EINVAL.  The elements between columns and matrices are
+ *    never read or written.  The 2-D plan transforms `batch` row-major ny x nx matrices (nx fastest), the
  *    reference's FFTdim = 2 application (templateFFT/batchTest/Test_2D.cpp). */
 typedef struct dfft_lines_plan_s* dfft_lines_plan;
 int dfft_lines_plan_create(int n, long long stride, long long nlines, long long inner, long long inner_dist,

@@ -3,7 +3,8 @@
 - tests/golden/lines_plan_ops.json: one SHA-256 per case of the JSON that one of the five host-only hooks
   (dfft_debug_lines_ops, dfft_debug_real_lines_ops, dfft_debug_lines_3d_ops, dfft_debug_lines_conv_3d_ops and
   dfft_debug_lines_conv_2d_ops) returns, or the hook's return code for a spec it rejects.  The cases cover both precisions and
-  directions, tuned and run-time-scheduled lengths, four-step long lines, strided columns, square and non-square 2-D and 3-D
+  directions, tuned and run-time-scheduled lengths, four-step long lines, strided columns (dense, padded, gapped and
+  interleaved; overlapping ones are rejected), square and non-square 2-D and 3-D
   plans with the plane kernels on, off (DFFT_NO_PLANE), forced (DFFT_FORCE_PLANE) and generic (DFFT_GENERIC), real plans,
   convolve plans (C2C and R2C, one or per-image multipliers, scaled or not) and odd batches, whose last tile or real pair is
   partial.
@@ -66,6 +67,10 @@ def ops_cases():
                 {"DFFT_NO_LONG_LINES": "1"})
             add("lines_cols_96x21x3_%s" % s, "dfft_debug_lines_ops", (96, 21, 63, 21, 1, 96 * 21, prec, d, 0))
             add("lines_cols_64x10x3_%s" % s, "dfft_debug_lines_ops", (64, 10, 30, 10, 1, 640, prec, d, 0))
+            # columns with padded rows, a gap between matrices, interleaved matrices
+            add("lines_cols_padded_96x21x3_%s" % s, "dfft_debug_lines_ops", (96, 24, 63, 21, 1, 96 * 24, prec, d, 0))
+            add("lines_cols_gapped_64x10x3_%s" % s, "dfft_debug_lines_ops", (64, 10, 30, 10, 1, 640 + 37, prec, d, 0))
+            add("lines_cols_interleaved_48x7x2_%s" % s, "dfft_debug_lines_ops", (48, 14, 14, 7, 1, 7, prec, d, 0))
             for nx, ny, b in ((32, 32, 5), (64, 48, 3), (14, 22, 3), (16, 9, 1)):
                 add("lines2d_%dx%dx%d_%s" % (nx, ny, b, s), "dfft_debug_lines_ops", (nx, ny, b, 0, 0, 0, prec, d, 1))
             # real 1-D and 2-D (odd line counts: a partial last pair)
@@ -103,6 +108,13 @@ def ops_cases():
     add("reject_lines_17_strided", "dfft_debug_lines_ops", (17, 4, 8, 4, 1, 68, DOUBLE, FORWARD, 0))
     add("reject_lines_prime_long", "dfft_debug_lines_ops", (8191, 1, 2, 2, 8191, 0, DOUBLE, FORWARD, 0))
     add("reject_lines_not_dense", "dfft_debug_lines_ops", (16, 1, 8, 4, 16, 80, DOUBLE, FORWARD, 0))
+    add("reject_lines_fourstep_gapped", "dfft_debug_lines_ops", (8192, 1, 4, 2, 8192, 3 * 8192, DOUBLE, FORWARD, 0))
+    # columns that overlap: more columns than a row holds, two matrices at one address, a negative matrix distance, interleaved
+    # matrices that collide
+    add("reject_lines_cols_overlap", "dfft_debug_lines_ops", (16, 4, 10, 5, 1, 80, DOUBLE, FORWARD, 0))
+    add("reject_lines_cols_outer0", "dfft_debug_lines_ops", (16, 4, 8, 4, 1, 0, DOUBLE, FORWARD, 0))
+    add("reject_lines_cols_outer_negative", "dfft_debug_lines_ops", (16, 4, 8, 4, 1, -64, DOUBLE, FORWARD, 0))
+    add("reject_lines_cols_interleave_overlap", "dfft_debug_lines_ops", (16, 8, 8, 4, 1, 6, DOUBLE, FORWARD, 0))
     add("reject_real_17", "dfft_debug_real_lines_ops", (17, 1, 4, DOUBLE, FORWARD, 0))
     add("reject_real_1", "dfft_debug_real_lines_ops", (1, 1, 4, DOUBLE, FORWARD, 0))
     add("reject_real_direction", "dfft_debug_real_lines_ops", (16, 1, 4, DOUBLE, 0, 0))

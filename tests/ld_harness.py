@@ -1,6 +1,7 @@
 """The harness of the long-double kernel matrices (test_gpu_tma_matrix.py, test_gpu_tile_matrix.py): seeded or structured inputs
 and their long-double references (tests/ldfft.py), cached per (shape, seed, precision, sign, kind, axis); the device layouts of a
-P = 1 plan; one plan on fenced, NaN-prefilled buffers executed several times; and the two error ratios against the bounds
+P = 1 plan; one plan on fenced, NaN-prefilled buffers executed several times; an in-place lines plan in a fenced layout whose
+gaps must stay unchanged; and the two error ratios against the bounds
 ldfft.REL_L2_K / ldfft.LINF_K (in units of eps * log2(Ntot))."""
 import collections
 
@@ -116,6 +117,37 @@ def run_fenced(shape, prec, direction, dev_in, flags=0, inplace=False, offset=0,
     if tin is not None:
         assert np.array_equal(bits(tin.cpu().numpy()), bits(dev_in)), "out-of-place input modified"
     return got, mask, fused
+
+
+def run_lines(plan, x, prec, direction, repeat=2, offsets=None, size=None, offset=0):
+    """in-place lines plan on a fenced device copy of `x`, executed `repeat` times from the same input; returns the result in x's
+    shape.  `offsets` (x's shape, the element offsets of x's points in a buffer of `size` elements, as a layout places them)
+    scatter x into that buffer; by default x is dense.  Every element of the arena outside x -- the canaries at both ends and the
+    gaps inside the layout -- holds a random pattern that must come back bit for bit.  `offset`: elements between the leading
+    canary and the buffer (the arena itself is 256-byte aligned)."""
+    npdt = CDT[prec][0]
+    if offsets is None:
+        offsets, size = np.arange(x.size).reshape(x.shape), x.size
+    lo = CANARY + offset
+    total = lo + size + CANARY
+    pattern = (np.random.default_rng(5).standard_normal(total) * (1 + 1j)).astype(npdt)
+    filled = pattern.copy()
+    filled[lo + offsets] = x
+    dev = torch.device("cuda", 0)
+    arena = torch.empty(total, dtype=CDT[prec][1], device=dev)
+    outs = []
+    for _ in range(repeat):
+        arena.copy_(torch.from_numpy(filled))
+        torch.cuda.synchronize(dev)                  # the plan runs on its own stream
+        plan.execute(arena[lo:].data_ptr(), direction)
+        plan.synchronize()
+        outs.append(arena.cpu().numpy())
+    keep = np.ones(total, dtype=bool)
+    keep[lo + offsets] = False
+    assert np.array_equal(bits(outs[0][keep]), bits(pattern[keep])), "an element outside the lines (a canary or a gap) was written"
+    for o in outs[1:]:
+        assert np.array_equal(bits(o), bits(outs[0])), "executes differ"
+    return outs[0][lo + offsets]
 
 
 # ---- the bounds ----------------------------------------------------------------------------------------------------------

@@ -31,7 +31,7 @@ torch = pytest.importorskip("torch")
 import distributedfft_b200 as dfft  # noqa: E402
 import ld_harness  # noqa: E402
 import ldfft  # noqa: E402
-from ld_harness import CDT, EPS, bits, layouts, ratios64, run_fenced  # noqa: E402
+from ld_harness import CDT, EPS, bits, layouts, ratios64, run_fenced, run_lines  # noqa: E402
 from tile_entries import DOUBLE, ENTRIES, FLOAT, NOT_FUSED, entry_id, lengths, thin_shape, threads  # noqa: E402
 
 FWD, BWD = dfft.FORWARD, dfft.BACKWARD
@@ -243,28 +243,6 @@ def test_forced_generic_kernel_on_tuned_lengths(n, prec, axis, monkeypatch):
 
 
 # ---- lines engine: four-step long lines, 2-D plans ---------------------------------------------------------------------------
-def run_lines(plan, x, prec, direction, repeat=2):
-    """in-place lines plan on a fenced device copy of `x`, executed `repeat` times from the same input"""
-    npdt = CDT[prec][0]
-    n = x.size
-    C = ld_harness.CANARY
-    dev = torch.device("cuda", 0)
-    pattern = (np.random.default_rng(5).standard_normal(n + 2 * C) * (1 + 1j)).astype(npdt)
-    arena = torch.from_numpy(pattern).to(dev)
-    view = arena[C: C + n]
-    outs = []
-    for _ in range(repeat):
-        view.copy_(torch.from_numpy(np.ascontiguousarray(x).reshape(-1)).to(dev))
-        plan.execute(view.data_ptr(), direction)
-        plan.synchronize()
-        outs.append(view.cpu().numpy().copy())
-    host = arena.cpu().numpy()
-    assert np.array_equal(bits(host[:C]), bits(pattern[:C])) and np.array_equal(bits(host[C + n:]), bits(pattern[C + n:])), "canary overwritten"
-    for o in outs[1:]:
-        assert np.array_equal(bits(o), bits(outs[0])), "executes differ"
-    return outs[0].reshape(x.shape)
-
-
 # the lengths of test_gpu_parity.py::test_four_step_long_lines; in fp32, 6561, 8192 and 12000 still fit one shared-memory line
 # and run as a single generic pass
 FOUR_STEP = [8192, 16384, 131072, 6561, 19683, 78125, 16807, 12000]
