@@ -23,7 +23,7 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++"]
 
 LIB_SOURCES = ["dfft_api.cu", "dfft_kernels_common.cu", "dfft_kernels_generic.cu", "dfft_kernels_f64.cu", "dfft_kernels_f32.cu", "dfft_kernels_tma.cu"]
-HEADERS = ["fft_core.cuh", "fft_passes.cuh", "fft_real.cuh", "fft_generic.cuh", "fft_tma.cuh", "fft_plane.cuh", "dfft_kernels.cuh", "dfft_kernels_inst.cuh", os.path.join("..", "..", "include", "dfft.h")]
+HEADERS = ["fft_core.cuh", "fft_passes.cuh", "fft_real.cuh", "fft_generic.cuh", "fft_tma.cuh", "fft_plane.cuh", "dfft_kernels.cuh", "dfft_kernels_inst.cuh", "dfft_launch.cuh", os.path.join("..", "..", "include", "dfft.h")]
 
 
 def _newer(target, deps):

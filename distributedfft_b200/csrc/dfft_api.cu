@@ -494,7 +494,8 @@ static inline cudaError_t ev_record(dfft_plan p, cudaEvent_t e) { return p->dry 
 static inline cudaError_t ev_record_on(dfft_plan p, cudaEvent_t e, cudaStream_t st) { return p->dry ? cudaSuccess : cudaEventRecord(e, st); }
 static inline cudaError_t stream_wait(dfft_plan p, cudaStream_t st, cudaEvent_t e) { return p->dry ? cudaSuccess : cudaStreamWaitEvent(st, e, 0); }
 
-static const char* const kPassNames[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW", "Z_R2C", "Z_C2R", "XCONV", "XCONV_CO"};
+static const char* const kPassNames[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW", "Z_R2C", "Z_C2R", "XCONV", "XCONV_CO",
+                                                  "XY_PLANE", "XY_PLANE_CONV", "LINE_CONV", "LINE_CONV_R2C"};
 
 // `extra`: further fields of the record, each starting with ", "
 template <typename T>
@@ -2307,7 +2308,7 @@ static int replay_op(const char* op, const dfft_debug_op* r, const char* op2, co
         int kind = -1;
         for (int k = 0; k < PK_COUNT; k++)
             if (!strcmp(op, kPassNames[k])) kind = k;
-        if (kind < 0 || kind == PK_Z_R2C || kind == PK_Z_C2R)
+        if (kind < 0 || kind == PK_Z_R2C || kind == PK_Z_C2R || kind >= PK_PLANE)
             return fail(DFFT_EINVAL, "dfft_debug_launch_op: '%s' is not a record this hook launches", op);
         if (!e->launch[kind]) return fail(DFFT_EUNSUPPORTED, "dfft_debug_launch_op: length %d has no %s kernel", r->N, op);
         if (r2 || op2) return fail(DFFT_EINVAL, "dfft_debug_launch_op: %s is one record", op);
@@ -2375,21 +2376,17 @@ extern "C" void* dfft_plan_stream(dfft_plan p) { return p ? (void*)p->stream : n
 // batched local transforms: plan / launch / delete, the templateFFT engine surface
 // (3dmpifft_opt/include/templateFFT.h:361-365 initializeFFT / launchFFTKernel / deleteFFT)
 // ------------------------------------------------------------------------------------------------
-// launches of the lines engine beyond the pass kinds: X + Y of whole e->N x e->N planes in one launch of e->plane (PlaneArgs),
-// the whole 2-D convolution of whole images in one launch of e->plane_conv (PlaneConvArgs), and the whole 1-D convolution of
-// contiguous lines in one launch of e->line_conv (LineConvArgs) or, real lines, e->line_conv_r2c (RealLineConvArgs)
-enum { LK_PLANE = PK_COUNT, LK_PLANE_CONV, LK_LINE_CONV, LK_LINE_CONV_R2C };
 enum { LB_IN = 0, LB_TEMP = 1, LB_OUT = 2 };
 struct LinePass {
     const SizeEntry* e = nullptr;
-    int kind = PK_Z;             // a PassKind or an LK_ launch kind
+    int kind = PK_Z;             // a PassKind
     void* lut = nullptr;
     Affine ia{}, oa{};           // plane kinds, for the records: plane (image), 0, row and point strides
     int G = 0, W = 0;
     long long ntiles = 0;        // plane kinds: planes (images)
     long long tw_n = 0;          // four-step twiddle modulus (PK_XF_TW)
     int src = LB_IN, dst = LB_IN;   // LB_IN (the caller's data / a real or convolve plan's `in`), LB_TEMP (the plan's temporary), LB_OUT
-    long long ld_in = 0, ld_out = 0;   // PK_Z_R2C / PK_Z_C2R / LK_LINE_CONV_R2C: distance between the two lines of a pair (RealZArgs), each side's elements
+    long long ld_in = 0, ld_out = 0;   // PK_Z_R2C / PK_Z_C2R / PK_LINE_CONV_R2C: distance between the two lines of a pair (RealZArgs), each side's elements
     bool inv = false;            // the inverse transform
 };
 // which execute runs a plan: dfft_lines_execute, dfft_lines_execute_real or dfft_lines_execute_convolve
@@ -2426,7 +2423,7 @@ static bool fits_int(long long a, long long b = 1, long long c = 1)
 // kernels the contiguous configuration
 static int plain_kind(int kind)
 {
-    return kind == PK_XCONV ? PK_Y : (kind == PK_Z_R2C || kind == PK_Z_C2R || kind >= PK_COUNT) ? PK_Z : kind;
+    return kind == PK_XCONV ? PK_Y : (kind == PK_Z_R2C || kind == PK_Z_C2R || kind >= PK_PLANE) ? PK_Z : kind;
 }
 
 // columns that touch no element twice: the (extent, stride) pairs (inner, 1), (n, stride) and (mats, outer_dist), sorted by
@@ -2572,12 +2569,12 @@ static int make_lines_3d(dfft_lines_plan p, int nx, int ny, int nz, long long ba
     if (!fits_int(ny, nz, batch)) return fail(DFFT_EUNSUPPORTED, "%d x %d x %lld rows: at most 2^31 - 1 per plan", ny, nz, batch);
     const long long planes = (long long)nz * batch, rows = planes * ny, plane = (long long)nx * ny;
     const SizeEntry* ex = find_size_entry(nx, precision);
-    const bool use_plane = ex && nx == ny && ex->plane && !env_on("DFFT_NO_PLANE") && (plane_default(nx, precision) || env_on("DFFT_FORCE_PLANE"));
+    const bool use_plane = ex && nx == ny && ex->launch[PK_PLANE] && !env_on("DFFT_NO_PLANE") && (plane_default(nx, precision) || env_on("DFFT_FORCE_PLANE"));
     LinePass* f = p->run[0];
     int rc = 0, k = 0;
     if (use_plane) {
         LinePass& lp = f[k++];
-        lp.e = ex; lp.kind = LK_PLANE; lp.ntiles = planes;
+        lp.e = ex; lp.kind = PK_PLANE; lp.ntiles = planes;
         lp.ia = lp.oa = Affine{plane, 0, nx, 1};
     } else {
         rc = make_line_pass(f[k++], nx, 1, rows, rows, nx, 0, precision);
@@ -2653,7 +2650,7 @@ static int make_real_lines(dfft_lines_plan p, int n, int ny, int nz, long long b
 //   3-D C2C, plane kernel: XY_PLANE in -> out, XCONV, inverse XY_PLANE (6 volume sweeps + the multiplier)
 //   3-D C2C, other shapes: X in -> out, Y, XCONV, inverse Y, inverse X (10 sweeps)
 //   3-D R2C:               Z_R2C in -> temp, Y, XCONV, inverse Y, Z_C2R temp -> out
-//   2-D C2C, plane conv:   XY_PLANE_CONV in -> out: the whole convolution of nx == ny images in one launch of e->plane_conv
+//   2-D C2C, plane conv:   XY_PLANE_CONV in -> out: the whole convolution of nx == ny images in one launch of launch[PK_PLANE_CONV]
 //                          (plane_conv_default; DFFT_FORCE_PLANE=1: wherever instantiated; DFFT_NO_PLANE=1: never) (2 sweeps)
 //   2-D C2C, other shapes: X in -> out, XCONV, inverse X (6 sweeps)
 //   2-D R2C:               Z_R2C in -> temp, XCONV, Z_C2R temp -> out
@@ -2686,9 +2683,9 @@ static int make_lines_conv(dfft_lines_plan p, int dims, int nx, int ny, int nz, 
     }
     const long long vol = (long long)nx * ny * (dims == 3 ? nz : 1);
     if (real) make_real_pass(c[k++], f[0].e, vol / nx * batch, false, LB_TEMP, LB_OUT);   // Z_C2R temp -> out
-    if (dims == 2 && !real && nx == ny && f[0].e->plane_conv && !env_on("DFFT_NO_PLANE") && (plane_conv_default(nx, p->prec) || env_on("DFFT_FORCE_PLANE"))) {
+    if (dims == 2 && !real && nx == ny && f[0].e->launch[PK_PLANE_CONV] && !env_on("DFFT_NO_PLANE") && (plane_conv_default(nx, p->prec) || env_on("DFFT_FORCE_PLANE"))) {
         // the three passes become one, on the X pass's buffers and contiguous twiddle table (one Sched at these lengths)
-        c[0].kind = LK_PLANE_CONV; c[0].ntiles = batch;
+        c[0].kind = PK_PLANE_CONV; c[0].ntiles = batch;
         c[0].ia = c[0].oa = Affine{(long long)nx * ny, 0, nx, 1};
         k = 1;
     }
@@ -2716,7 +2713,7 @@ static int make_lines_conv_1d(dfft_lines_plan p, int n, long long nlines, bool r
     if (n < 1 || nlines < 0 || bad_precision(p->prec)) return fail(DFFT_EINVAL, "bad arguments");
     if (real && n < 2) return fail(DFFT_EUNSUPPORTED, "real lines of %d points: a real convolution needs at least 2", n);
     const SizeEntry* e = find_size_entry(n, p->prec);
-    if (!e || e->gen || !(real ? e->line_conv_r2c : e->line_conv))
+    if (!e || e->gen || !e->launch[real ? PK_LINE_CONV_R2C : PK_LINE_CONV])
         return fail(DFFT_EUNSUPPORTED, "length %d has no line-convolution kernel: it needs a tuned length (dfft_length_kind == 2) of the default "
                     "kernel table; generic lengths and lines longer than one shared-memory line are not convolved", n);
     if (!fits_int(nlines)) return fail(DFFT_EUNSUPPORTED, "%lld lines: at most 2^31 - 1 per plan", nlines);
@@ -2726,12 +2723,12 @@ static int make_lines_conv_1d(dfft_lines_plan p, int n, long long nlines, bool r
     lp.src = LB_IN; lp.dst = LB_OUT;
     lp.W = (int)nlines;
     if (real) {
-        lp.kind = LK_LINE_CONV_R2C;
+        lp.kind = PK_LINE_CONV_R2C;
         lp.G = (int)cdiv(cdiv(nlines, 2), C);
         lp.ia = lp.oa = Affine{0, 2LL * C * n, 2LL * n, 1};   // tile, pair and point strides (reals)
         lp.ld_in = lp.ld_out = n;
     } else {
-        lp.kind = LK_LINE_CONV;
+        lp.kind = PK_LINE_CONV;
         lp.G = (int)cdiv(nlines, C);
         lp.ia = lp.oa = Affine{0, (long long)C * n, n, 1};
     }
@@ -2880,8 +2877,8 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
 {
     const void* src = line_buf(lp.src, in, out, p->temp);
     void* dst = line_buf(lp.dst, in, out, p->temp);
-    const bool conv = lp.kind == PK_XCONV || lp.kind == LK_PLANE_CONV || lp.kind == LK_LINE_CONV || lp.kind == LK_LINE_CONV_R2C;
-    const bool realk = lp.kind == PK_Z_R2C || lp.kind == PK_Z_C2R || lp.kind == LK_LINE_CONV_R2C;
+    const bool conv = lp.kind == PK_XCONV || lp.kind == PK_PLANE_CONV || lp.kind == PK_LINE_CONV || lp.kind == PK_LINE_CONV_R2C;
+    const bool realk = lp.kind == PK_Z_R2C || lp.kind == PK_Z_C2R || lp.kind == PK_LINE_CONV_R2C;
     ConvArgs<T> c{};
     TileArgs<T>& a = c.t;
     a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)lp.lut;
@@ -2896,37 +2893,39 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
         int len = 0;
         if (realk) len = snprintf(extra, sizeof(extra), ", \"nzh\": %d, \"pair\": [%lld, %lld]", lp.e->N / 2 + 1, lp.ld_in, lp.ld_out);
         if (conv) snprintf(extra + len, sizeof(extra) - len, ", \"mult\": %llu, \"shared\": %d", (unsigned long long)(size_t)mult, shared ? 1 : 0);
-        const bool plane = lp.kind == LK_PLANE || lp.kind == LK_PLANE_CONV;
-        const char* name = lp.kind == LK_PLANE ? "XY_PLANE" : lp.kind == LK_PLANE_CONV ? "XY_PLANE_CONV" : lp.kind == LK_LINE_CONV ? "LINE_CONV"
-                         : lp.kind == LK_LINE_CONV_R2C ? "LINE_CONV_R2C" : kPassNames[lp.kind];
-        record_op<T>(*ops, name, phase, lp.e->N, plane ? lp.e->N : kind_C(lp.e, plain_kind(lp.kind)), false, false, lp.kind == PK_XF_TW, a, extra);
+        const bool plane = lp.kind == PK_PLANE || lp.kind == PK_PLANE_CONV;
+        record_op<T>(*ops, kPassNames[lp.kind], phase, lp.e->N, plane ? lp.e->N : kind_C(lp.e, plain_kind(lp.kind)), false, false, lp.kind == PK_XF_TW, a,
+                     extra);
         return cudaSuccess;
     }
+    // the kind's argument struct: the tile arguments (a), the column convolve's (c), or one of these
+    PlaneConvArgs<T> pc{};      // PK_PLANE: pc.p
+    RealLineConvArgs<T> rl{};   // PK_Z_R2C / PK_Z_C2R: rl.r
+    LineConvArgs<T> lc{};
+    const void* args = conv ? (const void*)&c : (const void*)&a;
     switch (lp.kind) {
-    case LK_PLANE: {
-        const PlaneArgs<T> pa{a.in, a.out, a.lut, lp.ntiles, a.inv};
-        return lp.e->plane(&pa, p->sms, p->stream);
+    case PK_PLANE:
+        pc.p = {a.in, a.out, a.lut, lp.ntiles, a.inv};
+        args = &pc.p;
+        break;
+    case PK_PLANE_CONV:
+        pc = {{a.in, a.out, a.lut, lp.ntiles, 0}, c.mult, shared ? 0 : (long long)lp.e->N * lp.e->N, a.scale, a.do_scale};
+        args = &pc;
+        break;
+    case PK_Z_R2C: case PK_Z_C2R:
+        rl.r = {a, (const T*)src, (T*)dst, lp.ld_in, lp.ld_out};
+        args = &rl.r;
+        break;
+    case PK_LINE_CONV:
+        lc = {a, c.mult, shared ? 0 : (long long)lp.e->N};
+        args = &lc;
+        break;
+    case PK_LINE_CONV_R2C:
+        rl = {{a, (const T*)src, (T*)dst, lp.ld_in, lp.ld_out}, c.mult, shared ? 0 : (long long)(lp.e->N / 2 + 1)};
+        args = &rl;
+        break;
     }
-    case LK_PLANE_CONV: {
-        const long long n = lp.e->N;
-        const PlaneConvArgs<T> pc{{a.in, a.out, a.lut, lp.ntiles, 0}, c.mult, shared ? 0 : n * n, a.scale, a.do_scale};
-        return lp.e->plane_conv(&pc, p->sms, p->stream);
-    }
-    case PK_Z_R2C: case PK_Z_C2R: {
-        const RealZArgs<T> r{a, (const T*)src, (T*)dst, lp.ld_in, lp.ld_out};
-        return lp.e->launch[lp.kind](&r, p->sms, p->stream);
-    }
-    case LK_LINE_CONV: {
-        const LineConvArgs<T> lc{a, c.mult, shared ? 0 : (long long)lp.e->N};
-        return lp.e->line_conv(&lc, p->sms, p->stream);
-    }
-    case LK_LINE_CONV_R2C: {
-        const RealLineConvArgs<T> lc{{a, (const T*)src, (T*)dst, lp.ld_in, lp.ld_out}, c.mult, shared ? 0 : (long long)(lp.e->N / 2 + 1)};
-        return lp.e->line_conv_r2c(&lc, p->sms, p->stream);
-    }
-    default:
-        return lp.e->launch[lp.kind](conv ? (const void*)&c : (const void*)&a, p->sms, p->stream);
-    }
+    return lp.e->launch[lp.kind](args, p->sms, p->stream);
 }
 
 // one execute: the passes of run[list] between the plan's two events

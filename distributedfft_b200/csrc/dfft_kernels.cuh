@@ -25,6 +25,13 @@ enum PassKind {
     PK_XCONV,      // spectral convolution along x: forward, multiply, inverse in one column pass (fft_conv_kernel; args = ConvArgs),
                    // strided local configuration, local store
     PK_XCONV_CO,   // + chunked (peer) store split by xd, in the peer-store configuration
+    // the lines engine's whole-plane and whole-line kernels, on the contiguous schedule; default entries only, else nullptr
+    PK_PLANE,          // X + Y passes of whole N x N planes in one kernel (fft_plane_kernel; args = PlaneArgs); N = 16, 32, 64 only
+                       // (both roles share one schedule there)
+    PK_PLANE_CONV,     // 2-D convolution of whole N x N images in one kernel (fft_plane_conv_kernel; args = PlaneConvArgs); set where
+                       // PK_PLANE is
+    PK_LINE_CONV,      // 1-D convolution of contiguous lines in one pass (fft_line_conv_kernel; args = LineConvArgs)
+    PK_LINE_CONV_R2C,  // + real lines, two per complex transform (fft_line_conv_r2c_kernel; args = RealLineConvArgs)
     PK_COUNT
 };
 
@@ -43,8 +50,6 @@ typedef cudaError_t (*FusedLaunchFn)(const void* args_a, const void* args_b, con
 // send side (Y pass of part k, peer stores) and receive side (X pass of part k-1) of the exchange in one kernel (fft_fused_yx_kernel)
 typedef cudaError_t (*FusedYxLaunchFn)(const void* args_y, const void* args_x, const YxCtl* ctl, int sm_count, cudaStream_t stream);
 typedef cudaError_t (*Fused3LaunchFn)(const void* args_z, const void* args_y, const void* args_x, const Fused3Ctl* ctl, int sm_count, cudaStream_t stream);
-// X and Y passes of square planes in one sweep (fft_plane_kernel): args = PlaneArgs<T>
-typedef cudaError_t (*PlaneLaunchFn)(const void* plane_args, int sm_count, cudaStream_t stream);
 
 struct SizeEntry {
     int N;
@@ -63,13 +68,6 @@ struct SizeEntry {
     FusedYxLaunchFn fused_yx;        // Y (peer-store configuration) + X roles of this entry in one kernel; nullptr unless both fill the same CTA
     Fused3LaunchFn fused3;           // same restriction, and the X configuration must fill the same CTA as the peer-store Y role (else nullptr)
     const void* gen;      // run-time schedule (GenSched) of a generic-length entry, nullptr for tuned lengths
-    PlaneLaunchFn plane;  // valid for square planes: the contiguous (X) and strided (Y) passes of whole N x N planes in one kernel;
-                          // default entries of N = 16, 32, 64 only (both roles share one schedule there), else nullptr
-    PlaneLaunchFn plane_conv;   // set where `plane` is: the 2-D convolution of whole N x N images in one kernel
-                                // (fft_plane_conv_kernel, args = PlaneConvArgs<T>), else nullptr
-    // 1-D convolution of contiguous lines in one pass, in the contiguous configuration; default entries only, else nullptr
-    PassLaunchFn line_conv;       // complex lines (fft_line_conv_kernel, args = LineConvArgs<T>)
-    PassLaunchFn line_conv_r2c;   // real lines, two per complex transform (fft_line_conv_r2c_kernel, args = RealLineConvArgs<T>)
 };
 
 // whether fft_plane_kernel is the default for (N, prec) (measured against the two separate passes, dfft_kernels_common.cu)

@@ -3,6 +3,7 @@
 #include <map>
 #include <mutex>
 #include "dfft_kernels.cuh"
+#include "dfft_launch.cuh"
 #include "fft_generic.cuh"
 
 namespace dfft {
@@ -41,35 +42,33 @@ static bool make_generic_sched(int N, int prec, GenSched& g)
     return true;
 }
 
+// Shared memory depends on the run-time length, so the opt-in is raised once per device to the most any length uses (200 KiB,
+// make_generic_sched) and the resident CTAs per SM are queried at every launch
+template <auto Kern> static cudaError_t generic_grid(size_t smem, int cap, long long work, int sm_count, long long& grid)
+{
+    grid = 0;
+    cudaError_t e = smem_optin<Kern>(200 * 1024);
+    if (e != cudaSuccess || work <= 0) return e;
+    int occ = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, Kern, GEN_THREADS, smem);
+    if (e != cudaSuccess) return e;
+    if (occ < 1) return cudaErrorLaunchOutOfResources;
+    grid = grid_for(sm_count, occ, cap, work);
+    return cudaSuccess;
+}
+
+// complex passes: vargs is a TileArgs<T>; capped by TileArgs::max_ctas_per_sm, as launch_pass is
 template <typename T, int MI, int MO, bool CI, bool CO>
 static cudaError_t launch_generic(const void* vargs, int sm_count, cudaStream_t st)
 {
     const TileArgs<T>& a = *reinterpret_cast<const TileArgs<T>*>(vargs);
     if (!a.gen) return cudaErrorInvalidValue;
     const GenSched& g = *reinterpret_cast<const GenSched*>(a.gen);
-    auto kern = fft_generic_kernel<T, MI, MO, CI, CO>;
+    constexpr auto kern = fft_generic_kernel<T, MI, MO, CI, CO>;
     const size_t smem = 2 * (size_t)g.C * g.N * sizeof(cx<T>);
-    static std::mutex mu;
-    static size_t attr_set[64] = {0};
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    {
-        std::lock_guard<std::mutex> lk(mu);
-        if (attr_set[dev & 63] < smem) {
-            e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024));
-            if (e != cudaSuccess) return e;
-            attr_set[dev & 63] = 200 * 1024;
-        }
-    }
-    if (a.ntiles <= 0) return cudaSuccess;
-    int occ = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, GEN_THREADS, smem);
-    if (e != cudaSuccess) return e;
-    if (occ < 1) return cudaErrorLaunchOutOfResources;
-    if (a.max_ctas_per_sm > 0 && occ > a.max_ctas_per_sm) occ = a.max_ctas_per_sm;
-    long long grid = (long long)sm_count * occ;
-    if (grid > a.ntiles) grid = a.ntiles;
+    long long grid = 0;
+    const cudaError_t e = generic_grid<kern>(smem, a.max_ctas_per_sm, a.ntiles, sm_count, grid);
+    if (e != cudaSuccess || grid == 0) return e;
     kern<<<(unsigned)grid, GEN_THREADS, smem, st>>>(a, g);
     return cudaGetLastError();
 }
@@ -81,28 +80,11 @@ static cudaError_t launch_generic_real(const void* vargs, int sm_count, cudaStre
     const RealZArgs<T>& a = *reinterpret_cast<const RealZArgs<T>*>(vargs);
     if (!a.t.gen) return cudaErrorInvalidValue;
     const GenSched& g = *reinterpret_cast<const GenSched*>(a.t.gen);
-    auto kern = INV ? fft_generic_c2r_kernel<T> : fft_generic_r2c_kernel<T>;
+    constexpr auto kern = INV ? fft_generic_c2r_kernel<T> : fft_generic_r2c_kernel<T>;
     const size_t smem = 2 * (size_t)g.C * g.N * sizeof(cx<T>);
-    static std::mutex mu;
-    static size_t attr_set[64] = {0};
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    {
-        std::lock_guard<std::mutex> lk(mu);
-        if (attr_set[dev & 63] < smem) {
-            e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024));
-            if (e != cudaSuccess) return e;
-            attr_set[dev & 63] = 200 * 1024;
-        }
-    }
-    if (a.t.ntiles <= 0) return cudaSuccess;
-    int occ = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, GEN_THREADS, smem);
-    if (e != cudaSuccess) return e;
-    if (occ < 1) return cudaErrorLaunchOutOfResources;
-    long long grid = (long long)sm_count * occ;
-    if (grid > a.t.ntiles) grid = a.t.ntiles;
+    long long grid = 0;
+    const cudaError_t e = generic_grid<kern>(smem, 0, a.t.ntiles, sm_count, grid);
+    if (e != cudaSuccess || grid == 0) return e;
     kern<<<(unsigned)grid, GEN_THREADS, smem, st>>>(a, g);
     return cudaGetLastError();
 }

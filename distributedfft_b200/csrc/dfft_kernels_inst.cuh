@@ -1,35 +1,24 @@
 // dfft_kernels_inst.cuh -- launcher template + size-table macros, included by the per-precision
 // instantiation units.
 #pragma once
-#include <atomic>
 #include <type_traits>
 #include "dfft_kernels.cuh"
+#include "dfft_launch.cuh"
 
 namespace dfft {
 
+// Every launcher below picks its kernel, block size, dynamic shared memory and argument struct, and sizes its persistent grid
+// with resident_grid (dfft_launch.cuh).  Only launch_pass (and launch_generic) cap the resident CTAs per SM with
+// TileArgs::max_ctas_per_sm: the pipelined Y and X passes are the only passes that set it
 template <class S, typename T, int C, int MI, int MO, bool TW, bool CI, bool CO, int MINB, bool PP, bool EPI = false>
 cudaError_t launch_pass(const void* vargs, int sm_count, cudaStream_t st)
 {
     const TileArgs<T>& a = *reinterpret_cast<const TileArgs<T>*>(vargs);
-    auto kern = fft_tile_kernel<S, T, C, MI, MO, TW, CI, CO, MINB, PP, false, EPI>;
+    constexpr auto kern = fft_tile_kernel<S, T, C, MI, MO, TW, CI, CO, MINB, PP, false, EPI>;
     constexpr size_t smem = TileSmem<S, T, C, PP>::bytes(CI || CO);
-    static std::atomic<int> occ_cache[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    int occ = occ_cache[dev & 63].load();
-    if (occ == 0) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, S::T * C, smem);
-        if (e != cudaSuccess) return e;
-        if (occ < 1) return cudaErrorLaunchOutOfResources;
-        occ_cache[dev & 63].store(occ);
-    }
-    if (a.ntiles <= 0) return cudaSuccess;
-    if (a.max_ctas_per_sm > 0 && occ > a.max_ctas_per_sm) occ = a.max_ctas_per_sm;
-    long long grid = (long long)sm_count * occ;
-    if (grid > a.ntiles) grid = a.ntiles;
+    long long grid = 0;
+    const cudaError_t e = resident_grid<kern>(S::T * C, smem, a.max_ctas_per_sm, a.ntiles, sm_count, grid);
+    if (e != cudaSuccess || grid == 0) return e;
     kern<<<(unsigned)grid, S::T * C, smem, st>>>(a);
     return cudaGetLastError();
 }
@@ -39,27 +28,14 @@ template <class S, typename T, int C, bool TW, int MINB, bool PP, bool C2R>
 cudaError_t launch_real(const void* vargs, int sm_count, cudaStream_t st)
 {
     const RealZArgs<T>& a = *reinterpret_cast<const RealZArgs<T>*>(vargs);
-    auto kern = [] {   // only the kernel of this direction is instantiated
+    constexpr auto kern = [] {   // only the kernel of this direction is instantiated
         if constexpr (C2R) return fft_z_c2r_kernel<S, T, C, TW, MINB, PP>;
         else return fft_z_r2c_kernel<S, T, C, TW, MINB, PP>;
     }();
     constexpr size_t smem = TileSmem<S, T, C, PP>::bytes(false);
-    static std::atomic<int> occ_cache[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    int occ = occ_cache[dev & 63].load();
-    if (occ == 0) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, S::T * C, smem);
-        if (e != cudaSuccess) return e;
-        if (occ < 1) return cudaErrorLaunchOutOfResources;
-        occ_cache[dev & 63].store(occ);
-    }
-    if (a.t.ntiles <= 0) return cudaSuccess;
-    long long grid = (long long)sm_count * occ;
-    if (grid > a.t.ntiles) grid = a.t.ntiles;
+    long long grid = 0;
+    const cudaError_t e = resident_grid<kern>(S::T * C, smem, 0, a.t.ntiles, sm_count, grid);
+    if (e != cudaSuccess || grid == 0) return e;
     kern<<<(unsigned)grid, S::T * C, smem, st>>>(a);
     return cudaGetLastError();
 }
@@ -68,27 +44,14 @@ cudaError_t launch_real(const void* vargs, int sm_count, cudaStream_t st)
 template <class S, typename T, int C, bool TW, bool CO, int MINB, bool PP, bool SH>
 cudaError_t launch_conv_k(const ConvArgs<T>& a, int sm_count, cudaStream_t st)
 {
-    auto kern = [] {   // only the kernel of this mode is instantiated
+    constexpr auto kern = [] {   // only the kernel of this mode is instantiated
         if constexpr (SH) return fft_conv_shared_kernel<S, T, C, TW, MINB, PP>;
         else return fft_conv_kernel<S, T, C, TW, CO, MINB, PP>;
     }();
     constexpr size_t smem = TileSmem<S, T, C, PP>::bytes(CO);
-    static std::atomic<int> occ_cache[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    int occ = occ_cache[dev & 63].load();
-    if (occ == 0) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, S::T * C, smem);
-        if (e != cudaSuccess) return e;
-        if (occ < 1) return cudaErrorLaunchOutOfResources;
-        occ_cache[dev & 63].store(occ);
-    }
-    if (a.t.ntiles <= 0) return cudaSuccess;
-    long long grid = (long long)sm_count * occ;
-    if (grid > a.t.ntiles) grid = a.t.ntiles;
+    long long grid = 0;
+    const cudaError_t e = resident_grid<kern>(S::T * C, smem, 0, a.t.ntiles, sm_count, grid);
+    if (e != cudaSuccess || grid == 0) return e;
     kern<<<(unsigned)grid, S::T * C, smem, st>>>(a);
     return cudaGetLastError();
 }
@@ -110,30 +73,18 @@ cudaError_t launch_conv(const void* vargs, int sm_count, cudaStream_t st)
 template <class S, typename T, int C, bool TW, int MINB, bool PP, bool R2C>
 cudaError_t launch_line_conv(const void* vargs, int sm_count, cudaStream_t st)
 {
-    const TileArgs<T>& a = R2C ? reinterpret_cast<const RealLineConvArgs<T>*>(vargs)->r.t : reinterpret_cast<const LineConvArgs<T>*>(vargs)->t;
-    auto kern = [] {   // only the kernel of this kind is instantiated
+    using Args = std::conditional_t<R2C, RealLineConvArgs<T>, LineConvArgs<T>>;
+    const Args& a = *reinterpret_cast<const Args*>(vargs);
+    constexpr auto kern = [] {   // only the kernel of this kind is instantiated
         if constexpr (R2C) return fft_line_conv_r2c_kernel<S, T, C, TW, MINB, PP>;
         else return fft_line_conv_kernel<S, T, C, TW, MINB, PP>;
     }();
     constexpr size_t smem = TileSmem<S, T, C, PP>::bytes(false);
-    static std::atomic<int> occ_cache[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    int occ = occ_cache[dev & 63].load();
-    if (occ == 0) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, S::T * C, smem);
-        if (e != cudaSuccess) return e;
-        if (occ < 1) return cudaErrorLaunchOutOfResources;
-        occ_cache[dev & 63].store(occ);
-    }
-    if (a.ntiles <= 0) return cudaSuccess;
-    long long grid = (long long)sm_count * occ;
-    if (grid > a.ntiles) grid = a.ntiles;
-    if constexpr (R2C) kern<<<(unsigned)grid, S::T * C, smem, st>>>(*reinterpret_cast<const RealLineConvArgs<T>*>(vargs));
-    else kern<<<(unsigned)grid, S::T * C, smem, st>>>(*reinterpret_cast<const LineConvArgs<T>*>(vargs));
+    const TileArgs<T>& t = [&]() -> const TileArgs<T>& { if constexpr (R2C) return a.r.t; else return a.t; }();
+    long long grid = 0;
+    const cudaError_t e = resident_grid<kern>(S::T * C, smem, 0, t.ntiles, sm_count, grid);
+    if (e != cudaSuccess || grid == 0) return e;
+    kern<<<(unsigned)grid, S::T * C, smem, st>>>(a);
     return cudaGetLastError();
 }
 
@@ -142,25 +93,11 @@ template <class S, typename T, int P, int MINB>
 cudaError_t launch_plane(const void* vargs, int sm_count, cudaStream_t st)
 {
     const PlaneArgs<T>& a = *reinterpret_cast<const PlaneArgs<T>*>(vargs);
-    auto kern = fft_plane_kernel<S, T, P, MINB>;
+    constexpr auto kern = fft_plane_kernel<S, T, P, MINB>;
     constexpr size_t smem = PlaneSmem<S, T, P>::bytes;
-    static std::atomic<int> occ_cache[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    int occ = occ_cache[dev & 63].load();
-    if (occ == 0) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, S::T * S::N * P, smem);
-        if (e != cudaSuccess) return e;
-        if (occ < 1) return cudaErrorLaunchOutOfResources;
-        occ_cache[dev & 63].store(occ);
-    }
-    const long long groups = (a.planes + P - 1) / P;
-    if (groups <= 0) return cudaSuccess;
-    long long grid = (long long)sm_count * occ;
-    if (grid > groups) grid = groups;
+    long long grid = 0;
+    const cudaError_t e = resident_grid<kern>(S::T * S::N * P, smem, 0, (a.planes + P - 1) / P, sm_count, grid);
+    if (e != cudaSuccess || grid == 0) return e;
     kern<<<(unsigned)grid, S::T * S::N * P, smem, st>>>(a);
     return cudaGetLastError();
 }
@@ -170,121 +107,12 @@ template <class S, typename T, int P, int MINB>
 cudaError_t launch_plane_conv(const void* vargs, int sm_count, cudaStream_t st)
 {
     const PlaneConvArgs<T>& a = *reinterpret_cast<const PlaneConvArgs<T>*>(vargs);
-    auto kern = fft_plane_conv_kernel<S, T, P, MINB>;
+    constexpr auto kern = fft_plane_conv_kernel<S, T, P, MINB>;
     constexpr size_t smem = PlaneSmem<S, T, P>::bytes;
-    static std::atomic<int> occ_cache[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    int occ = occ_cache[dev & 63].load();
-    if (occ == 0) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, S::T * S::N * P, smem);
-        if (e != cudaSuccess) return e;
-        if (occ < 1) return cudaErrorLaunchOutOfResources;
-        occ_cache[dev & 63].store(occ);
-    }
-    const long long groups = (a.p.planes + P - 1) / P;
-    if (groups <= 0) return cudaSuccess;
-    long long grid = (long long)sm_count * occ;
-    if (grid > groups) grid = groups;
+    long long grid = 0;
+    const cudaError_t e = resident_grid<kern>(S::T * S::N * P, smem, 0, (a.p.planes + P - 1) / P, sm_count, grid);
+    if (e != cudaSuccess || grid == 0) return e;
     kern<<<(unsigned)grid, S::T * S::N * P, smem, st>>>(a);
-    return cudaGetLastError();
-}
-
-template <class OpA, class OpB, typename T, int MINB>
-cudaError_t launch_fused(const void* va, const void* vb, const FusedCtl* ctl, int sm_count, cudaStream_t st)
-{
-    const TileArgs<T>& a = *reinterpret_cast<const TileArgs<T>*>(va);
-    const TileArgs<T>& b = *reinterpret_cast<const TileArgs<T>*>(vb);
-    auto kern = fft_fused2_kernel<OpA, OpB, T, MINB>;
-    constexpr size_t exch = OpA::SM::exch_bytes > OpB::SM::exch_bytes ? OpA::SM::exch_bytes : OpB::SM::exch_bytes;
-    constexpr size_t smem = exch + OpA::aux_bytes + OpB::aux_bytes;
-    static std::atomic<int> occ_cache[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    int occ = occ_cache[dev & 63].load();
-    if (occ == 0) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, OpA::NT, smem);
-        if (e != cudaSuccess) return e;
-        if (occ < 1) return cudaErrorLaunchOutOfResources;
-        occ_cache[dev & 63].store(occ);
-    }
-    if (ctl->planes <= 0) return cudaSuccess;
-    const long long total = ctl->planes * ((long long)ctl->GA + ctl->GB);
-    if (total >= (1ll << 31)) return cudaErrorInvalidConfiguration;   // the kernel decodes tickets in 32 bits
-    long long grid = (long long)sm_count * occ;
-    if (grid > total) grid = total;
-    FusedCtl c = *ctl;
-    if (c.lag <= 0) c.lag = (int)((grid + c.GA + c.GB - 1) / ((long long)c.GA + c.GB)) + 1;   // role A stays one in-flight window ahead
-    kern<<<(unsigned)grid, OpA::NT, smem, st>>>(a, b, c);
-    return cudaGetLastError();
-}
-
-template <class OpA, class OpB, typename T, int MINB>
-cudaError_t launch_fused_yx(const void* va, const void* vb, const YxCtl* ctl, int sm_count, cudaStream_t st)
-{
-    const TileArgs<T>& a = *reinterpret_cast<const TileArgs<T>*>(va);
-    const TileArgs<T>& b = *reinterpret_cast<const TileArgs<T>*>(vb);
-    auto kern = fft_fused_yx_kernel<OpA, OpB, T, MINB>;
-    constexpr size_t exch = OpA::SM::exch_bytes > OpB::SM::exch_bytes ? OpA::SM::exch_bytes : OpB::SM::exch_bytes;
-    constexpr size_t smem = exch + OpA::aux_bytes + OpB::aux_bytes;
-    static std::atomic<int> occ_cache[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    int occ = occ_cache[dev & 63].load();
-    if (occ == 0) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, OpA::NT, smem);
-        if (e != cudaSuccess) return e;
-        if (occ < 1) return cudaErrorLaunchOutOfResources;
-        occ_cache[dev & 63].store(occ);
-    }
-    const long long total = (long long)ctl->TA + ctl->TB;
-    if (total <= 0) return cudaSuccess;
-    long long grid = (long long)sm_count * occ;
-    if (grid > total) grid = total;
-    kern<<<(unsigned)grid, OpA::NT, smem, st>>>(a, b, *ctl);
-    return cudaGetLastError();
-}
-
-template <class OpA, class OpB, class OpC, typename T, int MINB>
-cudaError_t launch_fused3(const void* va, const void* vb, const void* vc, const Fused3Ctl* ctl, int sm_count, cudaStream_t st)
-{
-    const TileArgs<T>& a = *reinterpret_cast<const TileArgs<T>*>(va);
-    const TileArgs<T>& b = *reinterpret_cast<const TileArgs<T>*>(vb);
-    const TileArgs<T>& c = *reinterpret_cast<const TileArgs<T>*>(vc);
-    auto kern = fft_fused3_kernel<OpA, OpB, OpC, T, MINB>;
-    constexpr size_t e1 = OpA::SM::exch_bytes > OpB::SM::exch_bytes ? OpA::SM::exch_bytes : OpB::SM::exch_bytes;
-    constexpr size_t exch = e1 > OpC::SM::exch_bytes ? e1 : OpC::SM::exch_bytes;
-    constexpr size_t smem = exch + OpA::aux_bytes + OpB::aux_bytes + OpC::aux_bytes;
-    static std::atomic<int> occ_cache[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    int occ = occ_cache[dev & 63].load();
-    if (occ == 0) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, OpA::NT, smem);
-        if (e != cudaSuccess) return e;
-        if (occ < 1) return cudaErrorLaunchOutOfResources;
-        occ_cache[dev & 63].store(occ);
-    }
-    if (ctl->planes <= 0) return cudaSuccess;
-    const long long total = ctl->planes * ((long long)ctl->GA + ctl->GB) + ctl->rows * (long long)ctl->GX;
-    if (total >= (1ll << 31)) return cudaErrorInvalidConfiguration;   // the kernel decodes tickets in 32 bits
-    long long grid = (long long)sm_count * occ;
-    if (grid > total) grid = total;
-    Fused3Ctl f = *ctl;
-    if (f.lag <= 0) f.lag = (int)((grid + f.GA + f.GBk - 1) / ((long long)f.GA + f.GBk)) + 1;
-    kern<<<(unsigned)grid, OpA::NT, smem, st>>>(a, b, c, f);
     return cudaGetLastError();
 }
 
@@ -299,6 +127,61 @@ template <class... Ops> constexpr size_t roles_smem()
     ((exch = Ops::SM::exch_bytes > exch ? Ops::SM::exch_bytes : exch), ...);
     return exch + (Ops::aux_bytes + ...);
 }
+
+// The multi-role kernels below decode their tickets in 32 bits: a launch of 2^31 or more tickets is refused
+template <class OpA, class OpB, typename T, int MINB>
+cudaError_t launch_fused(const void* va, const void* vb, const FusedCtl* ctl, int sm_count, cudaStream_t st)
+{
+    const TileArgs<T>& a = *reinterpret_cast<const TileArgs<T>*>(va);
+    const TileArgs<T>& b = *reinterpret_cast<const TileArgs<T>*>(vb);
+    constexpr auto kern = fft_fused2_kernel<OpA, OpB, T, MINB>;
+    constexpr size_t smem = roles_smem<OpA, OpB>();
+    const long long total = ctl->planes > 0 ? ctl->planes * ((long long)ctl->GA + ctl->GB) : 0;
+    long long grid = 0;
+    const cudaError_t e = resident_grid<kern>(OpA::NT, smem, 0, total, sm_count, grid);
+    if (e != cudaSuccess) return e;
+    if (total >= (1ll << 31)) return cudaErrorInvalidConfiguration;
+    if (grid == 0) return cudaSuccess;
+    FusedCtl c = *ctl;
+    if (c.lag <= 0) c.lag = (int)((grid + c.GA + c.GB - 1) / ((long long)c.GA + c.GB)) + 1;   // role A stays one in-flight window ahead
+    kern<<<(unsigned)grid, OpA::NT, smem, st>>>(a, b, c);
+    return cudaGetLastError();
+}
+
+template <class OpA, class OpB, typename T, int MINB>
+cudaError_t launch_fused_yx(const void* va, const void* vb, const YxCtl* ctl, int sm_count, cudaStream_t st)
+{
+    const TileArgs<T>& a = *reinterpret_cast<const TileArgs<T>*>(va);
+    const TileArgs<T>& b = *reinterpret_cast<const TileArgs<T>*>(vb);
+    constexpr auto kern = fft_fused_yx_kernel<OpA, OpB, T, MINB>;
+    constexpr size_t smem = roles_smem<OpA, OpB>();
+    long long grid = 0;
+    const cudaError_t e = resident_grid<kern>(OpA::NT, smem, 0, (long long)ctl->TA + ctl->TB, sm_count, grid);
+    if (e != cudaSuccess || grid == 0) return e;
+    kern<<<(unsigned)grid, OpA::NT, smem, st>>>(a, b, *ctl);
+    return cudaGetLastError();
+}
+
+template <class OpA, class OpB, class OpC, typename T, int MINB>
+cudaError_t launch_fused3(const void* va, const void* vb, const void* vc, const Fused3Ctl* ctl, int sm_count, cudaStream_t st)
+{
+    const TileArgs<T>& a = *reinterpret_cast<const TileArgs<T>*>(va);
+    const TileArgs<T>& b = *reinterpret_cast<const TileArgs<T>*>(vb);
+    const TileArgs<T>& c = *reinterpret_cast<const TileArgs<T>*>(vc);
+    constexpr auto kern = fft_fused3_kernel<OpA, OpB, OpC, T, MINB>;
+    constexpr size_t smem = roles_smem<OpA, OpB, OpC>();
+    const long long total = ctl->planes > 0 ? ctl->planes * ((long long)ctl->GA + ctl->GB) + ctl->rows * (long long)ctl->GX : 0;
+    long long grid = 0;
+    const cudaError_t e = resident_grid<kern>(OpA::NT, smem, 0, total, sm_count, grid);
+    if (e != cudaSuccess) return e;
+    if (total >= (1ll << 31)) return cudaErrorInvalidConfiguration;
+    if (grid == 0) return cudaSuccess;
+    Fused3Ctl f = *ctl;
+    if (f.lag <= 0) f.lag = (int)((grid + f.GA + f.GBk - 1) / ((long long)f.GA + f.GBk)) + 1;
+    kern<<<(unsigned)grid, OpA::NT, smem, st>>>(a, b, c, f);
+    return cudaGetLastError();
+}
+
 template <class OpA, class OpB, typename T, int MINB> constexpr FusedLaunchFn fused_if_fits()
 {
     if constexpr (roles_smem<OpA, OpB>() <= SMEM_OPTIN_MAX) return launch_fused<OpA, OpB, T, MINB>;
@@ -380,17 +263,17 @@ SizeEntry make_entry(int variant = 0)
         e.launch[PK_XCONV_CO] = launch_conv<SS, T, PEER::C, PEER::TW, true, PEER::MB, PEER::PP>;
         // 1-D convolution of contiguous lines in the contiguous configuration: the complex kernel with the Z pass's register
         // budget, the real one with the real kernels' (shared-memory twiddles, MBI)
-        e.line_conv = launch_line_conv<ZS, T, Z::C, Z::TW, Z::MB, Z::PP, false>;
-        e.line_conv_r2c = launch_line_conv<ZS, T, Z::C, false, MBI, Z::PP, true>;
+        e.launch[PK_LINE_CONV] = launch_line_conv<ZS, T, Z::C, Z::TW, Z::MB, Z::PP, false>;
+        e.launch[PK_LINE_CONV_R2C] = launch_line_conv<ZS, T, Z::C, false, MBI, Z::PP, true>;
         // X and Y passes of whole square planes in one kernel, where both roles share one schedule (and so one twiddle table).
         // Register budget: 64 per thread (2 CTAs of 512 / 4 of 256 threads), except 32-point fp64, which spills at 64 and is
         // given 85 (3 CTAs of 256); 64-point fp64 keeps 2 CTAs of 512 with a small spill (DESIGN.md section 3.8)
         if constexpr (std::is_same<ZS, SS>::value && (ZS::N == 16 || ZS::N == 32 || ZS::N == 64)) {
             constexpr int P = plane_group<ZS>();
             constexpr int MBP = (sizeof(T) == 8 && ZS::N == 32) ? 3 : 1024 / (ZS::T * ZS::N * P);
-            e.plane = launch_plane<ZS, T, P, MBP>;
+            e.launch[PK_PLANE] = launch_plane<ZS, T, P, MBP>;
             // the 2-D convolution of whole images: the plane kernel's CTA shape and register budget
-            e.plane_conv = launch_plane_conv<ZS, T, P, MBP>;
+            e.launch[PK_PLANE_CONV] = launch_plane_conv<ZS, T, P, MBP>;
         }
     }
     // fused two-pass kernels: the contiguous role is re-tiled so that both roles fill the same CTA

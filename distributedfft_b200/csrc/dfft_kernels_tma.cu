@@ -4,6 +4,7 @@
 #include <mutex>
 
 #include "dfft_kernels.cuh"
+#include "dfft_launch.cuh"
 #include "fft_tma.cuh"
 
 namespace dfft {
@@ -47,34 +48,33 @@ int tma_encode_3d(void* map, void* base, int prec, long long d0, long long d1, l
     return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
+// The TMA kernels run one CTA per SM (their rings fill its shared memory), so they need the shared-memory opt-in but no
+// occupancy query
+template <class S, typename T, int C, int M>
+static cudaError_t launch_tma_mode(const TmaArgs<T>& a, const CUtensorMap& mi, const CUtensorMap& mo, int sm_count, cudaStream_t st)
+{
+    constexpr auto kern = fft_tma_pass_kernel<S, T, C, M>;
+    constexpr size_t smem = TmaGeom<S, T, C>::PASS_SMEM;
+    const cudaError_t e = smem_optin<kern>(smem);
+    if (e != cudaSuccess || a.ntiles <= 0) return e;
+    kern<<<(unsigned)grid_for(sm_count, 1, 0, a.ntiles), S::T * C, smem, st>>>(a, mi, mo);
+    return cudaGetLastError();
+}
+
 template <class S, typename T, int C>
 static cudaError_t launch_tma(int mode, const void* vargs, const void* map_in, const void* map_out, int sm_count, cudaStream_t st)
 {
     const TmaArgs<T>& a = *reinterpret_cast<const TmaArgs<T>*>(vargs);
-    using G_ = TmaGeom<S, T, C>;
     static CUtensorMap dummy{};
     const CUtensorMap& mi = map_in ? *reinterpret_cast<const CUtensorMap*>(map_in) : dummy;
     const CUtensorMap& mo = map_out ? *reinterpret_cast<const CUtensorMap*>(map_out) : dummy;
-    if (a.ntiles <= 0) return cudaSuccess;
-    long long grid = sm_count;
-    if (grid > a.ntiles) grid = a.ntiles;
-    cudaError_t e = cudaSuccess;
-#define DFFT_TMA_LAUNCH(M)                                                                                                  \
-    {                                                                                                                       \
-        auto kern = fft_tma_pass_kernel<S, T, C, M>;                                                                        \
-        static bool attr = false;                                                                                           \
-        if (!attr) { e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_::PASS_SMEM); if (e != cudaSuccess) return e; attr = true; } \
-        kern<<<(unsigned)grid, S::T * C, G_::PASS_SMEM, st>>>(a, mi, mo);                                                   \
-    }
     switch (mode) {
-        case TMA_Z: DFFT_TMA_LAUNCH(TMA_Z) break;
-        case TMA_Y: DFFT_TMA_LAUNCH(TMA_Y) break;
-        case TMA_XF: DFFT_TMA_LAUNCH(TMA_XF) break;
-        case TMA_XB: DFFT_TMA_LAUNCH(TMA_XB) break;
+        case TMA_Z: return launch_tma_mode<S, T, C, TMA_Z>(a, mi, mo, sm_count, st);
+        case TMA_Y: return launch_tma_mode<S, T, C, TMA_Y>(a, mi, mo, sm_count, st);
+        case TMA_XF: return launch_tma_mode<S, T, C, TMA_XF>(a, mi, mo, sm_count, st);
+        case TMA_XB: return launch_tma_mode<S, T, C, TMA_XB>(a, mi, mo, sm_count, st);
         default: return cudaErrorInvalidValue;
     }
-#undef DFFT_TMA_LAUNCH
-    return cudaGetLastError();
 }
 
 template <class S, typename T, int C>
@@ -82,18 +82,13 @@ static cudaError_t launch_tma_fused_zy(const void* vargs, const FusedCtl* ctl, c
 {
     const TmaFusedArgs<T>& a = *reinterpret_cast<const TmaFusedArgs<T>*>(vargs);
     using G_ = TmaGeom<S, T, C>;
-    auto kern = fft_tma_fused_zy_kernel<S, T, C>;
-    static bool attr = false;
-    if (!attr) {
-        const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_::SMEM);
-        if (e != cudaSuccess) return e;
-        attr = true;
-    }
+    constexpr auto kern = fft_tma_fused_zy_kernel<S, T, C>;
+    const cudaError_t e = smem_optin<kern>(G_::SMEM);
+    if (e != cudaSuccess) return e;
     if (ctl->planes <= 0) return cudaSuccess;
     const long long total = ctl->planes * ((long long)ctl->GA + ctl->GB);
     if (total >= (1ll << 31)) return cudaErrorInvalidConfiguration;   // the kernel decodes tickets in 32 bits
-    long long grid = sm_count;
-    if (grid > total) grid = total;
+    const long long grid = grid_for(sm_count, 1, 0, total);
     FusedCtl c = *ctl;
     // the Z role runs ahead of the Y role by the tiles the rings hold beside the ones each CTA is transforming
     // (NSLOT - NGROUP per CTA): 3 planes at 512 points on 132 SMs.  Each plane more keeps another 4 MiB of intermediate in

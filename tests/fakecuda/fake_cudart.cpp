@@ -25,7 +25,6 @@ struct dim3_ { unsigned x, y, z; };
 struct cudaIpcMemHandle_st { char reserved[64]; };
 
 static std::atomic<long long> g_launches{0}, g_events{0}, g_mallocs{0}, g_frees{0};
-static thread_local int t_device = 0;
 static thread_local dim3_ t_grid, t_block;
 static thread_local size_t t_smem;
 static thread_local cudaStream_t t_stream;
@@ -131,9 +130,45 @@ static int tile_args_params(const std::string& name)
     return 0;
 }
 
+// --- launch set-up per (device, kernel stub), the device being the calling thread's current one: the dynamic shared-memory limit
+// raised with cudaFuncSetAttribute(cudaFuncAttributeMaxDynamicSharedMemorySize), and how often the limit was raised, the
+// occupancy queried and the kernel launched.  As on the real runtime, a launch asking for more than 48 KiB of dynamic shared
+// memory fails unless this device's limit for the kernel covers it; a <<<>>> launch reports that through cudaGetLastError.
+// Not traced: the golden traces stay as they are
+struct LaunchSetup { long long smem_limit, attr_calls, occ_queries, launches; };
+static std::mutex& setup_mu() { static std::mutex m; return m; }
+static std::map<std::pair<int, const void*>, LaunchSetup>& setups() { static std::map<std::pair<int, const void*>, LaunchSetup> m; return m; }
+static thread_local int t_device = 0;
+static thread_local cudaError_t t_last_error = 0;
+
+// one line per (device, kernel): "device attr_calls occ_queries launches name"; returns the bytes needed (with the terminating zero)
+long long fakecuda_launch_setup(char* buf, long long cap)
+{
+    std::string o;
+    {
+        std::lock_guard<std::mutex> g(setup_mu());
+        for (const auto& kv : setups()) {
+            char line[64];
+            snprintf(line, sizeof(line), "%d %lld %lld %lld ", kv.first.first, kv.second.attr_calls, kv.second.occ_queries, kv.second.launches);
+            std::lock_guard<std::mutex> n(names_mu());
+            auto it = kernel_names().find(kv.first.second);
+            o += line + (it == kernel_names().end() ? std::string("?") : it->second) + "\n";
+        }
+    }
+    const long long n = (long long)o.size() + 1;
+    if (buf && cap >= n) memcpy(buf, o.c_str(), (size_t)n);
+    return n;
+}
+
 cudaError_t cudaLaunchKernel(const void* stub, dim3_ grid, dim3_ block, void** args, size_t smem, cudaStream_t st)
 {
     if (grid.x == 0 || block.x == 0 || block.x * block.y * block.z > 1024) return 9;   // cudaErrorInvalidConfiguration
+    {
+        std::lock_guard<std::mutex> g(setup_mu());
+        LaunchSetup& s = setups()[{t_device, stub}];
+        if (smem > 48 * 1024 && (long long)smem > s.smem_limit) return t_last_error = 1;   // cudaErrorInvalidValue
+        s.launches++;
+    }
     std::string name = "?";
     {
         std::lock_guard<std::mutex> g(names_mu());
@@ -169,10 +204,25 @@ cudaError_t cudaDeviceGetAttribute(int* v, int, int) { *v = 132; return 0; }
 cudaError_t cudaDeviceSynchronize(void) { return 0; }
 cudaError_t cudaDeviceCanAccessPeer(int* can, int, int) { *can = 1; return 0; }
 cudaError_t cudaDeviceEnablePeerAccess(int, unsigned) { return 0; }
-cudaError_t cudaGetLastError(void) { return 0; }
+cudaError_t cudaGetLastError(void) { const cudaError_t e = t_last_error; t_last_error = 0; return e; }
 const char* cudaGetErrorString(cudaError_t e) { return e ? "fake CUDA error" : "no error"; }
-cudaError_t cudaFuncSetAttribute(const void*, int, int) { return 0; }
-cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(int* n, const void*, int, size_t, unsigned) { *n = 2; return 0; }
+cudaError_t cudaFuncSetAttribute(const void* stub, int attr, int value)
+{
+    if (attr == 8) {   // cudaFuncAttributeMaxDynamicSharedMemorySize
+        std::lock_guard<std::mutex> g(setup_mu());
+        LaunchSetup& s = setups()[{t_device, stub}];
+        s.smem_limit = value;
+        s.attr_calls++;
+    }
+    return 0;
+}
+cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(int* n, const void* stub, int, size_t, unsigned)
+{
+    std::lock_guard<std::mutex> g(setup_mu());
+    setups()[{t_device, stub}].occ_queries++;
+    *n = 2;
+    return 0;
+}
 
 // --- memory: plain host memory (sizes are test-sized)
 static std::mutex& allocs_mu() { static std::mutex m; return m; }

@@ -117,7 +117,8 @@ WORKER = textwrap.dedent(r'''
         return r
     EINVAL = -1
     assert dfft.debug_launch_op(bad(op="Q"), dfft.DOUBLE) == EINVAL                      # unknown op
-    assert dfft.debug_launch_op(bad(op="Z_R2C"), dfft.DOUBLE) == EINVAL                  # a real-data record
+    for o in ("Z_R2C", "XY_PLANE", "XY_PLANE_CONV", "LINE_CONV", "LINE_CONV_R2C"):
+        assert dfft.debug_launch_op(bad(op=o), dfft.DOUBLE) == EINVAL                    # a real-data or lines-engine record
     for o in ("ovlZ", "ovlY", "ovlX"):
         assert dfft.debug_launch_op(bad(op=o), dfft.DOUBLE) == EINVAL                    # single-kernel forward
     assert dfft.debug_launch_op(yco, 2) == EINVAL and dfft.debug_launch_op(yco, -1) == EINVAL   # precision
