@@ -38,7 +38,7 @@ __all__ = [
     "BootstrapComm", "fft_mpi_init", "fft_mpi_plan_dft_c2c_3d", "fft_mpi_execute_dft_3d_c2c", "fft_mpi_destroy_plan",
     "fft_mpi_alloc_local_memory", "fft_mpi_local_size_3d", "fft_mpi_cleanup", "getMaxDataCount", "supported_lengths",
     "fft_mpi_plan_dft_r2c_3d", "local_size_r2c_3d", "fft_mpi_plan_dft_convolve_3d",
-    "fft_lines", "lines_ops", "LinesPlan", "RealLinesPlan", "real_lines_ops", "lines_3d_ops", "LinesConvolvePlan", "lines_conv_3d_ops", "lines_conv_2d_ops", "lines_conv_1d_ops", "length_kind", "length_schedule", "memcpy_htod", "memcpy_dtoh", "memcpy_dtod", "debug_launch_op", "exchange_table", "comm_allgather",
+    "fft_lines", "lines_ops", "LinesPlan", "RealLinesPlan", "real_lines_ops", "lines_3d_ops", "LinesConvolvePlan", "lines_conv_3d_ops", "lines_conv_2d_ops", "lines_conv_1d_ops", "lines_conv_padded_1d_ops", "length_kind", "length_schedule", "memcpy_htod", "memcpy_dtoh", "memcpy_dtod", "debug_launch_op", "exchange_table", "comm_allgather",
 ]
 
 
@@ -134,6 +134,9 @@ def lib():
     L.dfft_lines_plan_create_convolve_r2c_1d.argtypes = [i, ll, i, ctypes.c_uint, P(vp)]
     L.dfft_debug_lines_conv_1d_ops.argtypes = [i, ll, i, i, ctypes.c_uint, ll, ctypes.c_char_p, ll]
     L.dfft_debug_lines_conv_1d_ops.restype = ll
+    L.dfft_lines_plan_create_convolve_padded_1d.argtypes = [i, ll, ll, ll, i, ctypes.c_uint, P(vp)]
+    L.dfft_debug_lines_conv_padded_1d_ops.argtypes = [i, ll, ll, ll, i, ctypes.c_uint, ll, ctypes.c_char_p, ll]
+    L.dfft_debug_lines_conv_padded_1d_ops.restype = ll
     L.dfft_debug_real_lines_ops.argtypes = [i, i, ll, i, i, i, ctypes.c_char_p, ll]
     L.dfft_debug_real_lines_ops.restype = ll
     L.dfft_length_kind.argtypes = [i, i]
@@ -493,14 +496,23 @@ class LinesConvolvePlan(_LinesPlanBase):
     each its own.  in_ptr == out_ptr runs in place; `in` and the multiplier are never written otherwise.
     `two_d=(nx, ny, batch)` instead: the same over the last two axes of a[batch][ny][nx] (m: [ny][nx], real: [ny][nx//2+1]
     per image).  `one_d=(n, nlines)` instead: out = ifft(fft(in) * m) per line of a[nlines][n] (m: [n], real: [n//2+1] per line),
-    one kernel launch per execute.  Exactly one of one_d, two_d and three_d is given."""
+    one kernel launch per execute.  Exactly one of one_d, two_d and three_d is given.
+    `padded=(in_len, out_len)` with one_d (complex only): the zero-padded convolution out[l] = ifft(fft(in[l], n) * m)[:out_len]
+    of a[nlines][in_len] into out[nlines][out_len] (dfft_lines_plan_create_convolve_padded_1d), which also takes lines longer
+    than one shared-memory line."""
 
-    def __init__(self, three_d=None, precision=DOUBLE, real=False, flags=0, two_d=None, one_d=None):
+    def __init__(self, three_d=None, precision=DOUBLE, real=False, flags=0, two_d=None, one_d=None, padded=None):
         shapes = {"3d": three_d, "2d": two_d, "1d": one_d}
         given = [d for d, s in shapes.items() if s is not None]
         if len(given) != 1:
             raise ValueError("give exactly one of one_d, two_d and three_d")
         dims = given[0]
+        if padded is not None:
+            if dims != "1d" or real:
+                raise ValueError("padded=(in_len, out_len) is a complex one_d plan")
+            n, nlines = one_d
+            self._create("dfft_lines_plan_create_convolve_padded_1d", n, padded[0], padded[1], nlines, precision, flags)
+            return
         name = ("dfft_lines_plan_create_convolve_r2c_" if real else "dfft_lines_plan_create_convolve_") + dims
         self._create(name, *shapes[dims], precision, flags)
 
@@ -538,6 +550,13 @@ def lines_conv_1d_ops(n, nlines, precision=DOUBLE, real=False, flags=0, mult_cou
     dfft_debug_lines_conv_1d_ops; buffers as lines_conv_3d_ops); read DFFT_GENERIC / DFFT_VARIANT at the call, as plan creation
     does"""
     return _json_hook(lib().dfft_debug_lines_conv_1d_ops, n, nlines, precision, int(bool(real)), flags, mult_count)
+
+
+def lines_conv_padded_1d_ops(n, in_len, out_len, nlines, precision=DOUBLE, flags=0, mult_count=1):
+    """passes LinesConvolvePlan(one_d=(n, nlines), padded=(in_len, out_len), ...) would launch per execute (host-only test hook,
+    see dfft_debug_lines_conv_padded_1d_ops; buffers as lines_conv_3d_ops, temporary = 4); read DFFT_GENERIC / DFFT_VARIANT at
+    the call, as plan creation does"""
+    return _json_hook(lib().dfft_debug_lines_conv_padded_1d_ops, n, in_len, out_len, nlines, precision, flags, mult_count)
 
 
 def real_lines_ops(n, nlines, direction, precision=DOUBLE, two_d=None):

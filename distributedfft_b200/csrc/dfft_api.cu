@@ -495,7 +495,8 @@ static inline cudaError_t ev_record_on(dfft_plan p, cudaEvent_t e, cudaStream_t 
 static inline cudaError_t stream_wait(dfft_plan p, cudaStream_t st, cudaEvent_t e) { return p->dry ? cudaSuccess : cudaStreamWaitEvent(st, e, 0); }
 
 static const char* const kPassNames[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW", "Z_R2C", "Z_C2R", "XCONV", "XCONV_CO",
-                                                  "XY_PLANE", "XY_PLANE_CONV", "LINE_CONV", "LINE_CONV_R2C"};
+                                                  "XY_PLANE", "XY_PLANE_CONV", "LINE_CONV", "LINE_CONV_R2C", "LINE_CONV_PAD",
+                                                  "XF_TW_PAD", "XB_TW_PAD"};
 
 // `extra`: further fields of the record, each starting with ", "
 template <typename T>
@@ -2387,6 +2388,7 @@ struct LinePass {
     long long tw_n = 0;          // four-step twiddle modulus (PK_XF_TW)
     int src = LB_IN, dst = LB_IN;   // LB_IN (the caller's data / a real or convolve plan's `in`), LB_TEMP (the plan's temporary), LB_OUT
     long long ld_in = 0, ld_out = 0;   // PK_Z_R2C / PK_Z_C2R / PK_LINE_CONV_R2C: distance between the two lines of a pair (RealZArgs), each side's elements
+    long long in_len = 0, out_len = 0; // padded kinds (PadArgs): points of a line read from `in` / stored to `out`
     bool inv = false;            // the inverse transform
 };
 // which execute runs a plan: dfft_lines_execute, dfft_lines_execute_real or dfft_lines_execute_convolve
@@ -2404,6 +2406,7 @@ struct dfft_lines_plan_s {
     struct Lut { const SizeEntry* e; int kind; void* d; };
     std::vector<Lut> luts;       // twiddle tables, one per (entry, schedule), shared by the passes that run it
     long long rcount = 0, ccount = 0;   // reals and complex elements of the caller's real / complex buffer
+    long long in_count = 0, out_count = 0;   // convolve: elements of `in` and of `out` (dfft_lines_execute_convolve's buffer extents)
     long long batch = 0, mvol = 0;   // convolve: volumes (images); complex elements of one volume's (image's) multiplier
     double scale = 0;                // DFFT_SCALE_BACKWARD: 1 / (elements of a volume or image), folded into the multiply; 0 = unnormalised
     cudaStream_t stream = nullptr;
@@ -2419,10 +2422,12 @@ static bool fits_int(long long a, long long b = 1, long long c = 1)
 }
 
 // the plain pass kind whose tile size (kind_C) and twiddle schedule (upload_lut_kind) a lines pass has: the real kernels run the
-// contiguous configuration, the column convolve the strided one, the plane kernels the contiguous schedule and the line convolve
-// kernels the contiguous configuration
+// contiguous configuration, the column convolve the strided one, the plane kernels the contiguous schedule, the line convolve
+// kernels the contiguous configuration and the padded four-step passes the X configuration of the passes they extend
 static int plain_kind(int kind)
 {
+    if (kind == PK_XF_TW_PAD) return PK_XF_TW;
+    if (kind == PK_XB_TW_PAD) return PK_XB;
     return kind == PK_XCONV ? PK_Y : (kind == PK_Z_R2C || kind == PK_Z_C2R || kind >= PK_PLANE) ? PK_Z : kind;
 }
 
@@ -2489,23 +2494,31 @@ static int complex_lists(dfft_lines_plan p, int n, bool ordered)
 // -- what the reference does with its multi-upload axes and reorderFourStep = 1 (templateFFT.cpp:4007-4106, 5951).
 // Validated against numpy (tests/test_gpu_parity.py::test_four_step_long_lines);
 // DFFT_NO_LONG_LINES=1 restores the "unsupported length" answer.
-static int make_four_step(dfft_lines_plan p, int n, long long nlines)
+// The split n = n1 * n2 of a four-step plan: of the splits whose entries `accept` takes (n1 <= 2 sqrt(n)), the one with the most
+// tuned factors, then the most nearly square, then the smallest n1; 0 when there is none
+template <class Accept> static int four_step_split(int n, int precision, Accept accept)
 {
-    const int precision = p->prec;
     long long best1 = 0;
     int best_score = -1;
     for (long long d = 2; d * d <= (long long)n * 4 && d < n; d++) {
         if (n % d) continue;
         const SizeEntry *e1 = find_size_entry((int)d, precision), *e2 = find_size_entry((int)(n / d), precision);
-        if (!e1 || !e2) continue;
+        if (!e1 || !e2 || !accept(e1, e2)) continue;
         const long long q = n / d;
         const double ratio = d > q ? (double)d / q : (double)q / d;
         int score = (e1->gen ? 0 : 1000) + (e2->gen ? 0 : 1000) + (int)(500.0 / ratio);
         if (score > best_score) { best_score = score; best1 = d; }
     }
-    if (!best1) return fail(DFFT_EUNSUPPORTED, "length %d cannot be split into two supported factors", n);
+    return (int)best1;
+}
+
+static int make_four_step(dfft_lines_plan p, int n, long long nlines)
+{
+    const int precision = p->prec;
+    const int n1 = four_step_split(n, precision, [](const SizeEntry*, const SizeEntry*) { return true; });
+    if (!n1) return fail(DFFT_EUNSUPPORTED, "length %d cannot be split into two supported factors", n);
     if (!fits_int(nlines)) return fail(DFFT_EUNSUPPORTED, "%lld rows: at most 2^31 - 1 per plan", nlines);
-    const int n1 = (int)best1, n2 = n / n1;
+    const int n2 = n / n1;
     p->temp_bytes = (size_t)nlines * n * (precision == DFFT_FLOAT ? 8 : 16);
     // pass A: columns of the [n1][n2] matrix of every line, transposed store + twiddle
     LinePass& a = p->run[0][0];
@@ -2698,6 +2711,7 @@ static int make_lines_conv(dfft_lines_plan p, int dims, int nx, int ny, int nz, 
     p->mvol = real ? vol / nx * (nx / 2 + 1) : vol;
     if (real) p->rcount = vol * batch;
     else p->ccount = vol * batch;
+    p->in_count = p->out_count = real ? p->rcount : p->ccount;
     p->scale = (flags & DFFT_SCALE_BACKWARD) ? 1.0 / (double)vol : 0.0;
     return 0;
 }
@@ -2741,6 +2755,82 @@ static int make_lines_conv_1d(dfft_lines_plan p, int n, long long nlines, bool r
     p->mvol = real ? n / 2 + 1 : n;
     if (real) p->rcount = nlines * n;
     else p->ccount = nlines * n;
+    p->in_count = p->out_count = real ? p->rcount : p->ccount;
+    p->scale = (flags & DFFT_SCALE_BACKWARD) ? 1.0 / (double)n : 0.0;
+    return 0;
+}
+
+// ---- zero-padded 1-D spectral convolution: out[l] = ifft(fft(zero_pad(in[l], n)) * m_l)[0:out_len] -----------------------------
+// `nlines` lines of in_len points in and of out_len points out, each densely packed; 1 <= in_len, out_len <= n.  Two paths, chosen
+// from n:
+//   short (n has a tuned default entry): LINE_CONV_PAD in -> out, the line-convolve kernel with the padding folded into its loads
+//          and stores.  No temporary; (in_len + out_len) elements per line and the multiplier.
+//   long  (n = n1 * n2 of tuned default entries, n2 with the column-convolve kernel): the four-step plan without its reorder,
+//          XF_TW_PAD in -> temp (FFT along n1, twiddle, transposed store: temp [n2][n1] of every line), XCONV in temp (FFT along
+//          n2, multiply, inverse FFT along n2: element (k2, k1) of temp is X[k1 + n1*k2], so the natural-order multiplier sits at
+//          the element's own offset), XB_TW_PAD temp -> out (twiddle prologue, inverse FFT along n1, strided store).  A temporary
+//          of nlines * n elements; (in_len + 4n + out_len) elements per line and the multiplier.
+// in == out works when in_len == out_len: a short-path tile holds its lines in registers before it stores, and the long path
+// reads `in` only in its first pass
+static int make_lines_conv_padded_1d(dfft_lines_plan p, int n, long long in_len, long long out_len, long long nlines, unsigned flags)
+{
+    const int precision = p->prec;
+    if (flags & ~DFFT_SCALE_BACKWARD) return fail(DFFT_EINVAL, "convolve lines plans take no flag but DFFT_SCALE_BACKWARD");
+    if (n < 1 || nlines < 0 || bad_precision(precision)) return fail(DFFT_EINVAL, "bad arguments");
+    if (in_len < 1 || in_len > n || out_len < 1 || out_len > n)
+        return fail(DFFT_EINVAL, "in_len %lld and out_len %lld must lie in [1, n = %d]", in_len, out_len, n);
+    if (!fits_int(nlines)) return fail(DFFT_EUNSUPPORTED, "%lld lines: at most 2^31 - 1 per plan", nlines);
+    const SizeEntry* e = find_size_entry(n, precision);
+    LinePass* f = p->run[0];
+    if (e && !e->gen) {   // a tuned length: a default entry has the padded line-convolve kernel, an alternate tuning does not
+        if (!e->launch[PK_LINE_CONV_PAD])
+            return fail(DFFT_EUNSUPPORTED, "length %d has no padded line-convolution kernel (DFFT_VARIANT entries are not convolved)", n);
+        const int C = e->z_C;
+        LinePass& lp = f[0];
+        lp.e = e;
+        lp.kind = PK_LINE_CONV_PAD;
+        lp.src = LB_IN; lp.dst = LB_OUT;
+        lp.W = (int)nlines; lp.G = (int)cdiv(nlines, C); lp.ntiles = lp.G;
+        lp.ia = Affine{0, C * in_len, in_len, 1};
+        lp.oa = Affine{0, C * out_len, out_len, 1};
+        p->nrun[0] = 1;
+    } else {
+        const int n1 = four_step_split(n, precision, [](const SizeEntry* e1, const SizeEntry* e2) {
+            return !e1->gen && e1->launch[PK_XF_TW_PAD] && e1->launch[PK_XB_TW_PAD] && !e2->gen && e2->launch[PK_XCONV];
+        });
+        if (!n1)
+            return fail(DFFT_EUNSUPPORTED, "length %d is neither a tuned length nor a product n1 * n2 of tuned lengths of the default kernel "
+                        "table (n1 <= 2 sqrt(n)) with the kernels of the padded convolution", n);
+        const int n2 = n / n1;
+        LinePass& a = f[0];   // columns j2 of the [n1][n2] view of each input line -> temp [j2][k1], twiddled
+        a.e = find_size_entry(n1, precision);
+        const int CA = a.e->x_C;
+        a.kind = PK_XF_TW_PAD; a.src = LB_IN; a.dst = LB_TEMP; a.tw_n = n;
+        a.G = (int)cdiv(n2, CA); a.W = n2; a.ntiles = nlines * a.G;
+        a.ia = Affine{in_len, CA, 1, n2};
+        a.oa = Affine{(long long)n, (long long)CA * n1, n1, 1};
+        LinePass& b = f[1];   // columns k1 of temp [n2][n1]: forward along n2, multiply, inverse, in place
+        b.e = find_size_entry(n2, precision);
+        const int CB = b.e->s_C;
+        b.kind = PK_XCONV; b.src = b.dst = LB_TEMP;
+        b.G = (int)cdiv(n1, CB); b.W = n1; b.ntiles = nlines * b.G;
+        b.ia = b.oa = Affine{(long long)n, CB, 1, n1};
+        LinePass& c = f[2];   // rows j2 of temp -> output line offsets j1*n2 + j2
+        c.e = a.e;
+        c.kind = PK_XB_TW_PAD; c.src = LB_TEMP; c.dst = LB_OUT; c.tw_n = n; c.inv = true;
+        c.G = a.G; c.W = n2; c.ntiles = a.ntiles;
+        c.ia = Affine{(long long)n, (long long)CA * n1, n1, 1};
+        c.oa = Affine{out_len, CA, 1, n2};
+        p->nrun[0] = 3;
+        p->temp_bytes = (size_t)nlines * n * (precision == DFFT_FLOAT ? 8 : 16);
+    }
+    for (int k = 0; k < p->nrun[0]; k++) { f[k].in_len = in_len; f[k].out_len = out_len; }
+    p->nrun[1] = 0;
+    p->form = LF_CONV;
+    p->batch = nlines;
+    p->mvol = n;
+    p->in_count = nlines * in_len;
+    p->out_count = nlines * out_len;
     p->scale = (flags & DFFT_SCALE_BACKWARD) ? 1.0 / (double)n : 0.0;
     return 0;
 }
@@ -2854,6 +2944,12 @@ extern "C" int dfft_lines_plan_create_convolve_r2c_1d(int n, long long nlines, i
     return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv_1d(p, n, nlines, true, flags); });
 }
 
+extern "C" int dfft_lines_plan_create_convolve_padded_1d(int n, long long in_len, long long out_len, long long nlines, int precision,
+                                                         unsigned flags, dfft_lines_plan* plan)
+{
+    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv_padded_1d(p, n, in_len, out_len, nlines, flags); });
+}
+
 extern "C" int dfft_lines_plan_create_convolve_2d(int nx, int ny, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
 {
     return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv(p, 2, nx, ny, 1, batch, false, flags); });
@@ -2877,8 +2973,10 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
 {
     const void* src = line_buf(lp.src, in, out, p->temp);
     void* dst = line_buf(lp.dst, in, out, p->temp);
-    const bool conv = lp.kind == PK_XCONV || lp.kind == PK_PLANE_CONV || lp.kind == PK_LINE_CONV || lp.kind == PK_LINE_CONV_R2C;
+    const bool conv = lp.kind == PK_XCONV || lp.kind == PK_PLANE_CONV || lp.kind == PK_LINE_CONV || lp.kind == PK_LINE_CONV_R2C ||
+                      lp.kind == PK_LINE_CONV_PAD;
     const bool realk = lp.kind == PK_Z_R2C || lp.kind == PK_Z_C2R || lp.kind == PK_LINE_CONV_R2C;
+    const bool pad = lp.kind == PK_LINE_CONV_PAD || lp.kind == PK_XF_TW_PAD || lp.kind == PK_XB_TW_PAD;
     ConvArgs<T> c{};
     TileArgs<T>& a = c.t;
     a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)lp.lut;
@@ -2892,9 +2990,11 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
         char extra[192] = "";
         int len = 0;
         if (realk) len = snprintf(extra, sizeof(extra), ", \"nzh\": %d, \"pair\": [%lld, %lld]", lp.e->N / 2 + 1, lp.ld_in, lp.ld_out);
+        if (pad) len = snprintf(extra, sizeof(extra), ", \"in_len\": %lld, \"out_len\": %lld", lp.in_len, lp.out_len);
         if (conv) snprintf(extra + len, sizeof(extra) - len, ", \"mult\": %llu, \"shared\": %d", (unsigned long long)(size_t)mult, shared ? 1 : 0);
         const bool plane = lp.kind == PK_PLANE || lp.kind == PK_PLANE_CONV;
-        record_op<T>(*ops, kPassNames[lp.kind], phase, lp.e->N, plane ? lp.e->N : kind_C(lp.e, plain_kind(lp.kind)), false, false, lp.kind == PK_XF_TW, a,
+        record_op<T>(*ops, kPassNames[lp.kind], phase, lp.e->N, plane ? lp.e->N : kind_C(lp.e, plain_kind(lp.kind)), false, false,
+                     lp.kind == PK_XF_TW || lp.kind == PK_XF_TW_PAD, a,
                      extra);
         return cudaSuccess;
     }
@@ -2902,6 +3002,7 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
     PlaneConvArgs<T> pc{};      // PK_PLANE: pc.p
     RealLineConvArgs<T> rl{};   // PK_Z_R2C / PK_Z_C2R: rl.r
     LineConvArgs<T> lc{};
+    PadArgs<T> pa{};
     const void* args = conv ? (const void*)&c : (const void*)&a;
     switch (lp.kind) {
     case PK_PLANE:
@@ -2923,6 +3024,10 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
     case PK_LINE_CONV_R2C:
         rl = {{a, (const T*)src, (T*)dst, lp.ld_in, lp.ld_out}, c.mult, shared ? 0 : (long long)(lp.e->N / 2 + 1)};
         args = &rl;
+        break;
+    case PK_LINE_CONV_PAD: case PK_XF_TW_PAD: case PK_XB_TW_PAD:
+        pa = {{a, c.mult, shared ? 0 : (long long)lp.e->N}, lp.in_len, lp.out_len};
+        args = &pa;
         break;
     }
     return lp.e->launch[lp.kind](args, p->sms, p->stream);
@@ -2977,9 +3082,10 @@ extern "C" int dfft_lines_execute_convolve(dfft_lines_plan p, const void* in, vo
     const size_t rsz = p->prec == DFFT_FLOAT ? 4 : 8, csz = 2 * rsz, esz = real ? rsz : csz;
     const uintptr_t a = (uintptr_t)in, b = (uintptr_t)out, m = (uintptr_t)mult;
     if (a % esz || b % esz || m % csz) return fail(DFFT_EINVAL, "a buffer is not aligned to its element size");
-    const uintptr_t io = (uintptr_t)((real ? p->rcount : p->ccount) * esz), mb = (uintptr_t)(mult_count * p->mvol * csz);
-    if (a != b && a < b + io && b < a + io) return fail(DFFT_EINVAL, "`in` and `out` overlap without being the same buffer");
-    if (m < b + io && b < m + mb) return fail(DFFT_EINVAL, "the multiplier overlaps `out`");
+    const uintptr_t ib = (uintptr_t)(p->in_count * esz), ob = (uintptr_t)(p->out_count * esz), mb = (uintptr_t)(mult_count * p->mvol * csz);
+    if (a == b && p->in_count != p->out_count) return fail(DFFT_EINVAL, "in place (in == out) needs lines of the same length in and out");
+    if (a != b && a < b + ob && b < a + ib) return fail(DFFT_EINVAL, "`in` and `out` overlap without being the same buffer");
+    if (m < b + ob && b < m + mb) return fail(DFFT_EINVAL, "the multiplier overlaps `out`");
     const bool shared = mult_count == 1;
     return p->prec == DFFT_DOUBLE ? lines_run<double>(p, 0, in, out, mult, shared) : lines_run<float>(p, 0, in, out, mult, shared);
 }
@@ -3071,6 +3177,19 @@ extern "C" long long dfft_debug_lines_conv_1d_ops(int n, long long nlines, int p
 {
     auto build = [&](dfft_lines_plan p) {
         const int rc = make_lines_conv_1d(p, n, nlines, real != 0, flags);
+        return rc || mult_count == 1 || mult_count == nlines ? rc : fail(DFFT_EINVAL, "mult_count must be 1 or the plan's line count");
+    };
+    return lines_ops_json(precision, build, 0, 5, 2, mult_count == 1, buf, cap);
+}
+
+/* test hook (host only): the passes of a zero-padded 1-D convolve lines plan, JSON as dfft_debug_lines_conv_1d_ops (in = buffer 5,
+ * out = 2, temporary = 4, multiplier = 8 of device 0).  Short path: one "LINE_CONV_PAD" record; long path: "XF_TW_PAD", "XCONV",
+ * "XB_TW_PAD".  The padded records carry "in_len" and "out_len", LINE_CONV_PAD and XCONV "mult" and "shared" */
+extern "C" long long dfft_debug_lines_conv_padded_1d_ops(int n, long long in_len, long long out_len, long long nlines, int precision,
+                                                         unsigned flags, long long mult_count, char* buf, long long cap)
+{
+    auto build = [&](dfft_lines_plan p) {
+        const int rc = make_lines_conv_padded_1d(p, n, in_len, out_len, nlines, flags);
         return rc || mult_count == 1 || mult_count == nlines ? rc : fail(DFFT_EINVAL, "mult_count must be 1 or the plan's line count");
     };
     return lines_ops_json(precision, build, 0, 5, 2, mult_count == 1, buf, cap);

@@ -32,6 +32,10 @@ enum PassKind {
                        // PK_PLANE is
     PK_LINE_CONV,      // 1-D convolution of contiguous lines in one pass (fft_line_conv_kernel; args = LineConvArgs)
     PK_LINE_CONV_R2C,  // + real lines, two per complex transform (fft_line_conv_r2c_kernel; args = RealLineConvArgs)
+    // the zero-padded 1-D convolve lines plans (args = PadArgs); default entries only, else nullptr
+    PK_LINE_CONV_PAD,  // PK_LINE_CONV over lines of in_len points in and out_len out (fft_line_conv_pad_kernel), contiguous configuration
+    PK_XF_TW_PAD,      // PK_XF_TW reading input lines of in_len points (fft_four_step_pad_kernel), X configuration
+    PK_XB_TW_PAD,      // its inverse: contiguous load, twiddle prologue, strided store to output lines of out_len points, X configuration
     PK_COUNT
 };
 

@@ -88,6 +88,24 @@ cudaError_t launch_line_conv(const void* vargs, int sm_count, cudaStream_t st)
     return cudaGetLastError();
 }
 
+// the zero-padded 1-D convolve lines plans' kinds: vargs is a PadArgs<T>; PK_LINE_CONV_PAD runs fft_line_conv_pad_kernel,
+// PK_XF_TW_PAD / PK_XB_TW_PAD the forward / inverse fft_four_step_pad_kernel
+template <class S, typename T, int C, bool TW, int MINB, bool PP, int KIND>
+cudaError_t launch_pad(const void* vargs, int sm_count, cudaStream_t st)
+{
+    const PadArgs<T>& a = *reinterpret_cast<const PadArgs<T>*>(vargs);
+    constexpr auto kern = [] {   // only the kernel of this kind is instantiated
+        if constexpr (KIND == PK_LINE_CONV_PAD) return fft_line_conv_pad_kernel<S, T, C, TW, MINB, PP>;
+        else return fft_four_step_pad_kernel<S, T, C, TW, MINB, PP, KIND == PK_XF_TW_PAD>;
+    }();
+    constexpr size_t smem = TileSmem<S, T, C, PP>::bytes(false);
+    long long grid = 0;
+    const cudaError_t e = resident_grid<kern>(S::T * C, smem, 0, a.c.t.ntiles, sm_count, grid);
+    if (e != cudaSuccess || grid == 0) return e;
+    kern<<<(unsigned)grid, S::T * C, smem, st>>>(a);
+    return cudaGetLastError();
+}
+
 // X + Y passes of square planes (fft_plane_kernel): vargs is a PlaneArgs<T>; P planes per CTA
 template <class S, typename T, int P, int MINB>
 cudaError_t launch_plane(const void* vargs, int sm_count, cudaStream_t st)
@@ -265,6 +283,11 @@ SizeEntry make_entry(int variant = 0)
         // budget, the real one with the real kernels' (shared-memory twiddles, MBI)
         e.launch[PK_LINE_CONV] = launch_line_conv<ZS, T, Z::C, Z::TW, Z::MB, Z::PP, false>;
         e.launch[PK_LINE_CONV_R2C] = launch_line_conv<ZS, T, Z::C, false, MBI, Z::PP, true>;
+        // the zero-padded 1-D convolution: the short path in PK_LINE_CONV's configuration, the long path's outer passes in the X
+        // configuration of PK_XF_TW and PK_XB
+        e.launch[PK_LINE_CONV_PAD] = launch_pad<ZS, T, Z::C, Z::TW, Z::MB, Z::PP, PK_LINE_CONV_PAD>;
+        e.launch[PK_XF_TW_PAD] = launch_pad<XS, T, X::C, X::TW, X::MB, X::PP, PK_XF_TW_PAD>;
+        e.launch[PK_XB_TW_PAD] = launch_pad<XS, T, X::C, X::TW, X::MB, X::PP, PK_XB_TW_PAD>;
         // X and Y passes of whole square planes in one kernel, where both roles share one schedule (and so one twiddle table).
         // Register budget: 64 per thread (2 CTAs of 512 / 4 of 256 threads), except 32-point fp64, which spills at 64 and is
         // given 85 (3 CTAs of 256); 64-point fp64 keeps 2 CTAs of 512 with a small spill (DESIGN.md section 3.8)

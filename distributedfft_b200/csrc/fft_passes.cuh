@@ -518,8 +518,17 @@ template <typename T> struct LineConvArgs {
     long long mult_line;   // multiplier elements between lines: 0 (one multiplier for every line) or N
 };
 
-template <class S, typename T, int C, bool TWREG, int MINB, bool PINGPONG>
-__global__ void __launch_bounds__(S::T* C, MINB) fft_line_conv_kernel(const LineConvArgs<T> R)
+// PadArgs: the padded kinds' arguments (the zero-padded convolve lines plan).  A line of the caller's `in` holds in_len points and
+// one of `out` out_len; the transform length n is longer, the missing input points are zero and the output points past out_len
+// are not stored.  LINE_CONV_PAD: the line strides are in_len / out_len (ia.cs, oa.cs); the four-step kinds: ia.SA / oa.SA
+template <typename T> struct PadArgs {
+    LineConvArgs<T> c;     // tile arguments, and the multiplier of LINE_CONV_PAD
+    long long in_len, out_len;
+};
+
+// PAD: point e of a line loads only where e < in_len and stores only where e < out_len (fft_line_conv_pad_kernel)
+template <class S, typename T, int C, bool TWREG, bool PINGPONG, bool PAD>
+__device__ __forceinline__ void line_conv_tiles(const LineConvArgs<T>& R, long long in_len, long long out_len)
 {
     static_assert(S::valid(), "bad schedule");
     using Op = TileOp<S, T, C, MAP_T, MAP_T, TWREG, false, false, PINGPONG>;
@@ -539,7 +548,7 @@ __global__ void __launch_bounds__(S::T* C, MINB) fft_line_conv_kernel(const Line
         const cx<T>* mp = R.mult + line * R.mult_line + t;
         cx<T> v[RR];
 #pragma unroll
-        for (int u = 0; u < RR; u++) v[u] = ok ? ld_stream(p + (long long)u * TT * A.ia.es) : mk<T>(0, 0);
+        for (int u = 0; u < RR; u++) v[u] = ok && (!PAD || t + u * TT < in_len) ? ld_stream(p + (long long)u * TT * A.ia.es) : mk<T>(0, 0);
         StageRunner<S, 0, T, C, MAP_T, MAP_T, TWREG, PINGPONG>::run(v, t, c, t, c, k.exch, k.pp, k.lut_s, twr, [] {});
         // multiply, then the inverse as swap -> forward -> swap (the swap-in is folded into the multiply's result)
 #pragma unroll
@@ -554,7 +563,80 @@ __global__ void __launch_bounds__(S::T* C, MINB) fft_line_conv_kernel(const Line
         if (ok) {
             cx<T>* q = A.out + tile * A.oa.SB + c * A.oa.cs + (long long)t * A.oa.es;
 #pragma unroll
-            for (int u = 0; u < RR; u++) st_stream(q + (long long)u * TT * A.oa.es, cswap(v[u]));
+            for (int u = 0; u < RR; u++)
+                if (!PAD || t + u * TT < out_len) st_stream(q + (long long)u * TT * A.oa.es, cswap(v[u]));
+        }
+    }
+}
+
+template <class S, typename T, int C, bool TWREG, int MINB, bool PINGPONG>
+__global__ void __launch_bounds__(S::T* C, MINB) fft_line_conv_kernel(const LineConvArgs<T> R)
+{
+    line_conv_tiles<S, T, C, TWREG, PINGPONG, false>(R, 0, 0);
+}
+
+// the short path of the zero-padded 1-D convolve lines plans: fft_line_conv_kernel over lines of in_len points in, out_len out
+template <class S, typename T, int C, bool TWREG, int MINB, bool PINGPONG>
+__global__ void __launch_bounds__(S::T* C, MINB) fft_line_conv_pad_kernel(const PadArgs<T> P)
+{
+    line_conv_tiles<S, T, C, TWREG, PINGPONG, true>(P.c, P.in_len, P.out_len);
+}
+
+// ------------------------------------------------------------------------------------------
+// The outer passes of the long path of the zero-padded 1-D convolve lines plans: the four-step transform n = n1 * n2 of a line,
+// with the multiply of the middle pass (PK_XCONV of n2) between them, and the padding folded into the loads and stores of the
+// caller's lines.  The X configuration of n1; tile `tile` = (line a, tile b of columns), columns b*C + c < W = n2.
+//   FWD (XF_TW_PAD): column j2 of the [n1][n2] view of input line a (ia.SA = in_len), point j1 at offset j1*n2 + j2, loaded only
+//                    where that offset is < in_len; FFT along n1; twiddle W_n^(j2*k1); transposed store to temp [j2][k1] (MAP_C ->
+//                    MAP_T, PK_XF_TW's addressing).
+//   !FWD (XB_TW_PAD): the inverse: row j2 of temp [n2][n1] (contiguous, MAP_T), twiddle prologue, FFT along n1, stored to output
+//                    line a (oa.SA = out_len) at j1*n2 + j2 where that offset is < out_len (MAP_C).  The inverse is swap -> forward
+//                    -> swap, and swap(v * conj(w)) = swap(v) * w, so the prologue multiplies the swapped values by the SAME
+//                    W_n^(j2*k1) that the forward pass's epilogue applies.
+// Unnormalised; DFFT_SCALE_BACKWARD is folded into the middle pass's multiply.  TileArgs::inv, do_scale are unused.
+// ------------------------------------------------------------------------------------------
+template <class S, typename T, int C, bool TWREG, int MINB, bool PINGPONG, bool FWD>
+__global__ void __launch_bounds__(S::T* C, MINB) fft_four_step_pad_kernel(const PadArgs<T> P)
+{
+    static_assert(S::valid(), "bad schedule");
+    static_assert(S::NSTAGES > 1, "a thread-map change needs an exchange");
+    constexpr int MI = FWD ? MAP_C : MAP_T, MO = FWD ? MAP_T : MAP_C;
+    using Op = TileOp<S, T, C, MI, MO, TWREG, false, false, PINGPONG>;
+    constexpr int RR = S::R, TT = S::T;
+    const TileArgs<T>& A = P.c.t;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    typename Op::Ctx k;
+    Op::setup(A, smem_raw, smem_raw + Op::SM::exch_bytes, k);
+    cx<T> twr[Op::NTW];
+    Op::load_twiddles(k, twr);
+    const int t_in = k.t_in, c_in = k.c_in, t_out = k.t_out, c_out = k.c_out;
+    for (long long tile = blockIdx.x; tile < A.ntiles; tile += gridDim.x) {
+        const long long a = tile / A.G;
+        const int b = (int)(tile - a * A.G);
+        const long long col_in = (long long)b * C + c_in, col_out = (long long)b * C + c_out;
+        const bool ok_in = col_in < A.W;
+        const long long lin = b * A.ia.SB + c_in * A.ia.cs + (long long)t_in * A.ia.es;   // offset inside the line
+        const cx<T>* p = A.in + a * A.ia.SA + lin;
+        cx<T> v[RR];
+#pragma unroll
+        for (int u = 0; u < RR; u++) {
+            const long long e = (long long)u * TT * A.ia.es;
+            v[u] = ok_in && (!FWD || lin + e < P.in_len) ? ld_stream(p + e) : mk<T>(0, 0);
+        }
+        if constexpr (!FWD) {
+#pragma unroll
+            for (int u = 0; u < RR; u++) v[u] = cmul(cswap(v[u]), unit_root<T>((col_in * (long long)(t_in + u * TT)) % A.tw_n, A.tw_n));
+        }
+        StageRunner<S, 0, T, C, MI, MO, TWREG, PINGPONG>::run(v, t_in, c_in, t_out, c_out, k.exch, k.pp, k.lut_s, twr, [] {});
+        if (col_out < A.W) {
+            const long long lout = b * A.oa.SB + c_out * A.oa.cs + (long long)t_out * A.oa.es;
+            cx<T>* q = A.out + a * A.oa.SA + lout;
+#pragma unroll
+            for (int u = 0; u < RR; u++) {
+                const long long e = (long long)u * TT * A.oa.es;
+                if constexpr (FWD) st_stream(q + e, cmul(v[u], unit_root<T>((col_out * (long long)(t_out + u * TT)) % A.tw_n, A.tw_n)));
+                else if (lout + e < P.out_len) st_stream(q + e, cswap(v[u]));
+            }
         }
     }
 }

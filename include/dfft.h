@@ -378,12 +378,30 @@ int dfft_lines_plan_create_convolve_r2c_2d(int nx, int ny, long long batch, int 
  * Lengths: n needs a tuned kernel of the default table (dfft_length_kind(n, precision) == 2); generic lengths, DFFT_GENERIC and
  * DFFT_VARIANT entries and lines longer than one shared-memory line are DFFT_EUNSUPPORTED, as is R2C with n < 2.  2^31 or more
  * lines are DFFT_EUNSUPPORTED.  Flags: DFFT_SCALE_BACKWARD folds 1/n into the multiply; any other bit is DFFT_EINVAL.  Executed
- * with dfft_lines_execute_convolve (batch = nlines), under the same rules as the 2-D and 3-D plans. */
+ * with dfft_lines_execute_convolve (batch = nlines), under the same rules as the 2-D and 3-D plans.  Longer lines, and linear
+ * (zero-padded) convolution, are dfft_lines_plan_create_convolve_padded_1d's. */
 int dfft_lines_plan_create_convolve_1d(int n, long long nlines, int precision, unsigned flags, dfft_lines_plan* plan);
 int dfft_lines_plan_create_convolve_r2c_1d(int n, long long nlines, int precision, unsigned flags, dfft_lines_plan* plan);
+/* Batched zero-padded 1-D spectral convolution on the lines engine (C2C): `in` holds nlines densely packed lines of in_len points
+ * (line l at l*in_len), `out` nlines lines of out_len points (line l at l*out_len), and per line
+ *   out[l] = (ifft(fft(zero_pad(in[l], n)) * m_l))[0:out_len],
+ * unnormalised (x n) unless DFFT_SCALE_BACKWARD.  With n >= in_len + K - 1 this is the linear convolution of a line with a filter of
+ * K points whose n-point spectrum is m; in_len = out_len = n is the circular convolution of dfft_lines_plan_create_convolve_1d.
+ * A shift of the output window is a phase ramp on m.  m is [n] complex in the plan's precision, natural order, per line or shared.
+ * Two paths, chosen from n:
+ *   n with a tuned kernel of the default table: one launch that reads in_len and writes out_len points per line; no temporary.
+ *   n = n1 * n2 (n1 <= 2 sqrt(n)) of tuned lengths of the default table: three launches of the four-step transform (the padding
+ *   folded into the first pass's loads and the last pass's stores, the multiply into the middle pass), with a temporary of
+ *   nlines * n complex elements owned by the plan.  Lines of up to 4096 * 4096 = 2^24 points, and short untuned lengths that split so.
+ * DFFT_EINVAL: in_len or out_len outside [1, n], n < 1, nlines < 0, a bad precision, any flag but DFFT_SCALE_BACKWARD, a null plan
+ * pointer.  DFFT_EUNSUPPORTED: 2^31 or more lines, a length that takes neither path, DFFT_GENERIC and DFFT_VARIANT entries.
+ * Executed with dfft_lines_execute_convolve (batch = nlines) under its rules; in == out is allowed only when in_len == out_len. */
+int dfft_lines_plan_create_convolve_padded_1d(int n, long long in_len, long long out_len, long long nlines, int precision,
+                                              unsigned flags, dfft_lines_plan* plan);
 /* mult_count = 1: one multiplier shared by every line / image / volume; = batch: one each, densely packed.  in == out (in place) or
  * disjoint buffers; `in` is never written when they are distinct, `mult` never.  DFFT_EINVAL: a null pointer, a buffer not
- * aligned to its element size (fp32 complex at an 8-byte offset is fine), a partial overlap of in and out, a multiplier that
+ * aligned to its element size (fp32 complex at an 8-byte offset is fine), a partial overlap of in and out (or in == out for a padded
+ * plan whose in_len and out_len differ), a multiplier that
  * overlaps out, another mult_count, and a plan that is not a convolve lines plan (dfft_lines_execute / dfft_lines_execute_real
  * on a convolve plan are DFFT_EINVAL too).  Asynchronous on the plan's stream (dfft_lines_synchronize waits). */
 int dfft_lines_execute_convolve(dfft_lines_plan plan, const void* in, void* out, const void* mult, long long mult_count);
@@ -399,6 +417,10 @@ long long dfft_debug_lines_conv_2d_ops(int nx, int ny, long long batch, int prec
  * "pair" as the real lines records) with C lines (line pairs) per tile, ntiles = G tiles, W = nlines, "mult" and "shared" */
 long long dfft_debug_lines_conv_1d_ops(int n, long long nlines, int precision, int real, unsigned flags, long long mult_count,
                                        char* buf, long long cap);
+/* the same for the zero-padded 1-D convolve lines plans: one "LINE_CONV_PAD" record (short path) or "XF_TW_PAD", "XCONV" and
+ * "XB_TW_PAD" (long path, temporary = buffer 4); the padded records carry "in_len" and "out_len" */
+long long dfft_debug_lines_conv_padded_1d_ops(int n, long long in_len, long long out_len, long long nlines, int precision,
+                                              unsigned flags, long long mult_count, char* buf, long long cap);
 /* one-shot convenience (plan + execute + synchronize + destroy), used by the per-axis parity tests */
 int dfft_fft_lines(void* data, int n, long long stride, long long nlines, long long inner, long long inner_dist,
                    long long outer_dist, int direction, int precision);
