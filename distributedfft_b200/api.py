@@ -137,6 +137,9 @@ def lib():
     L.dfft_lines_plan_create_convolve_padded_1d.argtypes = [i, ll, ll, ll, i, ctypes.c_uint, P(vp)]
     L.dfft_debug_lines_conv_padded_1d_ops.argtypes = [i, ll, ll, ll, i, ctypes.c_uint, ll, ctypes.c_char_p, ll]
     L.dfft_debug_lines_conv_padded_1d_ops.restype = ll
+    L.dfft_lines_plan_create_convolve_padded_r2c_1d.argtypes = [i, ll, ll, ll, i, ctypes.c_uint, P(vp)]
+    L.dfft_debug_lines_conv_padded_r2c_1d_ops.argtypes = [i, ll, ll, ll, i, ctypes.c_uint, ll, ctypes.c_char_p, ll]
+    L.dfft_debug_lines_conv_padded_r2c_1d_ops.restype = ll
     L.dfft_debug_real_lines_ops.argtypes = [i, i, ll, i, i, i, ctypes.c_char_p, ll]
     L.dfft_debug_real_lines_ops.restype = ll
     L.dfft_length_kind.argtypes = [i, i]
@@ -499,14 +502,21 @@ class LinesConvolvePlan(_LinesPlanBase):
     one kernel launch per execute.  Exactly one of one_d, two_d and three_d is given.
     `padded=(in_len, out_len)` with one_d (complex only): the zero-padded convolution out[l] = ifft(fft(in[l], n) * m)[:out_len]
     of a[nlines][in_len] into out[nlines][out_len] (dfft_lines_plan_create_convolve_padded_1d), which also takes lines longer
-    than one shared-memory line."""
+    than one shared-memory line.  `real_padded=(in_len, out_len)` with one_d instead: the same for real lines,
+    out[l] = irfft(rfft(in[l], n) * m, n)[:out_len] (m: [n//2+1] per line; dfft_lines_plan_create_convolve_padded_r2c_1d)."""
 
-    def __init__(self, three_d=None, precision=DOUBLE, real=False, flags=0, two_d=None, one_d=None, padded=None):
+    def __init__(self, three_d=None, precision=DOUBLE, real=False, flags=0, two_d=None, one_d=None, padded=None, real_padded=None):
         shapes = {"3d": three_d, "2d": two_d, "1d": one_d}
         given = [d for d, s in shapes.items() if s is not None]
         if len(given) != 1:
             raise ValueError("give exactly one of one_d, two_d and three_d")
         dims = given[0]
+        if real_padded is not None:
+            if dims != "1d" or real or padded is not None:
+                raise ValueError("real_padded=(in_len, out_len) is a one_d plan, given without real=True and padded")
+            n, nlines = one_d
+            self._create("dfft_lines_plan_create_convolve_padded_r2c_1d", n, real_padded[0], real_padded[1], nlines, precision, flags)
+            return
         if padded is not None:
             if dims != "1d" or real:
                 raise ValueError("padded=(in_len, out_len) is a complex one_d plan")
@@ -552,11 +562,12 @@ def lines_conv_1d_ops(n, nlines, precision=DOUBLE, real=False, flags=0, mult_cou
     return _json_hook(lib().dfft_debug_lines_conv_1d_ops, n, nlines, precision, int(bool(real)), flags, mult_count)
 
 
-def lines_conv_padded_1d_ops(n, in_len, out_len, nlines, precision=DOUBLE, flags=0, mult_count=1):
+def lines_conv_padded_1d_ops(n, in_len, out_len, nlines, precision=DOUBLE, flags=0, mult_count=1, real=False):
     """passes LinesConvolvePlan(one_d=(n, nlines), padded=(in_len, out_len), ...) would launch per execute (host-only test hook,
     see dfft_debug_lines_conv_padded_1d_ops; buffers as lines_conv_3d_ops, temporary = 4); read DFFT_GENERIC / DFFT_VARIANT at
-    the call, as plan creation does"""
-    return _json_hook(lib().dfft_debug_lines_conv_padded_1d_ops, n, in_len, out_len, nlines, precision, flags, mult_count)
+    the call, as plan creation does.  real=True: those of real_padded=(in_len, out_len) (dfft_debug_lines_conv_padded_r2c_1d_ops)"""
+    fn = lib().dfft_debug_lines_conv_padded_r2c_1d_ops if real else lib().dfft_debug_lines_conv_padded_1d_ops
+    return _json_hook(fn, n, in_len, out_len, nlines, precision, flags, mult_count)
 
 
 def real_lines_ops(n, nlines, direction, precision=DOUBLE, two_d=None):

@@ -496,7 +496,8 @@ static inline cudaError_t stream_wait(dfft_plan p, cudaStream_t st, cudaEvent_t 
 
 static const char* const kPassNames[PK_COUNT] = {"Z", "Y", "Y_CO", "Y_CI", "XF", "XB", "XB_CO", "XF_TW", "Z_R2C", "Z_C2R", "XCONV", "XCONV_CO",
                                                   "XY_PLANE", "XY_PLANE_CONV", "LINE_CONV", "LINE_CONV_R2C", "LINE_CONV_PAD",
-                                                  "XF_TW_PAD", "XB_TW_PAD"};
+                                                  "XF_TW_PAD", "XB_TW_PAD", "LINE_CONV_PAD_R2C", "XF_TW_PAD_R2C", "XCONV_R2C",
+                                                  "XB_TW_PAD_C2R"};
 
 // `extra`: further fields of the record, each starting with ", "
 template <typename T>
@@ -2389,6 +2390,7 @@ struct LinePass {
     int src = LB_IN, dst = LB_IN;   // LB_IN (the caller's data / a real or convolve plan's `in`), LB_TEMP (the plan's temporary), LB_OUT
     long long ld_in = 0, ld_out = 0;   // PK_Z_R2C / PK_Z_C2R / PK_LINE_CONV_R2C: distance between the two lines of a pair (RealZArgs), each side's elements
     long long in_len = 0, out_len = 0; // padded kinds (PadArgs): points of a line read from `in` / stored to `out`
+    long long lines = 0;         // real padded kinds (RealPadArgs): the caller's real lines
     bool inv = false;            // the inverse transform
 };
 // which execute runs a plan: dfft_lines_execute, dfft_lines_execute_real or dfft_lines_execute_convolve
@@ -2423,11 +2425,13 @@ static bool fits_int(long long a, long long b = 1, long long c = 1)
 
 // the plain pass kind whose tile size (kind_C) and twiddle schedule (upload_lut_kind) a lines pass has: the real kernels run the
 // contiguous configuration, the column convolve the strided one, the plane kernels the contiguous schedule, the line convolve
-// kernels the contiguous configuration and the padded four-step passes the X configuration of the passes they extend
+// kernels the contiguous configuration, the padded four-step passes the X configuration of the passes they extend and the real
+// column convolve the strided one
 static int plain_kind(int kind)
 {
-    if (kind == PK_XF_TW_PAD) return PK_XF_TW;
-    if (kind == PK_XB_TW_PAD) return PK_XB;
+    if (kind == PK_XF_TW_PAD || kind == PK_XF_TW_PAD_R2C) return PK_XF_TW;
+    if (kind == PK_XB_TW_PAD || kind == PK_XB_TW_PAD_C2R) return PK_XB;
+    if (kind == PK_XCONV_R2C) return PK_Y;
     return kind == PK_XCONV ? PK_Y : (kind == PK_Z_R2C || kind == PK_Z_C2R || kind >= PK_PLANE) ? PK_Z : kind;
 }
 
@@ -2771,64 +2775,84 @@ static int make_lines_conv_1d(dfft_lines_plan p, int n, long long nlines, bool r
 //          the element's own offset), XB_TW_PAD temp -> out (twiddle prologue, inverse FFT along n1, strided store).  A temporary
 //          of nlines * n elements; (in_len + 4n + out_len) elements per line and the multiplier.
 // in == out works when in_len == out_len: a short-path tile holds its lines in registers before it stores, and the long path
-// reads `in` only in its first pass
-static int make_lines_conv_padded_1d(dfft_lines_plan p, int n, long long in_len, long long out_len, long long nlines, unsigned flags)
+// reads `in` only in its first pass.
+// real: out[l] = irfft(rfft(zero_pad(in[l], n)) * m_l, n)[0:out_len] of real lines, two per complex transform (z = a + i b), with
+// the kinds' real twins on the same paths and splits:
+//   short: LINE_CONV_PAD_R2C, C line pairs per tile (the pair distances are in_len and out_len reals).
+//   long:  XF_TW_PAD_R2C, XCONV_R2C, XB_TW_PAD_C2R over ceil(nlines / 2) complex lines; the temporary holds each row's columns in
+//          mirror-adjacent order (mirror_pos) so that the middle pass finds Z[e] and Z[n - e] in one tile.  A temporary of
+//          ceil(nlines / 2) * n complex elements; (in_len + out_len) / 2 + 2n complex elements per line and the multiplier.
+static int make_lines_conv_padded_1d(dfft_lines_plan p, int n, long long in_len, long long out_len, long long nlines, bool real,
+                                     unsigned flags)
 {
     const int precision = p->prec;
     if (flags & ~DFFT_SCALE_BACKWARD) return fail(DFFT_EINVAL, "convolve lines plans take no flag but DFFT_SCALE_BACKWARD");
     if (n < 1 || nlines < 0 || bad_precision(precision)) return fail(DFFT_EINVAL, "bad arguments");
     if (in_len < 1 || in_len > n || out_len < 1 || out_len > n)
         return fail(DFFT_EINVAL, "in_len %lld and out_len %lld must lie in [1, n = %d]", in_len, out_len, n);
+    if (real && n < 2) return fail(DFFT_EUNSUPPORTED, "real lines of %d points: a real convolution needs at least 2", n);
     if (!fits_int(nlines)) return fail(DFFT_EUNSUPPORTED, "%lld lines: at most 2^31 - 1 per plan", nlines);
     const SizeEntry* e = find_size_entry(n, precision);
     LinePass* f = p->run[0];
+    const long long rows = real ? cdiv(nlines, 2) : nlines;   // complex lines transformed
     if (e && !e->gen) {   // a tuned length: a default entry has the padded line-convolve kernel, an alternate tuning does not
-        if (!e->launch[PK_LINE_CONV_PAD])
+        if (!e->launch[real ? PK_LINE_CONV_PAD_R2C : PK_LINE_CONV_PAD])
             return fail(DFFT_EUNSUPPORTED, "length %d has no padded line-convolution kernel (DFFT_VARIANT entries are not convolved)", n);
         const int C = e->z_C;
         LinePass& lp = f[0];
         lp.e = e;
-        lp.kind = PK_LINE_CONV_PAD;
+        lp.kind = real ? PK_LINE_CONV_PAD_R2C : PK_LINE_CONV_PAD;
         lp.src = LB_IN; lp.dst = LB_OUT;
-        lp.W = (int)nlines; lp.G = (int)cdiv(nlines, C); lp.ntiles = lp.G;
-        lp.ia = Affine{0, C * in_len, in_len, 1};
-        lp.oa = Affine{0, C * out_len, out_len, 1};
+        lp.W = (int)nlines; lp.G = (int)cdiv(rows, C); lp.ntiles = lp.G;
+        if (real) {   // tile, pair and point strides (reals)
+            lp.ia = Affine{0, 2 * C * in_len, 2 * in_len, 1};
+            lp.oa = Affine{0, 2 * C * out_len, 2 * out_len, 1};
+            lp.ld_in = in_len; lp.ld_out = out_len;
+        } else {
+            lp.ia = Affine{0, C * in_len, in_len, 1};
+            lp.oa = Affine{0, C * out_len, out_len, 1};
+        }
         p->nrun[0] = 1;
     } else {
-        const int n1 = four_step_split(n, precision, [](const SizeEntry* e1, const SizeEntry* e2) {
-            return !e1->gen && e1->launch[PK_XF_TW_PAD] && e1->launch[PK_XB_TW_PAD] && !e2->gen && e2->launch[PK_XCONV];
+        const int n1 = four_step_split(n, precision, [real](const SizeEntry* e1, const SizeEntry* e2) {
+            if (e1->gen || e2->gen) return false;
+            if (real) return e1->launch[PK_XF_TW_PAD_R2C] && e1->launch[PK_XB_TW_PAD_C2R] && e2->launch[PK_XCONV_R2C];
+            return e1->launch[PK_XF_TW_PAD] && e1->launch[PK_XB_TW_PAD] && e2->launch[PK_XCONV];
         });
         if (!n1)
             return fail(DFFT_EUNSUPPORTED, "length %d is neither a tuned length nor a product n1 * n2 of tuned lengths of the default kernel "
                         "table (n1 <= 2 sqrt(n)) with the kernels of the padded convolution", n);
         const int n2 = n / n1;
-        LinePass& a = f[0];   // columns j2 of the [n1][n2] view of each input line -> temp [j2][k1], twiddled
+        const long long pi = real ? 2 * in_len : in_len, po = real ? 2 * out_len : out_len;   // between the lines (pairs) of in / out
+        LinePass& a = f[0];   // columns j2 of the [n1][n2] view of each input line (pair) -> temp [j2][k1], twiddled
         a.e = find_size_entry(n1, precision);
         const int CA = a.e->x_C;
-        a.kind = PK_XF_TW_PAD; a.src = LB_IN; a.dst = LB_TEMP; a.tw_n = n;
-        a.G = (int)cdiv(n2, CA); a.W = n2; a.ntiles = nlines * a.G;
-        a.ia = Affine{in_len, CA, 1, n2};
+        a.kind = real ? PK_XF_TW_PAD_R2C : PK_XF_TW_PAD; a.src = LB_IN; a.dst = LB_TEMP; a.tw_n = n;
+        a.G = (int)cdiv(n2, CA); a.W = n2; a.ntiles = rows * a.G;
+        a.ia = Affine{pi, CA, 1, n2};
         a.oa = Affine{(long long)n, (long long)CA * n1, n1, 1};
         LinePass& b = f[1];   // columns k1 of temp [n2][n1]: forward along n2, multiply, inverse, in place
         b.e = find_size_entry(n2, precision);
         const int CB = b.e->s_C;
-        b.kind = PK_XCONV; b.src = b.dst = LB_TEMP;
-        b.G = (int)cdiv(n1, CB); b.W = n1; b.ntiles = nlines * b.G;
+        b.kind = real ? PK_XCONV_R2C : PK_XCONV; b.src = b.dst = LB_TEMP;
+        b.G = (int)cdiv(n1, CB); b.W = n1; b.ntiles = rows * b.G;
         b.ia = b.oa = Affine{(long long)n, CB, 1, n1};
-        LinePass& c = f[2];   // rows j2 of temp -> output line offsets j1*n2 + j2
+        LinePass& c = f[2];   // rows j2 of temp -> output line (pair) offsets j1*n2 + j2
         c.e = a.e;
-        c.kind = PK_XB_TW_PAD; c.src = LB_TEMP; c.dst = LB_OUT; c.tw_n = n; c.inv = true;
+        c.kind = real ? PK_XB_TW_PAD_C2R : PK_XB_TW_PAD; c.src = LB_TEMP; c.dst = LB_OUT; c.tw_n = n; c.inv = true;
         c.G = a.G; c.W = n2; c.ntiles = a.ntiles;
         c.ia = Affine{(long long)n, (long long)CA * n1, n1, 1};
-        c.oa = Affine{out_len, CA, 1, n2};
+        c.oa = Affine{po, CA, 1, n2};
+        if (real) { a.ld_in = in_len; c.ld_out = out_len; }
         p->nrun[0] = 3;
-        p->temp_bytes = (size_t)nlines * n * (precision == DFFT_FLOAT ? 8 : 16);
+        p->temp_bytes = (size_t)rows * n * (precision == DFFT_FLOAT ? 8 : 16);
     }
-    for (int k = 0; k < p->nrun[0]; k++) { f[k].in_len = in_len; f[k].out_len = out_len; }
+    for (int k = 0; k < p->nrun[0]; k++) { f[k].in_len = in_len; f[k].out_len = out_len; f[k].lines = nlines; }
     p->nrun[1] = 0;
     p->form = LF_CONV;
+    p->real = real;
     p->batch = nlines;
-    p->mvol = n;
+    p->mvol = real ? n / 2 + 1 : n;
     p->in_count = nlines * in_len;
     p->out_count = nlines * out_len;
     p->scale = (flags & DFFT_SCALE_BACKWARD) ? 1.0 / (double)n : 0.0;
@@ -2947,7 +2971,13 @@ extern "C" int dfft_lines_plan_create_convolve_r2c_1d(int n, long long nlines, i
 extern "C" int dfft_lines_plan_create_convolve_padded_1d(int n, long long in_len, long long out_len, long long nlines, int precision,
                                                          unsigned flags, dfft_lines_plan* plan)
 {
-    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv_padded_1d(p, n, in_len, out_len, nlines, flags); });
+    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv_padded_1d(p, n, in_len, out_len, nlines, false, flags); });
+}
+
+extern "C" int dfft_lines_plan_create_convolve_padded_r2c_1d(int n, long long in_len, long long out_len, long long nlines, int precision,
+                                                             unsigned flags, dfft_lines_plan* plan)
+{
+    return lines_create(plan, precision, [&](dfft_lines_plan p) { return make_lines_conv_padded_1d(p, n, in_len, out_len, nlines, true, flags); });
 }
 
 extern "C" int dfft_lines_plan_create_convolve_2d(int nx, int ny, long long batch, int precision, unsigned flags, dfft_lines_plan* plan)
@@ -2974,9 +3004,10 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
     const void* src = line_buf(lp.src, in, out, p->temp);
     void* dst = line_buf(lp.dst, in, out, p->temp);
     const bool conv = lp.kind == PK_XCONV || lp.kind == PK_PLANE_CONV || lp.kind == PK_LINE_CONV || lp.kind == PK_LINE_CONV_R2C ||
-                      lp.kind == PK_LINE_CONV_PAD;
+                      lp.kind == PK_LINE_CONV_PAD || lp.kind == PK_LINE_CONV_PAD_R2C || lp.kind == PK_XCONV_R2C;
     const bool realk = lp.kind == PK_Z_R2C || lp.kind == PK_Z_C2R || lp.kind == PK_LINE_CONV_R2C;
-    const bool pad = lp.kind == PK_LINE_CONV_PAD || lp.kind == PK_XF_TW_PAD || lp.kind == PK_XB_TW_PAD;
+    const bool real_pad = lp.kind == PK_LINE_CONV_PAD_R2C || lp.kind == PK_XF_TW_PAD_R2C || lp.kind == PK_XCONV_R2C || lp.kind == PK_XB_TW_PAD_C2R;
+    const bool pad = lp.kind == PK_LINE_CONV_PAD || lp.kind == PK_XF_TW_PAD || lp.kind == PK_XB_TW_PAD || real_pad;
     ConvArgs<T> c{};
     TileArgs<T>& a = c.t;
     a.in = (const cx<T>*)src; a.out = (cx<T>*)dst; a.lut = (const cx<T>*)lp.lut;
@@ -2987,14 +3018,19 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
         c.mult = (const cx<T>*)mult; c.mult_shared = shared ? 1 : 0;
     }
     if (ops) {
-        char extra[192] = "";
+        char extra[256] = "";
         int len = 0;
         if (realk) len = snprintf(extra, sizeof(extra), ", \"nzh\": %d, \"pair\": [%lld, %lld]", lp.e->N / 2 + 1, lp.ld_in, lp.ld_out);
         if (pad) len = snprintf(extra, sizeof(extra), ", \"in_len\": %lld, \"out_len\": %lld", lp.in_len, lp.out_len);
+        if (real_pad) {
+            len += snprintf(extra + len, sizeof(extra) - len, ", \"lines\": %lld", lp.lines);
+            if (lp.kind != PK_XCONV_R2C) len += snprintf(extra + len, sizeof(extra) - len, ", \"pair\": [%lld, %lld]", lp.ld_in, lp.ld_out);
+            if (conv) len += snprintf(extra + len, sizeof(extra) - len, ", \"nzh\": %lld", (long long)lp.e->N * (lp.kind == PK_XCONV_R2C ? lp.W : 1) / 2 + 1);
+        }
         if (conv) snprintf(extra + len, sizeof(extra) - len, ", \"mult\": %llu, \"shared\": %d", (unsigned long long)(size_t)mult, shared ? 1 : 0);
         const bool plane = lp.kind == PK_PLANE || lp.kind == PK_PLANE_CONV;
         record_op<T>(*ops, kPassNames[lp.kind], phase, lp.e->N, plane ? lp.e->N : kind_C(lp.e, plain_kind(lp.kind)), false, false,
-                     lp.kind == PK_XF_TW || lp.kind == PK_XF_TW_PAD, a,
+                     lp.kind == PK_XF_TW || lp.kind == PK_XF_TW_PAD || lp.kind == PK_XF_TW_PAD_R2C, a,
                      extra);
         return cudaSuccess;
     }
@@ -3003,6 +3039,7 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
     RealLineConvArgs<T> rl{};   // PK_Z_R2C / PK_Z_C2R: rl.r
     LineConvArgs<T> lc{};
     PadArgs<T> pa{};
+    RealPadArgs<T> ra{};
     const void* args = conv ? (const void*)&c : (const void*)&a;
     switch (lp.kind) {
     case PK_PLANE:
@@ -3029,6 +3066,12 @@ static cudaError_t line_pass(const dfft_lines_plan_s* p, const LinePass& lp, int
         pa = {{a, c.mult, shared ? 0 : (long long)lp.e->N}, lp.in_len, lp.out_len};
         args = &pa;
         break;
+    case PK_LINE_CONV_PAD_R2C: case PK_XF_TW_PAD_R2C: case PK_XCONV_R2C: case PK_XB_TW_PAD_C2R: {
+        const long long nzh = (long long)lp.e->N * (lp.kind == PK_XCONV_R2C ? lp.W : 1) / 2 + 1;   // the multiplier's points per line
+        ra = {{{a, (const T*)src, (T*)dst, lp.ld_in, lp.ld_out}, c.mult, shared ? 0 : nzh}, lp.in_len, lp.out_len, lp.lines};
+        args = &ra;
+        break;
+    }
     }
     return lp.e->launch[lp.kind](args, p->sms, p->stream);
 }
@@ -3189,7 +3232,21 @@ extern "C" long long dfft_debug_lines_conv_padded_1d_ops(int n, long long in_len
                                                          unsigned flags, long long mult_count, char* buf, long long cap)
 {
     auto build = [&](dfft_lines_plan p) {
-        const int rc = make_lines_conv_padded_1d(p, n, in_len, out_len, nlines, flags);
+        const int rc = make_lines_conv_padded_1d(p, n, in_len, out_len, nlines, false, flags);
+        return rc || mult_count == 1 || mult_count == nlines ? rc : fail(DFFT_EINVAL, "mult_count must be 1 or the plan's line count");
+    };
+    return lines_ops_json(precision, build, 0, 5, 2, mult_count == 1, buf, cap);
+}
+
+/* test hook (host only): the passes of a real zero-padded 1-D convolve lines plan, JSON as dfft_debug_lines_conv_padded_1d_ops.
+ * Short path: one "LINE_CONV_PAD_R2C" record; long path: "XF_TW_PAD_R2C", "XCONV_R2C", "XB_TW_PAD_C2R".  Every record carries
+ * "in_len", "out_len" and "lines" (real lines); those that touch the real lines "pair" (the distance between a pair's two lines on
+ * the input and output side, 0 on a complex side); LINE_CONV_PAD_R2C and XCONV_R2C "mult", "shared" and "nzh" (n/2 + 1) */
+extern "C" long long dfft_debug_lines_conv_padded_r2c_1d_ops(int n, long long in_len, long long out_len, long long nlines, int precision,
+                                                             unsigned flags, long long mult_count, char* buf, long long cap)
+{
+    auto build = [&](dfft_lines_plan p) {
+        const int rc = make_lines_conv_padded_1d(p, n, in_len, out_len, nlines, true, flags);
         return rc || mult_count == 1 || mult_count == nlines ? rc : fail(DFFT_EINVAL, "mult_count must be 1 or the plan's line count");
     };
     return lines_ops_json(precision, build, 0, 5, 2, mult_count == 1, buf, cap);

@@ -36,6 +36,11 @@ enum PassKind {
     PK_LINE_CONV_PAD,  // PK_LINE_CONV over lines of in_len points in and out_len out (fft_line_conv_pad_kernel), contiguous configuration
     PK_XF_TW_PAD,      // PK_XF_TW reading input lines of in_len points (fft_four_step_pad_kernel), X configuration
     PK_XB_TW_PAD,      // its inverse: contiguous load, twiddle prologue, strided store to output lines of out_len points, X configuration
+    // the real zero-padded 1-D convolve lines plans (args = RealPadArgs): two real lines per complex transform; default entries only
+    PK_LINE_CONV_PAD_R2C,  // PK_LINE_CONV_R2C over lines of in_len points in and out_len out (fft_line_conv_pad_r2c_kernel)
+    PK_XF_TW_PAD_R2C,      // PK_XF_TW_PAD over line pairs, columns stored at mirror_pos (fft_four_step_pad_kernel, REAL), X configuration
+    PK_XCONV_R2C,          // PK_XCONV with the pair untangled around the multiply (fft_conv_r2c_kernel), strided configuration
+    PK_XB_TW_PAD_C2R,      // PK_XB_TW_PAD loading at mirror_pos, storing Re / Im to the two lines (fft_four_step_pad_kernel, REAL)
     PK_COUNT
 };
 

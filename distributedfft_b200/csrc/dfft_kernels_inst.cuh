@@ -106,6 +106,25 @@ cudaError_t launch_pad(const void* vargs, int sm_count, cudaStream_t st)
     return cudaGetLastError();
 }
 
+// the real zero-padded 1-D convolve lines plans' kinds: vargs is a RealPadArgs<T>; PK_LINE_CONV_PAD_R2C runs
+// fft_line_conv_pad_r2c_kernel, PK_XF_TW_PAD_R2C / PK_XB_TW_PAD_C2R the real fft_four_step_pad_kernel, PK_XCONV_R2C fft_conv_r2c_kernel
+template <class S, typename T, int C, bool TW, int MINB, bool PP, int KIND>
+cudaError_t launch_real_pad(const void* vargs, int sm_count, cudaStream_t st)
+{
+    const RealPadArgs<T>& a = *reinterpret_cast<const RealPadArgs<T>*>(vargs);
+    constexpr auto kern = [] {   // only the kernel of this kind is instantiated
+        if constexpr (KIND == PK_LINE_CONV_PAD_R2C) return fft_line_conv_pad_r2c_kernel<S, T, C, TW, MINB, PP>;
+        else if constexpr (KIND == PK_XCONV_R2C) return fft_conv_r2c_kernel<S, T, C, TW, MINB, PP>;
+        else return fft_four_step_pad_kernel<S, T, C, TW, MINB, PP, KIND == PK_XF_TW_PAD_R2C, true>;
+    }();
+    constexpr size_t smem = TileSmem<S, T, C, PP>::bytes(false);
+    long long grid = 0;
+    const cudaError_t e = resident_grid<kern>(S::T * C, smem, 0, a.c.r.t.ntiles, sm_count, grid);
+    if (e != cudaSuccess || grid == 0) return e;
+    kern<<<(unsigned)grid, S::T * C, smem, st>>>(a);
+    return cudaGetLastError();
+}
+
 // X + Y passes of square planes (fft_plane_kernel): vargs is a PlaneArgs<T>; P planes per CTA
 template <class S, typename T, int P, int MINB>
 cudaError_t launch_plane(const void* vargs, int sm_count, cudaStream_t st)
@@ -288,6 +307,12 @@ SizeEntry make_entry(int variant = 0)
         e.launch[PK_LINE_CONV_PAD] = launch_pad<ZS, T, Z::C, Z::TW, Z::MB, Z::PP, PK_LINE_CONV_PAD>;
         e.launch[PK_XF_TW_PAD] = launch_pad<XS, T, X::C, X::TW, X::MB, X::PP, PK_XF_TW_PAD>;
         e.launch[PK_XB_TW_PAD] = launch_pad<XS, T, X::C, X::TW, X::MB, X::PP, PK_XB_TW_PAD>;
+        // the real zero-padded 1-D convolution: the short path in PK_LINE_CONV_R2C's configuration, the long path's outer passes in
+        // the X configuration, its middle pass in PK_XCONV's
+        e.launch[PK_LINE_CONV_PAD_R2C] = launch_real_pad<ZS, T, Z::C, false, MBI, Z::PP, PK_LINE_CONV_PAD_R2C>;
+        e.launch[PK_XF_TW_PAD_R2C] = launch_real_pad<XS, T, X::C, X::TW, X::MB, X::PP, PK_XF_TW_PAD_R2C>;
+        e.launch[PK_XCONV_R2C] = launch_real_pad<SS, T, Y::C, Y::TW, Y::MB, Y::PP, PK_XCONV_R2C>;
+        e.launch[PK_XB_TW_PAD_C2R] = launch_real_pad<XS, T, X::C, X::TW, X::MB, X::PP, PK_XB_TW_PAD_C2R>;
         // X and Y passes of whole square planes in one kernel, where both roles share one schedule (and so one twiddle table).
         // Register budget: 64 per thread (2 CTAs of 512 / 4 of 256 threads), except 32-point fp64, which spills at 64 and is
         // given 85 (3 CTAs of 256); 64-point fp64 keeps 2 CTAs of 512 with a small spill (DESIGN.md section 3.8)

@@ -12,6 +12,7 @@
 // the local send buffer chunk or -- fused all-to-all -- the peer's receive buffer mapped over
 // NVLink (fft_mpi_3d_api.cpp:613-630 hipMemcpyPeerAsync into nodeDataDev[i]).
 #pragma once
+#include <type_traits>
 #include "fft_core.cuh"
 
 namespace dfft {
@@ -594,16 +595,32 @@ __global__ void __launch_bounds__(S::T* C, MINB) fft_line_conv_pad_kernel(const 
 //                    -> swap, and swap(v * conj(w)) = swap(v) * w, so the prologue multiplies the swapped values by the SAME
 //                    W_n^(j2*k1) that the forward pass's epilogue applies.
 // Unnormalised; DFFT_SCALE_BACKWARD is folded into the middle pass's multiply.  TileArgs::inv, do_scale are unused.
+// REAL (the real plan's XF_TW_PAD_R2C / XB_TW_PAD_C2R, args = RealPadArgs, fft_real.cuh): line `a` of the temporary is real lines
+// 2a and 2a+1 of the caller's (ia.SA / oa.SA = 2 in_len / 2 out_len reals, the second line ld_in / ld_out further) as z = x + i y:
+// FWD loads the pair's points into z, !FWD stores Re z to line 2a and Im z to line 2a+1.  A missing second line reads 0 and is not
+// stored.  On the temporary's side column k1 of a row sits at mirror_pos<n1>(k1), not at k1.
 // ------------------------------------------------------------------------------------------
-template <class S, typename T, int C, bool TWREG, int MINB, bool PINGPONG, bool FWD>
-__global__ void __launch_bounds__(S::T* C, MINB) fft_four_step_pad_kernel(const PadArgs<T> P)
+template <typename T> struct RealPadArgs;
+
+// Position of column k1 inside a row of the real plan's temporary ([n2][n1] per line pair): mirror columns k1 and n1 - k1 are
+// adjacent, at 2q and 2q + 1, so every aligned position pair holds a mirror pair or self-mirrored columns.
+//   n1 even: 0 -> 0, n1/2 -> 1, q -> 2q, n1 - q -> 2q + 1 (1 <= q < n1/2)
+//   n1 odd:  q -> 2q - 2, n1 - q -> 2q - 1 (1 <= q <= (n1-1)/2), 0 -> n1 - 1
+template <int N1> __device__ __forceinline__ int mirror_pos(int k1)
+{
+    if constexpr (N1 % 2 == 0) return k1 == 0 ? 0 : (2 * k1 == N1 ? 1 : (2 * k1 < N1 ? 2 * k1 : 2 * (N1 - k1) + 1));
+    else return k1 == 0 ? N1 - 1 : (2 * k1 < N1 ? 2 * k1 - 2 : 2 * (N1 - k1) - 1);
+}
+
+template <class S, typename T, int C, bool TWREG, int MINB, bool PINGPONG, bool FWD, bool REAL = false>
+__global__ void __launch_bounds__(S::T* C, MINB) fft_four_step_pad_kernel(const std::conditional_t<REAL, RealPadArgs<T>, PadArgs<T>> P)
 {
     static_assert(S::valid(), "bad schedule");
     static_assert(S::NSTAGES > 1, "a thread-map change needs an exchange");
     constexpr int MI = FWD ? MAP_C : MAP_T, MO = FWD ? MAP_T : MAP_C;
     using Op = TileOp<S, T, C, MI, MO, TWREG, false, false, PINGPONG>;
     constexpr int RR = S::R, TT = S::T;
-    const TileArgs<T>& A = P.c.t;
+    const TileArgs<T>& A = [&]() -> const TileArgs<T>& { if constexpr (REAL) return P.c.r.t; else return P.c.t; }();
     extern __shared__ __align__(16) unsigned char smem_raw[];
     typename Op::Ctx k;
     Op::setup(A, smem_raw, smem_raw + Op::SM::exch_bytes, k);
@@ -616,12 +633,27 @@ __global__ void __launch_bounds__(S::T* C, MINB) fft_four_step_pad_kernel(const 
         const long long col_in = (long long)b * C + c_in, col_out = (long long)b * C + c_out;
         const bool ok_in = col_in < A.W;
         const long long lin = b * A.ia.SB + c_in * A.ia.cs + (long long)t_in * A.ia.es;   // offset inside the line
-        const cx<T>* p = A.in + a * A.ia.SA + lin;
         cx<T> v[RR];
+        if constexpr (REAL && FWD) {   // real lines 2a and 2a + 1 as z = x + i y
+            const bool okb = 2 * a + 1 < P.lines;
+            const T* p = P.c.r.rin + a * A.ia.SA + lin;
 #pragma unroll
-        for (int u = 0; u < RR; u++) {
-            const long long e = (long long)u * TT * A.ia.es;
-            v[u] = ok_in && (!FWD || lin + e < P.in_len) ? ld_stream(p + e) : mk<T>(0, 0);
+            for (int u = 0; u < RR; u++) {
+                const long long e = (long long)u * TT * A.ia.es;
+                const bool in = ok_in && lin + e < P.in_len;
+                v[u] = mk<T>(in ? ld_stream(p + e) : (T)0, in && okb ? ld_stream(p + P.c.r.ld_in + e) : (T)0);
+            }
+        } else if constexpr (REAL) {   // row col_in of the temporary, its columns at mirror_pos
+            const cx<T>* p = A.in + a * A.ia.SA + b * A.ia.SB + c_in * A.ia.cs;
+#pragma unroll
+            for (int u = 0; u < RR; u++) v[u] = ok_in ? ld_stream(p + mirror_pos<S::N>(t_in + u * TT)) : mk<T>(0, 0);
+        } else {
+            const cx<T>* p = A.in + a * A.ia.SA + lin;
+#pragma unroll
+            for (int u = 0; u < RR; u++) {
+                const long long e = (long long)u * TT * A.ia.es;
+                v[u] = ok_in && (!FWD || lin + e < P.in_len) ? ld_stream(p + e) : mk<T>(0, 0);
+            }
         }
         if constexpr (!FWD) {
 #pragma unroll
@@ -630,12 +662,30 @@ __global__ void __launch_bounds__(S::T* C, MINB) fft_four_step_pad_kernel(const 
         StageRunner<S, 0, T, C, MI, MO, TWREG, PINGPONG>::run(v, t_in, c_in, t_out, c_out, k.exch, k.pp, k.lut_s, twr, [] {});
         if (col_out < A.W) {
             const long long lout = b * A.oa.SB + c_out * A.oa.cs + (long long)t_out * A.oa.es;
-            cx<T>* q = A.out + a * A.oa.SA + lout;
+            if constexpr (REAL && FWD) {
+                cx<T>* q = A.out + a * A.oa.SA + b * A.oa.SB + c_out * A.oa.cs;
 #pragma unroll
-            for (int u = 0; u < RR; u++) {
-                const long long e = (long long)u * TT * A.oa.es;
-                if constexpr (FWD) st_stream(q + e, cmul(v[u], unit_root<T>((col_out * (long long)(t_out + u * TT)) % A.tw_n, A.tw_n)));
-                else if (lout + e < P.out_len) st_stream(q + e, cswap(v[u]));
+                for (int u = 0; u < RR; u++)
+                    st_stream(q + mirror_pos<S::N>(t_out + u * TT), cmul(v[u], unit_root<T>((col_out * (long long)(t_out + u * TT)) % A.tw_n, A.tw_n)));
+            } else if constexpr (REAL) {   // swapped back: Re z = v.y to line 2a, Im z = v.x to line 2a + 1
+                const bool okb = 2 * a + 1 < P.lines;
+                T* q = P.c.r.rout + a * A.oa.SA + lout;
+#pragma unroll
+                for (int u = 0; u < RR; u++) {
+                    const long long e = (long long)u * TT * A.oa.es;
+                    if (lout + e < P.out_len) {
+                        st_stream(q + e, v[u].y);
+                        if (okb) st_stream(q + P.c.r.ld_out + e, v[u].x);
+                    }
+                }
+            } else {
+                cx<T>* q = A.out + a * A.oa.SA + lout;
+#pragma unroll
+                for (int u = 0; u < RR; u++) {
+                    const long long e = (long long)u * TT * A.oa.es;
+                    if constexpr (FWD) st_stream(q + e, cmul(v[u], unit_root<T>((col_out * (long long)(t_out + u * TT)) % A.tw_n, A.tw_n)));
+                    else if (lout + e < P.out_len) st_stream(q + e, cswap(v[u]));
+                }
             }
         }
     }

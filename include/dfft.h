@@ -398,6 +398,19 @@ int dfft_lines_plan_create_convolve_r2c_1d(int n, long long nlines, int precisio
  * Executed with dfft_lines_execute_convolve (batch = nlines) under its rules; in == out is allowed only when in_len == out_len. */
 int dfft_lines_plan_create_convolve_padded_1d(int n, long long in_len, long long out_len, long long nlines, int precision,
                                               unsigned flags, dfft_lines_plan* plan);
+/* The same for real lines (R2C): `in` holds nlines densely packed real lines of in_len points, `out` nlines real lines of out_len
+ * points, and per line
+ *   out[l] = irfft(rfft(zero_pad(in[l], n)) * m_l, n)[0:out_len],
+ * unnormalised (x n) unless DFFT_SCALE_BACKWARD.  m is [n/2 + 1] complex in the plan's precision, per line or shared; the
+ * imaginary parts of m[0] and (even n) m[n/2] are ignored, as numpy's irfft ignores them.  Two real lines go through one complex
+ * transform.  The same two paths and splits as the complex plan:
+ *   n with a tuned kernel of the default table: one launch; no temporary.
+ *   n = n1 * n2: three launches of the four-step transform over ceil(nlines / 2) complex lines, with a temporary of
+ *   ceil(nlines / 2) * n complex elements owned by the plan; the middle pass finds each bin k and its mirror n - k in one tile.
+ * DFFT_EINVAL as the complex plan.  DFFT_EUNSUPPORTED: n < 2, and as the complex plan.  Executed with dfft_lines_execute_convolve
+ * (batch = nlines, real elements) under its rules; in == out is allowed only when in_len == out_len. */
+int dfft_lines_plan_create_convolve_padded_r2c_1d(int n, long long in_len, long long out_len, long long nlines, int precision,
+                                                  unsigned flags, dfft_lines_plan* plan);
 /* mult_count = 1: one multiplier shared by every line / image / volume; = batch: one each, densely packed.  in == out (in place) or
  * disjoint buffers; `in` is never written when they are distinct, `mult` never.  DFFT_EINVAL: a null pointer, a buffer not
  * aligned to its element size (fp32 complex at an 8-byte offset is fine), a partial overlap of in and out (or in == out for a padded
@@ -421,6 +434,12 @@ long long dfft_debug_lines_conv_1d_ops(int n, long long nlines, int precision, i
  * "XB_TW_PAD" (long path, temporary = buffer 4); the padded records carry "in_len" and "out_len" */
 long long dfft_debug_lines_conv_padded_1d_ops(int n, long long in_len, long long out_len, long long nlines, int precision,
                                               unsigned flags, long long mult_count, char* buf, long long cap);
+/* the same for the real zero-padded 1-D convolve lines plans: one "LINE_CONV_PAD_R2C" record (short path, C line pairs per tile)
+ * or "XF_TW_PAD_R2C", "XCONV_R2C" and "XB_TW_PAD_C2R" (long path, temporary = buffer 4).  Every record carries "in_len", "out_len"
+ * and "lines" (real lines); those that touch the real lines "pair" (the distance between a pair's two lines on the input / output
+ * side, 0 on a complex side); LINE_CONV_PAD_R2C and XCONV_R2C "mult", "shared" and "nzh" (n/2 + 1) */
+long long dfft_debug_lines_conv_padded_r2c_1d_ops(int n, long long in_len, long long out_len, long long nlines, int precision,
+                                                  unsigned flags, long long mult_count, char* buf, long long cap);
 /* one-shot convenience (plan + execute + synchronize + destroy), used by the per-axis parity tests */
 int dfft_fft_lines(void* data, int n, long long stride, long long nlines, long long inner, long long inner_dist,
                    long long outer_dist, int direction, int precision);
